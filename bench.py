@@ -5,7 +5,7 @@ Headline workload (BASELINE.json configs[1], SURVEY.md 8d config 2): batched syn
 4096 concurrent channels x 256 aligned symbols per channel = 1 048 576 symbols = 8 GiB of cf32 per GPU per step,
 symbol values ~ U[0,128), AWGN +10 dB, generated on the device by the library's own transmitter kernels
 (lora_b200_tx_symbols_dev / lora_b200_tx_expand_dev).  A "step" = one pass of K1 over the whole batch.  The
-input (8 GiB) is far larger than the 126 MB L2, so no L2 flush is needed between timed iterations.
+input (8 GiB) is far larger than the H100's 50 MB L2, so no L2 flush is needed between timed iterations.
 
 One JSON line:
   value         whole-job symbols/s, batch resident in HBM, CUDA events on the launch stream, max over ranks
@@ -66,6 +66,8 @@ def parse_args():
     ap.add_argument("--no-config4", action="store_true")
     ap.add_argument("--no-cpu", action="store_true")
     ap.add_argument("--cpu-seconds", type=float, default=12.0)
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write the last step's bins and magnitudes as DIR/<name>.npy")
     return ap.parse_args()
 
 
@@ -80,7 +82,7 @@ def measured_peak_gbs():
             return float(json.loads(p.read_text())["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs, burst copy)"
         except Exception:
             pass
-    return 6650.0, "fallback (B200_PROFILING.md)"
+    return 3350.0, "H100 SXM data sheet HBM3 bandwidth (not measured)"
 
 
 def config_dict(args):
@@ -90,7 +92,7 @@ def config_dict(args):
                          f"{args.symbols_per_channel} symbols per GPU (BASELINE.json configs[1])"),
             "sf": args.sf, "channels_per_gpu": args.channels, "symbols_per_channel": args.symbols_per_channel,
             "snr_db": args.snr_db, "batch_bytes_per_gpu": int(args.channels * args.symbols_per_channel * sps * 8),
-            "l2": "inputs (8 GiB) larger than L2, no flush needed", "parallelism": f"streams sharded x{args.gpus}"}
+            "l2": "inputs (8 GiB) larger than the 50 MB L2, no flush needed", "parallelism": f"streams sharded x{args.gpus}"}
 
 
 # ---------------------------------------------------------------------------------------------------------------------
@@ -375,7 +377,7 @@ def check_frames(fr, pays_per_stream, k, n_streams):
     return expected, ok
 
 
-K1_KERNEL = {7: "k1_sf7_warp_kernel<12,2>", 8: "k1_group_kernel<8,6,2>", 9: "k1_group_kernel<9,3,2>", 10: "k1_sf10_kernel<3>",
+K1_KERNEL = {7: "k1_sf7_warp_kernel<12,2>", 8: "k1_group_kernel<8,6,2>", 9: "k1_group_kernel<9,3,2>", 10: "k1_sf10_kernel<2>",
              11: "k1_rows_kernel<11>", 12: "k1_rows_kernel<12>"}
 
 
@@ -503,6 +505,8 @@ def main():
     if world > 1:
         dist.barrier()
     launches = dec.launch_count() - l0
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, bins, mags)
     ms = e0.elapsed_time(e1)
     ms_max = all_max(ms)
     clocks = sampler.stop(t0, t1) if rank == 0 else None
@@ -613,6 +617,21 @@ def main():
         print(json.dumps(out))
     if world > 1:
         dist.destroy_process_group()
+
+
+def dump_outputs(out_dir, bins, mags):
+    """What the timed K1 path returned in its last step: the bin (exact in float64) and the magnitude of every symbol
+    (1 Mi symbols at the default size: 12 MiB).  Above 64 MiB in all, a fixed seeded sample of the symbols is written,
+    with the symbol indices in sample_index.npy."""
+    d = Path(out_dir)
+    d.mkdir(parents=True, exist_ok=True)
+    b, m = bins.cpu().numpy().astype(np.float64), mags.cpu().numpy().astype(np.float32)
+    if b.size * 12 > (64 << 20):
+        idx = np.sort(np.random.default_rng(0).choice(b.size, (64 << 20) // 20, replace=False))
+        np.save(d / "sample_index.npy", idx.astype(np.float64))
+        b, m = b[idx], m[idx]
+    np.save(d / "bins.npy", b)
+    np.save(d / "mags.npy", m)
 
 
 def run_e2e(args, torch, dist, G, device, local, world, rank, dec, iq, bins_ref, n_sym_total, sps, all_max, all_min_int, all_sum):

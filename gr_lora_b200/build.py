@@ -1,4 +1,4 @@
-"""Build liblora_b200.so (the CUDA library + C ABI) in-tree with nvcc for sm_100a.
+"""Build liblora_b200.so (the CUDA library + C ABI) in-tree with nvcc for sm_90a (H100).
 
 The built .so sits next to this file so that it travels with the repository snapshot to the
 GPU box (the JIT cache under ~/.cache would not)."""
@@ -15,7 +15,7 @@ CSRC = PKG / "csrc"
 LIB = PKG / "liblora_b200.so"
 HOST_EMUL = ROOT / "build" / "host_emul.so"
 
-NVCC_FLAGS = ["-O3", "-std=c++17", "-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo",
+NVCC_FLAGS = ["-O3", "-std=c++17", "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo",
               "-Xcompiler", "-fPIC", "-shared", "--use_fast_math=false"]
 
 
@@ -62,7 +62,7 @@ def build(force: bool = False, verbose: bool = False) -> Path:
 
     with ThreadPoolExecutor(len(TRANSLATION_UNITS)) as ex:
         objs = list(ex.map(compile_one, TRANSLATION_UNITS))
-    cmd = [_nvcc(), "-shared", "-gencode", "arch=compute_100a,code=sm_100a", "-o", str(LIB), *map(str, objs)]
+    cmd = [_nvcc(), "-shared", "-gencode", "arch=compute_90a,code=sm_90a", "-o", str(LIB), *map(str, objs)]
     if verbose:
         print(" ".join(cmd))
     subprocess.run(cmd, check=True)
@@ -73,7 +73,7 @@ def build_host_emul(force: bool = False) -> Path:
     """CPU build of the kernels' __host__ __device__ phase functions (non-GPU tests only)."""
     if force or _stale(HOST_EMUL, _sources()):
         HOST_EMUL.parent.mkdir(exist_ok=True)
-        cmd = [_nvcc(), "-O2", "-std=c++17", "-gencode", "arch=compute_100a,code=sm_100a", "-Xcompiler", "-fPIC",
+        cmd = [_nvcc(), "-O2", "-std=c++17", "-gencode", "arch=compute_90a,code=sm_90a", "-Xcompiler", "-fPIC",
                "-shared", "-o", str(HOST_EMUL), str(CSRC / "host_emul.cu")]
         subprocess.run(cmd, check=True)
     return HOST_EMUL

@@ -10,15 +10,10 @@
 //   exch 2   second swizzled exchange ([bin][branch]) so that each thread holds all 8 branches of 4 bins
 //   combine  Horner over the 8 branches with ONE lane-invariant twiddle per bin, |.|^2, group argmax
 // Same arithmetic as get_shift_fft (lib/decoder_impl.cc:430-464); see k1_fft.cuh for the derivation.
-// Shared-memory traffic per symbol: 5 x 8*sps bytes (slot read, two exchanges).  The 16 float4 of the down-chirp a thread
-// multiplies with are symbol-invariant and live in tensor memory (tmem.cuh; 64 columns per thread, 12 warps = 3 per lane
-// quadrant = 192 columns), like k1_sf10's: the shared-memory chirp table of round 1 was a sixth of the traffic of a kernel
-// whose L1 / shared pipe was the busiest unit (ncu profiles/r2_k1_sf9.txt: l1tex 68 %).  -DLB_GROUP_CHIRP_SMEM builds the
-// old form for A/B runs.  (The 16 KiB this frees at SF8 hold a seventh group, but 14 warps leave 128 registers per thread:
-// measured 0.775 against 0.881 with six groups, profiles/r2_group_chirp_tmem_ab.jsonl.)
+// Shared-memory traffic per symbol: 6 x 8*sps bytes (slot read, chirp read, two exchanges).  The down-chirp is one
+// shared-memory table per CTA, read by every group (the samples a thread multiplies with are symbol-invariant).
 #pragma once
 #include "k1_warp.cuh"
-#include "tmem.cuh"
 #include "k1_group_consts.h"
 
 namespace lb {
@@ -92,36 +87,6 @@ LB_HD void g_pass0(int t, const float4 *slot, const float4 *chirp, const GConsts
         v1[br] = cmul(v1[br], c.twk[kc]);
     }
 }
-
-#if defined(__CUDACC__)
-// pass 0 with the thread's chirp samples in tensor memory (tm: lane and first column of this thread)
-template <int SF>
-LB_D void g_pass0_tm(int t, const float4 *slot, uint32_t tm, const GConsts<SF> &c, float2 *v0, float2 *v1) {
-    using C = GCfg<SF>;
-    float2 ch[2][8];
-    tm_ld16(tm, ch[0]);
-#pragma unroll
-    for (int q = 0; q < 4; q++) {
-        tm_wait_ld();
-        if (q < 3) tm_ld16(tm + 16u * (uint32_t)(q + 1), ch[(q + 1) & 1]);      // in flight under this chunk's products
-#pragma unroll
-        for (int j = 0; j < 4; j++) {
-            const int r = 4 * q + j;
-            const float4 xv = slot[r * C::T + t];
-            v0[r] = cmul(make_float2(xv.x, xv.y), ch[q & 1][2 * j]);
-            v1[r] = cmul(make_float2(xv.z, xv.w), ch[q & 1][2 * j + 1]);
-        }
-    }
-    dft_dif<16>(v0);
-    dft_dif<16>(v1);
-#pragma unroll
-    for (int kc = 1; kc < 16; kc++) {
-        const int br = bitrev<16>(kc);
-        v0[br] = cmul(v0[br], c.twk[kc]);
-        v1[br] = cmul(v1[br], c.twk[kc]);
-    }
-}
-#endif
 
 template <int SF>
 LB_HD void g_store1(int t, float4 *slot, const float2 *v0, const float2 *v1) {
@@ -306,16 +271,12 @@ LB_HD unsigned long long g_combine_p(int t, const float2 *slot2, const float2 *q
 #ifdef __CUDACC__
 template <int SF, int NGROUPS, int NSLOT>
 struct GSmem {
-#ifdef LB_GROUP_CHIRP_SMEM
     float4 chirp[GCfg<SF>::SLOT_F4];
-#endif
     float4 slots[NGROUPS][NSLOT][GCfg<SF>::SLOT_F4];
     uint64_t bars[NGROUPS][NSLOT];
     unsigned long long keys[NGROUPS][GCfg<SF>::W];
     float2 quirk[NGROUPS][4];
-    uint32_t tm_base;
 };
-constexpr int G_TM_COLS = 256;                          // 64 columns per thread, up to four warps per lane quadrant
 
 LB_D void group_bar(int id, int nthreads) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory"); }
 
@@ -335,30 +296,8 @@ k1_group_kernel(K1Args a, uint32_t *__restrict__ bins, float *__restrict__ mags)
         for (int s = 0; s < NSLOT; s++) mbar_init(&sm.bars[grp][s], 1);
         fence_mbar_init();
     }
-#ifdef LB_GROUP_CHIRP_SMEM
     for (int i = threadIdx.x; i < C::SLOT_F4; i += NGROUPS * C::T) sm.chirp[i] = k1_ld_table4(a.chirp + 2 * i);
     __syncthreads();
-#else
-    static_assert(NGROUPS * GCfg<SF>::W <= 16, "four warps per lane quadrant at most");
-    const int wcta = threadIdx.x >> 5;                  // warp of the CTA
-    if (wcta == 0) tm_alloc<G_TM_COLS>(&sm.tm_base);
-    tm_fence_before();
-    __syncthreads();
-    tm_fence_after();
-    const uint32_t tm = sm.tm_base + ((uint32_t)(32 * (wcta & 3)) << 16) + (uint32_t)(64 * (wcta >> 2));
-#pragma unroll
-    for (int q = 0; q < 4; q++) {                       // chirp float4 #(r * T + t), r = 4 q .. 4 q + 3 -> columns 16 q .. 16 q + 15
-        float2 buf[8];
-#pragma unroll
-        for (int j = 0; j < 4; j++) {
-            const float4 dv = k1_ld_table4(a.chirp + 2 * ((4 * q + j) * C::T + t));
-            buf[2 * j] = make_float2(dv.x, dv.y);
-            buf[2 * j + 1] = make_float2(dv.z, dv.w);
-        }
-        tm_st16(tm + 16u * (uint32_t)q, buf);
-    }
-    tm_wait_st();
-#endif
     if (t == 0) {
 #pragma unroll
         for (int s = 0; s < NSLOT; s++) {
@@ -380,11 +319,7 @@ k1_group_kernel(K1Args a, uint32_t *__restrict__ bins, float *__restrict__ mags)
         mbar_wait(&sm.bars[grp][s], parity);
         {
             float2 v0[16], v1[16];
-#ifdef LB_GROUP_CHIRP_SMEM
             g_pass0<SF>(t, slot, sm.chirp, c, v0, v1);
-#else
-            g_pass0_tm<SF>(t, slot, tm, c, v0, v1);
-#endif
             group_bar(bar_id, C::T);                    // everyone has read the slot
             g_store1<SF>(t, slot, v0, v1);
         }
@@ -437,12 +372,6 @@ k1_group_kernel(K1Args a, uint32_t *__restrict__ bins, float *__restrict__ mags)
         }
         // keys[] is rewritten only after four more group barriers: no hazard with thread 0's read
     }
-#ifndef LB_GROUP_CHIRP_SMEM
-    tm_fence_before();
-    __syncthreads();                                    // every group has finished its symbols
-    tm_fence_after();
-    if (wcta == 0) tm_dealloc<G_TM_COLS>(sm.tm_base);
-#endif
 }
 #endif  // __CUDACC__
 

@@ -1,9 +1,6 @@
-// k1_packed.cu -- the SF7 warp kernel and the SF9 group kernel compiled with the packed complex product
-// (LB_PACKED_CMUL: cmul / cfma as FMUL2 + FFMA2 with the swap and the half negation folded into operand modifiers,
-// lora_common.cuh).  Measured on B200 against the scalar-product build of the same sources (profiles/r2_packed_cmul_ab.jsonl):
-// SF7 0.903 -> 0.921 of the HBM roofline, SF9 0.615 -> 0.643, but SF8 0.796 -> 0.729 (0.881 -> 0.866 after its chirp table
-// moved to tensor memory) and SF10 0.571 -> 0.566 (0.608 -> 0.608 after the same move) -- so the choice is
-// per kernel, which is why these two live in their own translation unit (the inline product is a per-TU definition).
+// k1_packed.cu -- the SF7 warp kernel and the SF9 group kernel compiled with the LB_PACKED_CMUL complex product
+// (cmul / cfma as fma(b, a.x, (-b.y, b.x) * a.y), lora_common.cuh).  The product form decides the last bit of every
+// dechirped sample, and the inline product is a per-translation-unit definition, so these two kernels live in their own unit.
 #define LB_PACKED_CMUL 1
 #include "k1_group.cuh"
 #include "k1_packed.h"

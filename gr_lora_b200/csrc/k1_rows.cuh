@@ -10,18 +10,16 @@
 //     branches (8 x 2048 points = 128 KiB).  SF12: a cluster of two CTAs per symbol, CTA c takes branches 4c .. 4c+3 (4 x 4096
 //     points = 128 KiB, the 32-byte halves of every 64-byte group of samples, fetched with a 2-D tensor-map TMA so that L2
 //     delivers every sector once); the only data that crosses SMs is one partial sum per output bin (16 KiB per symbol
-//     and direction, st.async into the peer's shared memory) -- 1/16 of the symbol; the receiving warp parks its own
-//     half in tensor memory and completes the sums one symbol later.
+//     and direction, st.async into the peer's shared memory) -- 1/16 of the symbol; the receiving warp keeps its own
+//     half in registers and completes the sums one symbol later.
 //   * a symbol is 16 ROWS of 8 KiB (row j = n1 in [j L/16, (j+1) L/16), all local branches).  Rows live in a pool of
 //     28 (SF12: 24) shared-memory slots of 8 KiB that rotates: global row g of this CTA's symbol sequence sits in slot g mod P.
 //     16 slots hold the symbol being transformed, the others receive the next rows by TMA while it is; a slot is
 //     re-armed by the warp that finished with it.  All three FFT passes are IN PLACE, so shared-memory traffic is
 //     6 x 8 B per sample (TMA write, three read-modify passes): 48 B against the 128 B/clk crossbar = 0.8 of the HBM
 //     roofline; there is no room (and no need) for a second copy of anything.
-//   * the dechirp table (128 KiB per CTA) and the inter-pass twiddles do not fit in shared memory next to that and
-//     re-reading them through L2 would double the L2 traffic.  They are thread-invariant (a thread always handles the
-//     same sample positions), so they live in TENSOR MEMORY: written once per CTA with tcgen05.st, read back per symbol
-//     with tcgen05.ld (TMEM is otherwise idle in this library: the path has no matrix product).
+//   * the dechirp table (128 KiB per CTA) and the inter-pass twiddles do not fit in shared memory next to that; they are
+//     read per symbol from global memory, where every CTA reads the same few hundred KiB, so they stay in L2.
 //   * pass structure per symbol (512 threads = 16 warps, ONE CTA barrier per symbol):
 //       pass 0  warp a1, lane (a0, p): float4 #(a, p) of each of the 16 rows -> dechirp -> two radix-16 DIFs over the rows
 //               -> twiddle W_L^{a kc} -> written back to row kc (in place; 16-byte units XOR-swizzled by a1 & 7 inside
@@ -33,10 +31,9 @@
 //     bin k = kc + 16 kb + 256 q2.  Same arithmetic as get_shift_fft including tmp[N/2] += F[N/2] and the first-maximum
 //     tie break; bins are bit-equal to the oracle's on the parity inputs, magnitudes within fp32 rounding.
 // The index arithmetic and the butterflies are __host__ __device__ (r_emulate below runs them on the CPU for the
-// non-GPU tests, with shared memory, tensor memory and the peer exchange modelled as plain arrays).
+// non-GPU tests, with shared memory and the peer exchange modelled as plain arrays).
 #pragma once
 #include "k1_warp.cuh"
-#include "tmem.cuh"
 #ifdef __CUDACC__
 #include <cuda.h>      // CUtensorMap (type only; the encoder is fetched through cudaGetDriverEntryPoint)
 #endif
@@ -65,13 +62,6 @@ constexpr int R_NSYM_BAR = 4;                            // symbol barriers in r
 // prefetched into free slots).  They get their own barrier: pass 0 loads and dechirps the early rows first and only then
 // waits for the late ones (second capture: 8.8 % of all samples sat in the single wait at the top of the loop).
 template <int SF> struct RLate { static constexpr int EARLY = RCfg<SF>::NSLOT - 16; };      // 12 (SF11) / 8 (SF12) early rows
-
-// tensor-memory columns of one thread (lane = 32 (warp & 3) + lane):
-//   chirp   [64 (warp >> 2), +64)        c[j][b] of the thread's pass-0 samples, word 4 j + 2 b + {re, im}
-//   tw0     [256 + 32 (warp >> 2), +32)  W_L^{a kc}, kc = 1..15, word 2 (kc - 1) + {re, im}
-//   tw1     [384, +32)                   W_{L/16}^{a0 kb}, kb = 1..15 (a function of the lane only: shared by 4 warps)
-//   stash   [416 + 16 (warp >> 2), +16)  SF12: the lane's 8 partial sums of the previous symbol until the peer's have arrived
-constexpr int R_TM_COLS = 512, R_TM_CHIRP = 0, R_TM_TW0 = 256, R_TM_TW1 = 384, R_TM_STASH = 416;
 
 // ---- index arithmetic --------------------------------------------------------------------------------------------------
 template <int SF> LB_HD int r_a0(int lane) { return lane / RCfg<SF>::CPA; }
@@ -211,7 +201,6 @@ struct RSmem {
     uint64_t sym_full[R_NSYM_BAR];                        // early rows of a symbol
     uint64_t sym_late[R_NSYM_BAR];                        // its last 16 - EARLY rows
     uint64_t x_full[16], x_free[16];                      // SF12: per buffer and receiving / sending warp pair, index 8 b + i
-    uint32_t tm_base;
 };
 
 struct alignas(64) RParams {
@@ -248,12 +237,6 @@ k1_rows_kernel(const __grid_constant__ RParams P) {
                 if (i < 8 || n_mine > 1) mbar_expect_tx(&sm.x_full[i], 2048u);          // phase 0 of the receive barriers (symbols 0 and 1)
         fence_mbar_init();
     }
-    if (warp == 0) tm_alloc<R_TM_COLS>(&sm.tm_base);
-    tm_fence_before();
-    __syncthreads();
-    tm_fence_after();
-    const uint32_t tm_lane = sm.tm_base + ((uint32_t)(32 * (warp & 3)) << 16);
-
     // issue of global row g of this CTA's sequence (symbol g / 16, row g % 16) into slot g % NSLOT
     auto issue_row = [&](size_t g) {
         const size_t s = g >> 4;
@@ -269,51 +252,15 @@ k1_rows_kernel(const __grid_constant__ RParams P) {
     if (tid == 0)
         for (int g = 0; g < C::NSLOT; g++) issue_row((size_t)g);
 
-    // ---- thread-invariant tables into tensor memory -------------------------------------------------------------------
-    {
-        float2 buf[8];
-#pragma unroll
-        for (int q = 0; q < 4; q++) {                     // chirp: rows 4q .. 4q+3, two samples each
-#pragma unroll
-            for (int jj = 0; jj < 4; jj++) {
-                const float4 c4 = k1_ld_table4(a.chirp + r_sample<SF>((int)rank, warp, lane, 4 * q + jj));
-                buf[2 * jj] = make_float2(c4.x, c4.y);
-                buf[2 * jj + 1] = make_float2(c4.z, c4.w);
-            }
-            tm_st16(tm_lane + (uint32_t)(R_TM_CHIRP + 64 * (warp >> 2) + 16 * q), buf);
-        }
-        const int a_idx = warp * C::A0 + r_a0<SF>(lane);
-#pragma unroll
-        for (int q = 0; q < 2; q++) {                     // tw0[kc - 1] = W_L^{a kc} = W_sps^{8 a kc}
-#pragma unroll
-            for (int i = 0; i < 8; i++) {
-                const int kc = 8 * q + i + 1;
-                buf[i] = kc < 16 ? k1_ld_table(a.tw + ((8 * a_idx * kc) & (C::SPS - 1))) : make_float2(0.f, 0.f);
-            }
-            tm_st16(tm_lane + (uint32_t)(R_TM_TW0 + 32 * (warp >> 2) + 16 * q), buf);
-        }
-        if (warp < 4) {
-#pragma unroll
-            for (int q = 0; q < 2; q++) {                 // tw1[kb - 1] = W_{L/16}^{a0 kb} = W_sps^{128 a0 kb}
-#pragma unroll
-                for (int i = 0; i < 8; i++) {
-                    const int kb = 8 * q + i + 1;
-                    buf[i] = kb < 16 ? k1_ld_table(a.tw + ((128 * r_a0<SF>(lane) * kb) & (C::SPS - 1))) : make_float2(0.f, 0.f);
-                }
-                tm_st16(tm_lane + (uint32_t)(R_TM_TW1 + 16 * q), buf);
-            }
-        }
-        tm_wait_st();
-    }
+    // thread-invariant table offsets: pass-0 twiddles W_L^{a kc} = W_sps^{8 a kc}, pass-1 twiddles W_{L/16}^{a0 kb} = W_sps^{128 a0 kb}
+    const int tw0_step = 8 * (warp * C::A0 + r_a0<SF>(lane)), tw1_step = 128 * r_a0<SF>(lane);
     // pass-2 lane constants: kc = warp, kb = lane >> 1, h = lane & 1; E = global index of the lane's first branch
     const int kb2 = lane >> 1, h2 = lane & 1;
     const int E2 = (int)rank * C::NB + h2 * C::HB;
     const int e_idx = SF == 11 ? (E2 ? 1 : 0) : (E2 >> 1);            // row of RConsts::cq for w^E (unused when E == 0)
     const float2 wb1 = k1_ld_table(a.tw + ((warp + 16 * kb2) & (C::SPS - 1)));
     const float2 wbE = k1_ld_table(a.tw + ((E2 * (warp + 16 * kb2)) & (C::SPS - 1)));
-    tm_fence_before();
-    if (C::CL == 2) cluster_sync_all(); else __syncthreads();     // tw1 columns of warps 0-3 are read by every warp; peers' barriers are initialised
-    tm_fence_after();
+    if (C::CL == 2) cluster_sync_all(); else __syncthreads();     // barriers are initialised (the peer's too)
 
     // ---- shared-memory addressing (32-bit shared addresses; every per-access term below is an immediate) -------------------
     // rows of the current symbol sit in slots (base + j) mod NSLOT, base = 16 s mod NSLOT; NSLOT and 16 are multiples of 4, so
@@ -331,16 +278,15 @@ k1_rows_kernel(const __grid_constant__ RParams P) {
     // SF12 exchange roles: warp pair x_i; this CTA finishes the bins of rows kc with (kc >> 3) == rank
     const int x_i = warp & 7;
     const bool x_mine = C::CL == 2 && (uint32_t)(warp >> 3) == rank;
-    auto finalize_prev = [&](size_t sp) {          // receiver warps: own sums (tensor memory) + the peer's (recv) of symbol sp -> argmax
+    float2 stash[8];                               // SF12 receiver warps: own partial sums of the previous symbol
+    auto finalize_prev = [&](size_t sp) {          // receiver warps: own sums (stash) + the peer's (recv) of symbol sp -> argmax
         const int xb = (int)(sp & 1) * 8 + x_i;
         RT(0, mbar_wait(&sm.x_full[xb], (uint32_t)((sp >> 1) & 1)));
-        float2 o[8];
-        tm_ld16(tm_lane + (uint32_t)(R_TM_STASH + 16 * (warp >> 2)), o);
+        const float2 *o = stash;
         const float4 *rblk = reinterpret_cast<const float4 *>(&sm.recv[xb * 256]);
         float4 u[4];
 #pragma unroll
         for (int i = 0; i < 4; i++) u[i] = rblk[i * 32 + lane];
-        tm_wait_ld();
         uint32_t dep = 0;
         unsigned long long bk = 0ull;
 #pragma unroll
@@ -383,23 +329,22 @@ k1_rows_kernel(const __grid_constant__ RParams P) {
 #pragma unroll
             for (int q = 0; q < 4; q++) {
                 if (4 * q == RLate<SF>::EARLY) RT(3, mbar_wait(&sm.sym_late[s % R_NSYM_BAR], (uint32_t)((s / R_NSYM_BAR) & 1)));
-                float2 ch[8];
-                tm_ld16(tm_lane + (uint32_t)(R_TM_CHIRP + 64 * (warp >> 2) + 16 * q), ch);
+                float4 ch[4];
+#pragma unroll
+                for (int jj = 0; jj < 4; jj++) ch[jj] = k1_ld_table4(a.chirp + r_sample<SF>((int)rank, warp, lane, 4 * q + jj));
                 float4 xv[4];
                 const uint32_t ga = ld0 + gb[q];
 #pragma unroll
                 for (int jj = 0; jj < 4; jj++) xv[jj] = lds128(ga + (uint32_t)jj * C::ROW_BYTES);
-                tm_wait_ld();
 #pragma unroll
                 for (int jj = 0; jj < 4; jj++) {
-                    v0[4 * q + jj] = cmul(make_float2(xv[jj].x, xv[jj].y), ch[2 * jj]);
-                    v1[4 * q + jj] = cmul(make_float2(xv[jj].z, xv[jj].w), ch[2 * jj + 1]);
+                    v0[4 * q + jj] = cmul(make_float2(xv[jj].x, xv[jj].y), make_float2(ch[jj].x, ch[jj].y));
+                    v1[4 * q + jj] = cmul(make_float2(xv[jj].z, xv[jj].w), make_float2(ch[jj].z, ch[jj].w));
                 }
             }
             r_dif16(v0, v1);
-            tm_ld16(tm_lane + (uint32_t)(R_TM_TW0 + 32 * (warp >> 2)), tw);
-            tm_ld16(tm_lane + (uint32_t)(R_TM_TW0 + 32 * (warp >> 2) + 16), tw + 8);
-            tm_wait_ld();
+#pragma unroll
+            for (int kc = 1; kc < 16; kc++) tw[kc - 1] = k1_ld_table(a.tw + ((tw0_step * kc) & (C::SPS - 1)));
             r_twiddle16(v0, v1, tw);
             __syncwarp();      // the loads read the TMA's linear layout, the stores write the swizzled one: inside the warp's own
                                // block, but lanes swap units -- every lane's loads before any lane's stores
@@ -433,9 +378,8 @@ k1_rows_kernel(const __grid_constant__ RParams P) {
                 v1[a1] = make_float2(u.z, u.w);
             }
             r_dif16(v0, v1);
-            tm_ld16(tm_lane + (uint32_t)R_TM_TW1, tw);
-            tm_ld16(tm_lane + (uint32_t)(R_TM_TW1 + 16), tw + 8);
-            tm_wait_ld();
+#pragma unroll
+            for (int kb = 1; kb < 16; kb++) tw[kb - 1] = k1_ld_table(a.tw + ((tw1_step * kb) & (C::SPS - 1)));
             r_twiddle16(v0, v1, tw);
 #pragma unroll
             for (int kb = 0; kb < 16; kb++) {
@@ -536,9 +480,9 @@ k1_rows_kernel(const __grid_constant__ RParams P) {
 #pragma unroll
                     for (int i = 0; i < 4; i++) st_async_peer_f4(dst + (uint32_t)i * 512u, make_float4(f[2 * i].x, f[2 * i].y, f[2 * i + 1].x, f[2 * i + 1].y), bar);
                 } else {
-                    // own half: parked in tensor memory until the next pass 2 (finalize_prev)
-                    tm_st16(tm_lane + (uint32_t)(R_TM_STASH + 16 * (warp >> 2)), f);
-                    tm_wait_st();
+                    // own half: kept until the next pass 2 (finalize_prev)
+#pragma unroll
+                    for (int i = 0; i < 8; i++) stash[i] = f[i];
                 }
             } else {
                 if (quirk_warp && lane == 1) f[0] = cadd(f[0], tq);
@@ -565,15 +509,12 @@ k1_rows_kernel(const __grid_constant__ RParams P) {
             else { P.bins[psym] = key_idx(k); if (P.mags) P.mags[psym] = sqrtf(key_mag2(k)); }
         }
     }
-    tm_fence_before();
-    if (C::CL == 2) cluster_sync_all(); else __syncthreads();     // no CTA of the pair exits while the other may still store into it
-    tm_fence_after();
-    if (warp == 0) tm_dealloc<R_TM_COLS>(sm.tm_base);
+    if (C::CL == 2) cluster_sync_all();           // no CTA of the pair exits while the other may still store into it
 }
 #endif  // __CUDACC__
 
 // ---- CPU emulation of the same index arithmetic (tests/test_host_emulation.py) ---------------------------------------------------
-// Shared memory slots, the tensor-memory tables and the peer exchange are plain arrays; the threads of a pass run one after
+// Shared memory slots and the peer exchange are plain arrays; the threads of a pass run one after
 // the other (legal: a pass only reads what the previous barrier made visible, and its in-place writes stay inside the
 // thread's own units -- the emulation asserts that by poisoning).
 template <int SF>

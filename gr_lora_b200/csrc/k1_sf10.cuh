@@ -6,17 +6,10 @@
 // sample n = 256 c + t), pass 1 a radix-32 over the 32 columns of output column kc.  The inter-pass
 // twiddle W_N^{a kc} (31 values per lane) is formed from two short lane-invariant tables,
 // W^{a (kc & 3)} and W^{a (kc & ~3)}.
-// The 32 down-chirp samples a thread multiplies with are the same for every symbol; they live in tensor
-// memory (tmem.cuh: 64 columns per thread, four 16-column loads per symbol).  Round 1 kept the chirp as a
-// 64 KiB shared-memory table: one of seven 8-byte shared-memory accesses per sample of a kernel whose
-// L1 / shared pipe was the busiest unit (ncu, profiles/r2_k1_sf10.txt: l1tex 63 %, short scoreboard 19 % of
-// the stall samples); the freed 64 KiB are a third ring slot.
-// Measured alternatives (removed): one slot per CTA with the chirp read through L1 and two CTAs per SM
-// (0.52), and two single-slot groups per CTA sharing the chirp (0.50): both lose to the ring (0.58) --
-// the TMA prefetch is worth more than the extra resident warps.
+// The 32 down-chirp samples a thread multiplies with are the same for every symbol; the CTA keeps the chirp as a
+// 64 KiB shared-memory table next to a ring of two TMA slots (64 + 2 x 64 KiB).
 #pragma once
 #include "k1_group.cuh"
-#include "tmem.cuh"
 
 namespace lb {
 
@@ -46,21 +39,6 @@ LB_HD void s10_pass0(int t, const float2 *slot, const float2 *chirp, const S10Co
     for (int r = 0; r < 32; r++) v[r] = cmul(slot[r * S10_T + t], chirp[r * S10_T + t]);
     s10_pass0_fft(c, v);
 }
-#ifdef __CUDACC__
-// the same with the thread's chirp samples in tensor memory (tm: lane and first column of this thread)
-LB_D void s10_pass0_tm(int t, const float2 *slot, uint32_t tm, const S10Consts &c, float2 *v) {
-    float2 ch[2][8];
-    tm_ld16(tm, ch[0]);
-#pragma unroll
-    for (int q = 0; q < 4; q++) {
-        tm_wait_ld();
-        if (q < 3) tm_ld16(tm + 16u * (uint32_t)(q + 1), ch[(q + 1) & 1]);      // in flight under this chunk's products
-#pragma unroll
-        for (int r = 0; r < 8; r++) v[8 * q + r] = cmul(slot[(8 * q + r) * S10_T + t], ch[q & 1][r]);
-    }
-    s10_pass0_fft(c, v);
-}
-#endif
 LB_HD void s10_pass0_fft(const S10Consts &c, float2 *v) {
     dft_dif<32>(v);
 #pragma unroll
@@ -129,12 +107,11 @@ LB_HD unsigned long long s10_combine(int t, const float2 *slot, const S10Consts 
 #ifdef __CUDACC__
 template <int NSLOT>
 struct S10Smem {
+    float2 chirp[S10_SLOT_F2];
     float2 slots[NSLOT][S10_SLOT_F2];
     uint64_t bars[NSLOT];
     unsigned long long keys[S10_T / 32];
-    uint32_t tm_base;
 };
-constexpr int S10_TM_COLS = 128;                     // 64 columns per thread, two warps per lane quadrant
 
 template <int NSLOT>
 __global__ void __launch_bounds__(S10_T, 1)
@@ -148,19 +125,8 @@ k1_sf10_kernel(K1Args a, uint32_t *__restrict__ bins, float *__restrict__ mags) 
         for (int s = 0; s < NSLOT; s++) mbar_init(&sm.bars[s], 1);
         fence_mbar_init();
     }
-    if (warp == 0) tm_alloc<S10_TM_COLS>(&sm.tm_base);
-    tm_fence_before();
+    for (int i = t; i < S10_SLOT_F2; i += S10_T) sm.chirp[i] = k1_ld_table(a.chirp + i);
     __syncthreads();
-    tm_fence_after();
-    const uint32_t tm = sm.tm_base + ((uint32_t)(32 * (warp & 3)) << 16) + (uint32_t)(64 * (warp >> 2));
-#pragma unroll
-    for (int q = 0; q < 4; q++) {                    // chirp[r * 256 + t], r = 8 q .. 8 q + 7 -> columns 16 q .. 16 q + 15
-        float2 buf[8];
-#pragma unroll
-        for (int r = 0; r < 8; r++) buf[r] = k1_ld_table(a.chirp + (8 * q + r) * S10_T + t);
-        tm_st16(tm + 16u * (uint32_t)q, buf);
-    }
-    tm_wait_st();
     if (t == 0) {
 #pragma unroll
         for (int s = 0; s < NSLOT; s++) {
@@ -179,7 +145,7 @@ k1_sf10_kernel(K1Args a, uint32_t *__restrict__ bins, float *__restrict__ mags) 
         float2 *slot = sm.slots[s];
         mbar_wait(&sm.bars[s], (it / NSLOT) & 1u);
         float2 v[32];
-        s10_pass0_tm(t, slot, tm, c, v);
+        s10_pass0(t, slot, sm.chirp, c, v);
         __syncthreads();
         s10_store1(t, slot, v);
         __syncthreads();
@@ -205,10 +171,6 @@ k1_sf10_kernel(K1Args a, uint32_t *__restrict__ bins, float *__restrict__ mags) 
             if (mags) mags[sym] = sqrtf(key_mag2(bb));
         }
     }
-    tm_fence_before();
-    __syncthreads();
-    tm_fence_after();
-    if (warp == 0) tm_dealloc<S10_TM_COLS>(sm.tm_base);
 }
 #endif
 

@@ -2,7 +2,7 @@
 //
 // Same arithmetic as k1_fft.cuh (get_shift_fft, lib/decoder_impl.cc:430-464: dechirp, pruned
 // 8x128-point FFT, 8-branch twiddled sum, first argmax) but organised around what the first
-// ncu capture of the CTA-wide kernel showed (profiles/r1_k1_sf7_generic.md): the L1/LSU data
+// ncu capture of the CTA-wide kernel showed: the L1/LSU data
 // pipe was the limiter (78 %), half of it scattered twiddle loads, and long-scoreboard stalls
 // dominated because all warps of a CTA loaded in lock step.
 //

@@ -236,14 +236,14 @@ int launch_k1_group(lora_b200_decoder *d, K1Scratch &ks, const float2 *iq, size_
 // SF10: one 256-thread group per symbol, two radix-32 passes (k1_sf10.cuh)
 int launch_k1_sf10(lora_b200_decoder *d, K1Scratch &ks, const float2 *iq, size_t n_symbols, uint32_t *bins, float *mags, cudaStream_t st) {
     static bool attr_set[64] = {};
-    const size_t smem = sizeof(S10Smem<3>);
+    const size_t smem = sizeof(S10Smem<2>);
     if (!attr_set[d->device & 63]) {
-        CU(cudaFuncSetAttribute(k1_sf10_kernel<3>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        CU(cudaFuncSetAttribute(k1_sf10_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
         attr_set[d->device & 63] = true;
     }
     K1Args a{iq, tab<float2>(d, d->toff.down), tab<float2>(d, d->toff.tw), n_symbols};
     const int grid = (int)std::min<size_t>(n_symbols, (size_t)d->n_sms);
-    k1_sf10_kernel<3><<<grid, S10_T, smem, st>>>(a, bins, mags);
+    k1_sf10_kernel<2><<<grid, S10_T, smem, st>>>(a, bins, mags);
     d->launches++;
     CU(cudaGetLastError());
     return LORA_B200_OK;

@@ -1,4 +1,4 @@
-// lora_common.cuh -- small host/device helpers shared by the sm_100a kernels.
+// lora_common.cuh -- small host/device helpers shared by the sm_90a kernels.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -17,25 +17,26 @@ namespace lb {
 // The largest float below the double M_PI (0x40490FDA; the next float, 0x40490FDB, is above it).  The reference unwraps phase
 // differences with "while ((phase2 - phase) > M_PI)" (lib/decoder_impl.cc:236-237): a float difference promoted to double.
 // For a float d, (double)d > M_PI  <=>  d > LB_PI_BELOW, and (double)d < -M_PI  <=>  d < -LB_PI_BELOW, exactly -- the test
-// needs no fp64 conversion / compare per sample (they were 15 % of the stream kernel's stall samples, profiles/r2_rx_sf7_warp.txt).
+// needs no fp64 conversion / compare per sample (they were 15 % of the stream kernel's stall samples).
 #define LB_PI_BELOW 3.14159250259399414f
 
 // ---- complex arithmetic ---------------------------------------------------------------------
-// On the device every complex value lives in an aligned 64-bit register pair and the arithmetic uses
-// Blackwell's packed fp32 instructions (PTX add/sub/mul/fma .f32x2 -> SASS FADD2 / FMUL2 / FFMA2,
-// sm_100+).  They have the FLOP rate of the scalar ops but need half the issue slots, and the K1
-// kernels are issue bound (profiles/r1_k1_sf7_warp.md, profiles/r1_f32x2_tput.txt).  ptxas folds the
-// scalar broadcasts {x,x}, the pair swaps {y,x} and whole-pair negations below into operand modifiers
-// (R.F32, .LO_HI, -R), so a complex multiply-add is two instructions.  The host build (CPU emulation
-// of the kernels for the non-GPU tests) uses the plain scalar formulas.
+// On the device a complex value can be handled as a 64-bit register pair (lb_u64).  The pair operations below are two
+// scalar fp32 operations with explicit round-to-nearest (Hopper has no packed fp32 instructions): the explicit rounding
+// keeps ptxas from contracting a product and a sum into one FFMA, so every kernel rounds exactly where its source says.
+// LB_PACKED_CMUL selects the product form cmul(a, b) = fma(b, a.x, (-b.y, b.x) * a.y) for the translation units that
+// use it; the host build (CPU emulation of the kernels for the non-GPU tests) uses the plain scalar formulas.
 typedef unsigned long long lb_u64;
 #ifdef __CUDA_ARCH__
 LB_D lb_u64 pk2(float lo, float hi) { lb_u64 r; asm("mov.b64 %0, {%1, %2};" : "=l"(r) : "f"(lo), "f"(hi)); return r; }
 LB_D float2 up2(lb_u64 v) { float2 r; asm("mov.b64 {%0, %1}, %2;" : "=f"(r.x), "=f"(r.y) : "l"(v)); return r; }
-LB_D lb_u64 add2(lb_u64 a, lb_u64 b) { lb_u64 r; asm("add.rn.f32x2 %0, %1, %2;" : "=l"(r) : "l"(a), "l"(b)); return r; }
-LB_D lb_u64 sub2(lb_u64 a, lb_u64 b) { lb_u64 r; asm("sub.rn.f32x2 %0, %1, %2;" : "=l"(r) : "l"(a), "l"(b)); return r; }
-LB_D lb_u64 mul2(lb_u64 a, lb_u64 b) { lb_u64 r; asm("mul.rn.f32x2 %0, %1, %2;" : "=l"(r) : "l"(a), "l"(b)); return r; }
-LB_D lb_u64 fma2(lb_u64 a, lb_u64 b, lb_u64 c) { lb_u64 r; asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(r) : "l"(a), "l"(b), "l"(c)); return r; }
+LB_D lb_u64 add2(lb_u64 a, lb_u64 b) { const float2 x = up2(a), y = up2(b); return pk2(__fadd_rn(x.x, y.x), __fadd_rn(x.y, y.y)); }
+LB_D lb_u64 sub2(lb_u64 a, lb_u64 b) { const float2 x = up2(a), y = up2(b); return pk2(__fsub_rn(x.x, y.x), __fsub_rn(x.y, y.y)); }
+LB_D lb_u64 mul2(lb_u64 a, lb_u64 b) { const float2 x = up2(a), y = up2(b); return pk2(__fmul_rn(x.x, y.x), __fmul_rn(x.y, y.y)); }
+LB_D lb_u64 fma2(lb_u64 a, lb_u64 b, lb_u64 c) {
+    const float2 x = up2(a), y = up2(b), z = up2(c);
+    return pk2(__fmaf_rn(x.x, y.x, z.x), __fmaf_rn(x.y, y.y, z.y));
+}
 LB_D float2 cadd(float2 a, float2 b) { return up2(add2(pk2(a.x, a.y), pk2(b.x, b.y))); }
 LB_D float2 csub(float2 a, float2 b) { return up2(sub2(pk2(a.x, a.y), pk2(b.x, b.y))); }
 // packed product with a compile-time constant (used inside the radix butterflies)
@@ -45,9 +46,6 @@ LB_D float2 cmul_const(float2 a, float wx, float wy) {
 #ifdef LB_PACKED_CMUL
 // plain complex product (the reference multiplies by the down-chirp, not its conjugate,
 // lib/decoder_impl.cc:436-438):  a*b = (b.x, b.y)*a.x + (-b.y, b.x)*a.y
-// Operand ORDER matters: with the swapped / half-negated pair as the FIRST multiplicand ptxas folds the swap and the sign
-// into operand modifiers (FMUL2 R, -Rb.F32x2.LO_HI.NP, Ra.F32), so a complex product is exactly two instructions; with
-// the broadcast first it materialises the pair with a MOV and an FADD (measured on the SASS; A/B per kernel in profiles/r2_packed_cmul_ab.jsonl).
 LB_D float2 cmul(float2 a, float2 b) {
     return up2(fma2(pk2(b.x, b.y), pk2(a.x, a.x), mul2(pk2(-b.y, b.x), pk2(a.y, a.y))));
 }
@@ -159,7 +157,7 @@ LB_HD float key_mag2(unsigned long long k) {
 #ifdef __CUDACC__
 // arg(x + i y) for the instantaneous-frequency passes (the reference's std::arg, lib/decoder_impl.cc:232-233, one per sample).
 // CUDA's atan2f is a rational approximation with two divisions and their slow-path checks: 65 instructions, 22 % of the
-// stream kernel's instructions (profiles/r2_rx_sf7_warp.txt).  This one: one IEEE division, t + t s P(s) with s = t^2 and a
+// stream kernel's instructions.  This one: one IEEE division, t + t s P(s) with s = t^2 and a
 // degree-7 minimax P fitted to relative error (1.7e-8 before rounding), then the octant fix-ups: 26 instructions, measured
 // max error 1.8 ulp on 4e6 random points (CUDA documents 2 ulp for atan2f, so the two are interchangeable for parity:
 // both differ from glibc's result in the last bit on a fraction of the samples).  Zero, infinite and NaN inputs follow C99.
@@ -195,7 +193,7 @@ LB_HD float lb_atan2f(float y, float x) {
 }
 // Maximum key of the warp in every lane: two REDUX (the high words, then the low words of the lanes that hold the maximal
 // high word) instead of five dependent 64-bit shuffle + compare rounds (10 SHFL + 20 ALU; ~6 % of k1_rows<11>'s stall
-// samples sat on that chain, profiles/r2_k1_sf11.txt)
+// samples sat on that chain)
 LB_D unsigned long long warp_max_key(unsigned long long k) {
     const uint32_t hi = (uint32_t)(k >> 32);
     const uint32_t m = __reduce_max_sync(0xffffffffu, hi);

@@ -1,7 +1,7 @@
 // rx_warp.cuh -- the receive state machine for SF7 at fs / bw = 8 (sps = 1024), ONE WARP PER STREAM.
 //
 // rx_stream_kernel (rx_stream.cuh) spends a 256-thread CTA on one stream: ~2 100 instructions per thread and symbol window,
-// 16 CTA barriers and several dependent global round trips per step (ncu, profiles/r2_rx_sf7_cta.txt: issue slots 42 %
+// 16 CTA barriers and several dependent global round trips per step (issue slots 42 %
 // active, stalls wait / barrier / long scoreboard 19 % each; 8.1e6 windows/s on 4096 streams).  At SF7 a window is 1024
 // samples = 32 per lane, which is exactly the shape of the SF7 K1 warp kernel (k1_warp.cuh).  Here a warp owns a stream:
 //   * the window (<= 2 sps samples, 16 KiB), its instantaneous frequency (8 KiB) and the decoder_impl members
@@ -18,9 +18,9 @@
 //     lane over a block of 32 products; the three-lag fine_sync of a payload symbol keeps the CTA kernel's lane-strided
 //     order.  arg() is lb_atan2f (lora_common.cuh), four groups of 32 samples at a time.
 //   * what bounds it: two or three warps per scheduler, every one a chain of dependent steps (ncu,
-//     profiles/r2_rx_warp_final.txt: issue slots 42 % active, stalls wait 24 %, long scoreboard 18 %); 4 700 warp
+//     issue slots 42 % active, stalls wait 24 %, long scoreboard 18 %); 4 700 warp
 //     instructions per window, a third of them the per-sample arg() and unwrap.  The kernel alone runs 4096 streams x 256
-//     windows in 12 ms (8.7e7 windows/s); history in profiles/r2_rx_path.md.
+//     windows in 12 ms (8.7e7 windows/s).
 // Same observable behaviour as rx_stream_kernel: frames, consume amounts, per-step trace.  Other SFs and sample rates use
 // rx_stream_kernel.
 #pragma once
@@ -53,7 +53,7 @@ struct RWSmem {
 // window samples [0, n) of the stream into the warp's buffer (8-byte accesses: the window starts at any sample); the lines
 // of the following window are requested into L2 meanwhile -- where the next step starts is only known at the end of this
 // one (consumed = sps +- fine sync), but it is within a few samples of g + n, and a step's first act is this load
-// (11 % of the stall samples sat on it, profiles/r2b_rx_warp.txt)
+// (11 % of the stall samples sat on it)
 LB_D void rw_load(const float2 *__restrict__ g, float2 *win, int n, int lane, const float2 *g_end) {
     {
         const char *nx = reinterpret_cast<const char *>(g + n) + 128 * lane;

@@ -1,5 +1,5 @@
 /*
- * lora_b200.h -- C ABI of liblora_b200.so, the B200 (sm_100a) replacement for the hot path of
+ * lora_b200.h -- C ABI of liblora_b200.so, the H100 (sm_90a) replacement for the hot path of
  * rpp0/gr-lora: gr::lora::decoder_impl::work() and the DSP helpers it calls
  * (lib/decoder_impl.cc:141-903 of the reference).
  *

@@ -12,6 +12,7 @@ oracle/_ref/liblora_ref.so is present."""
 from __future__ import annotations
 
 import ctypes as C
+import os
 import subprocess
 from pathlib import Path
 
@@ -28,15 +29,20 @@ _lib = None
 
 def build(force: bool = False) -> Path | None:
     """(Re)build where the reference sources exist; otherwise keep whatever prebuilt file travelled here."""
-    if (REF_ROOT / "lib" / "decoder_impl.cc").exists():
+    if _have_sources():
         if force and LIB.exists():
             LIB.unlink()
         subprocess.run(["make", "-C", str(HERE), "-s", "ref"], check=True)
     return LIB if LIB.exists() else None
 
 
+def _have_sources() -> bool:
+    # isfile, not Path.exists: an unreadable parent directory means "absent", not an error
+    return os.path.isfile(REF_ROOT / "lib" / "decoder_impl.cc")
+
+
 def available() -> bool:
-    return LIB.exists() or (REF_ROOT / "lib" / "decoder_impl.cc").exists()
+    return LIB.exists() or _have_sources()
 
 
 def lib():

@@ -14,8 +14,8 @@ import pytest
 
 pytestmark = pytest.mark.gpu
 
-# symbols = more than (NSLOT + 2) passes of the default kernel's grid on 148 SMs, + a ragged tail
-MULTIPASS_N = {7: 148 * 12 * 4 + 7, 8: 148 * 6 * 4 + 7, 9: 148 * 3 * 4 + 7, 10: 148 * 4 + 315, 11: 148 * 4 + 15, 12: 233}
+# symbols = more than (NSLOT + 2) passes of the default kernel's grid on the H100's 132 SMs, + a ragged tail
+MULTIPASS_N = {7: 132 * 12 * 4 + 7, 8: 132 * 6 * 4 + 7, 9: 132 * 3 * 4 + 7, 10: 132 * 4 + 315, 11: 132 * 4 + 15, 12: 233}
 
 
 @pytest.fixture(scope="module")

@@ -65,12 +65,9 @@ def test_whitening_tables():
     for name in ("prng_header", "prng_payload_cr56", "prng_payload_cr78"):
         h.update(name.encode() + b"\0" + getattr(whitening, name.upper()) + b"\0")
     assert h.hexdigest() == whitening.SHA256
-    ref = Path("/root/reference/lib/tables.h")
-    if ref.exists():     # only in the build container
-        import sys
-        sys.path.insert(0, str(Path(__file__).parent.parent / "tools"))
-        import gen_tables
-        assert gen_tables.digest(gen_tables.parse(ref)) == whitening.SHA256
+    # the digest tools/gen_tables.py computed from the reference's lib/tables.h (tests/golden/reference_tables.json)
+    ref = json.loads((Path(__file__).parent / "golden" / "reference_tables.json").read_text())
+    assert ref["whitening_tables_sha256"] == whitening.SHA256
 
 
 def test_derived_parameters(oracle):

@@ -78,7 +78,7 @@ def test_get_shift_fft(oracle, ref, sf):
             assert np.array_equal(rb, vals)
     # the kept N bins of one symbol (bins 0..N/2-1 | sps-N/2..sps-1, plus the tmp[N/2] += F[N/2] quirk)
     spec = r.spectrum(x[: r.sps])
-    mult = x[: r.sps].astype(np.complex128) * r.downchirp.astype(np.complex128)
+    mult = x[: r.sps].astype(np.complex128) * o.downchirp.astype(np.complex128)      # == the reference's (test above)
     F = np.fft.fft(mult)
     N = r.n_bins
     want = np.concatenate([F[: N // 2], F[r.sps - N // 2:]])

@@ -47,7 +47,7 @@ def main():
     import gr_lora_b200 as G
     out = {"wideband_10MSps_64ch": run(torch, G, 10e6, 10, 64, 1.0),
            "reference_use_1MSps_1ch": run(torch, G, 1e6, 1, 1, 4.0),
-           "note": "fp32 CUDA-core FIR bank; B200 fp32 peak ~ 75 TFLOP/s (148 SMs x 128 lanes x 2 x 1.97 GHz)"}
+           "note": "fp32 CUDA-core FIR bank; H100 SXM data-sheet fp32 peak 67 TFLOP/s"}
     print(json.dumps(out))
 
 
