@@ -23,6 +23,12 @@ class Step(C.Structure):
                 ("metric", C.c_float)]
 
 
+class TxFrame(C.Structure):
+    """struct lora_b200_tx_frame (include/lora_b200.h): one frame placed by lora_b200_tx_frames_dev."""
+    _fields_ = [("start", C.c_uint64), ("stream", C.c_uint32), ("n_symbols", C.c_uint32), ("cfo_hz", C.c_float),
+                ("sync_word", C.c_uint8), ("pad", C.c_uint8 * 3)]
+
+
 FRAME_CB = C.CFUNCTYPE(None, C.c_void_p, C.c_uint32, C.POINTER(C.c_uint8), C.c_size_t)
 
 OK, EINVAL, ECUDA, ENOMEM, EUNSUPPORTED, EOVERFLOW = 0, -1, -2, -3, -4, -5
@@ -55,6 +61,9 @@ SIGNATURES = {
     "lora_b200_ifreq_dev": (_i, [_vp, _vp, _sz, _u32, _vp, _vp]),
     "lora_b200_tx_symbols_dev": (_i, [_vp, _vp, _vp, _vp, C.c_float, C.c_uint64, _sz, _vp, _vp]),
     "lora_b200_tx_expand_dev": (_i, [_vp, _vp, _u32, _sz, C.c_float, C.c_uint64, _sz, _vp, _vp]),
+    "lora_b200_tx_frame_symbols": (_u32, [C.POINTER(Config), _u32]),
+    "lora_b200_tx_encode_dev": (_i, [_vp, _vp, _vp, _vp, _sz, _vp, _u32, _vp]),
+    "lora_b200_tx_frames_dev": (_i, [_vp, _vp, C.POINTER(TxFrame), _sz, _vp, _u32, C.c_float, C.c_uint64, _sz, _sz, _vp, _vp]),
     "lora_b200_decode_codewords_dev": (_i, [_vp, _vp, _vp, _sz, _vp, _vp, _sz, _vp, _sz, _vp, _vp]),
     "lora_b200_deinterleave_dev": (_i, [_vp, _vp, _u32, _u32, _sz, _vp, _vp]),
     "lora_b200_work": (_i, [_vp, _u32, _vp, _sz, C.POINTER(_sz), FRAME_CB, _vp]),

@@ -8,6 +8,7 @@
 #include "k1_rows.cuh"
 #include "int_chain.cuh"
 #include "tx_channel.cuh"
+#include "tx_encode.cuh"
 
 extern "C" {
 
@@ -78,5 +79,18 @@ uint8_t lb_emul_hamming84_decode(uint8_t cw) { return lb::hamming84_decode(cw); 
 uint8_t lb_emul_hamming84_encode(uint8_t v) { return lb::hamming84_encode(v); }
 uint8_t lb_emul_deshuffle(uint8_t v) { return lb::deshuffle_byte(v); }
 int32_t lb_emul_payload_symbols(uint32_t len, uint32_t cr, uint32_t sf, int rr) { return lb::payload_symbols(len, cr, sf, rr); }
+
+// the frame encoder of tx_encode_kernel (tx_encode.cuh), one frame on the host: writes its data symbols' chirp shifts and
+// returns their number, 0 for a length the encoder refuses or more than cap symbols
+uint32_t lb_emul_tx_encode(const uint8_t *payload, uint32_t len, uint32_t sf, uint32_t cr, int implicit, int crc, int reduced_rate,
+                           uint32_t *shifts, uint32_t cap) {
+    const lb::TxCode c{sf, cr, implicit ? 0u : 1u, crc ? 1u : 0u, reduced_rate ? 1u : 0u};
+    if (!lb::tx_length_ok(c, len)) return 0;
+    const uint32_t n = lb::tx_data_symbols(c, len);
+    if (n > cap) return 0;
+    for (uint32_t i = 0; i < n; i++) shifts[i] = lb::tx_symbol_shift(c, payload, len, i);
+    return n;
+}
+uint32_t lb_emul_header_checksum(uint32_t length, uint32_t cr, uint32_t crc) { return lb::header_checksum(length, cr, crc); }
 
 }

@@ -10,6 +10,7 @@
 #include "rx_stream.cuh"
 #include "rx_warp.cuh"
 #include "tx_channel.cuh"
+#include "tx_encode.cuh"
 #include "k1_rows.h"
 #include "k1_packed.h"
 
@@ -111,6 +112,12 @@ struct lora_b200_decoder {
     std::vector<std::string> stdout_last;
     uint64_t launches = 0;
     bool cfo_estimate = false;            // lora_b200_set_cfo_estimate
+    // per-frame tables of lora_b200_tx_encode_dev / lora_b200_tx_frames_dev, uploaded on the caller's stream; `tx_done`
+    // marks the end of the last launch that reads them, so the next upload waits for it on the host
+    void *d_tx = nullptr;
+    size_t tx_cap = 0;
+    cudaEvent_t tx_done = nullptr;
+    bool tx_used = false;
 };
 
 namespace {
@@ -651,6 +658,8 @@ void lora_b200_destroy(lora_b200_decoder *d) {
     for (cudaEvent_t e : d->stage_events) if (e) cudaEventDestroy(e);
     if (d->h_stage) cudaFreeHost(d->h_stage);
     if (d->h_frames) cudaFreeHost(d->h_frames);
+    cudaFree(d->d_tx);
+    if (d->tx_done) cudaEventDestroy(d->tx_done);
     delete d;
 }
 
@@ -992,6 +1001,125 @@ int lora_b200_tx_expand_dev(lora_b200_decoder *d, const void *base, uint32_t k, 
     d->launches++;
     CU(cudaGetLastError());
     return LORA_B200_OK;
+}
+
+// the encoder's view of a configuration; false for one it does not support (SF7..12, CR 4/5..4/8)
+static bool tx_code(const lora_b200_config &cfg, TxCode *c) {
+    if (cfg.sf < 7 || cfg.sf > 12 || cfg.cr < 1 || cfg.cr > 4) return false;
+    *c = TxCode{cfg.sf, cfg.cr, cfg.implicit ? 0u : 1u, cfg.crc ? 1u : 0u, cfg.reduced_rate ? 1u : 0u};
+    return true;
+}
+
+// upload the per-frame table of a tx call into d->d_tx on `st`, after the previous call that read it has finished
+static int tx_upload(lora_b200_decoder *d, const void *src, size_t bytes, cudaStream_t st) {
+    if (d->tx_used) CU(cudaEventSynchronize(d->tx_done));
+    if (!d->tx_done) CU(cudaEventCreateWithFlags(&d->tx_done, cudaEventDisableTiming));
+    if (bytes > d->tx_cap) {
+        CU(cudaFree(d->d_tx));
+        d->d_tx = nullptr;
+        d->tx_cap = 0;
+        CU(cudaMalloc(&d->d_tx, bytes));
+        d->tx_cap = bytes;
+    }
+    CU(cudaMemcpyAsync(d->d_tx, src, bytes, cudaMemcpyHostToDevice, st));
+    return LORA_B200_OK;
+}
+
+static int tx_launched(lora_b200_decoder *d, cudaStream_t st) {
+    d->launches++;
+    CU(cudaGetLastError());
+    CU(cudaEventRecord(d->tx_done, st));
+    d->tx_used = true;
+    return LORA_B200_OK;
+}
+
+uint32_t lora_b200_tx_frame_symbols(const lora_b200_config *cfg, uint32_t payload_len) {
+    TxCode c;
+    if (!cfg || !tx_code(*cfg, &c) || !tx_length_ok(c, payload_len)) return 0;
+    return tx_data_symbols(c, payload_len);
+}
+
+int lora_b200_tx_encode_dev(lora_b200_decoder *d, const uint8_t *payloads, const uint32_t *offsets, const uint32_t *lengths,
+                            size_t n_frames, uint32_t *shifts, uint32_t max_symbols, void *stream) {
+    if (!d || (n_frames && (!offsets || !lengths || !shifts))) return fail(LORA_B200_EINVAL, "null argument");
+    TxCode c;
+    if (!tx_code(d->cfg, &c)) return fail(LORA_B200_EUNSUPPORTED, "frame encoder needs SF7..SF12 and CR 1..4");
+    std::vector<uint2> tab(n_frames);
+    for (size_t f = 0; f < n_frames; f++) {
+        const uint32_t len = lengths[f];
+        if (!tx_length_ok(c, len))
+            return fail(LORA_B200_EINVAL, "frame %zu: payload length %u out of range (at most %u%s)", f, len, 255u + 2u * c.crc,
+                        c.explicit_hdr && c.crc ? ", at least 2 with CRC" : "");
+        if (len && !payloads) return fail(LORA_B200_EINVAL, "null payloads");
+        if (tx_data_symbols(c, len) > max_symbols)
+            return fail(LORA_B200_EINVAL, "frame %zu needs %u symbols, max_symbols is %u", f, tx_data_symbols(c, len), max_symbols);
+        tab[f] = make_uint2(offsets[f], len);
+    }
+    CU(cudaSetDevice(d->device));
+    if (n_frames == 0) return LORA_B200_OK;
+    const cudaStream_t st = (cudaStream_t)stream;
+    if (int rc = tx_upload(d, tab.data(), sizeof(uint2) * n_frames, st)) return rc;
+    const size_t threads = n_frames * max_symbols;
+    const int grid = (int)std::min<size_t>((threads + 255) / 256, (size_t)d->n_sms * 16);
+    tx_encode_kernel<<<grid, 256, 0, st>>>(c, payloads, (const uint2 *)d->d_tx, n_frames, max_symbols, shifts);
+    return tx_launched(d, st);
+}
+
+static_assert(sizeof(lora_b200_tx_frame) == 24 && offsetof(lora_b200_tx_frame, stream) == 8 &&
+              offsetof(lora_b200_tx_frame, n_symbols) == 12 && offsetof(lora_b200_tx_frame, cfo_hz) == 16 &&
+              offsetof(lora_b200_tx_frame, sync_word) == 20, "lora_b200_tx_frame layout");
+
+int lora_b200_tx_frames_dev(lora_b200_decoder *d, const void *up_table, const lora_b200_tx_frame *frames, size_t n_frames,
+                            const uint32_t *shifts, uint32_t max_symbols, float noise_sigma, uint64_t seed, size_t n_streams,
+                            size_t n_items, void *out, void *stream) {
+    if (!d || (n_frames && (!frames || !shifts)) || (n_streams && n_items && !out)) return fail(LORA_B200_EINVAL, "null argument");
+    if (n_items & 1u) return fail(LORA_B200_EINVAL, "n_items must be even");
+    if (((uintptr_t)out & 15u) != 0) return fail(LORA_B200_EINVAL, "out must be 16-byte aligned");
+    if (d->sps & 1u) return fail(LORA_B200_EUNSUPPORTED, "odd samples per symbol");
+    if (n_frames >= 0xFFFFFFFFu || n_streams >= 0xFFFFFFFFu) return fail(LORA_B200_EINVAL, "too many frames or streams");
+    // sort by (row, start), check placement, then one upload: row_ptr[n_streams + 1] | pad | TxFrameDesc[n_frames]
+    std::vector<uint32_t> order(n_frames);
+    for (size_t f = 0; f < n_frames; f++) {
+        const lora_b200_tx_frame &fr = frames[f];
+        if (fr.stream >= n_streams) return fail(LORA_B200_EINVAL, "frame %zu: stream %u >= n_streams %zu", f, fr.stream, n_streams);
+        if (fr.n_symbols > max_symbols) return fail(LORA_B200_EINVAL, "frame %zu: n_symbols %u > max_symbols %u", f, fr.n_symbols, max_symbols);
+        const unsigned long long len = tx_frame_samples(fr.n_symbols, d->sps);
+        if (len > 0xFFFFFFFFull || fr.start > n_items || len > n_items - fr.start)
+            return fail(LORA_B200_EINVAL, "frame %zu: samples [%llu, %llu) run past n_items %zu", f, (unsigned long long)fr.start,
+                        (unsigned long long)fr.start + len, n_items);
+        order[f] = (uint32_t)f;
+    }
+    std::sort(order.begin(), order.end(), [&](uint32_t a, uint32_t b) {
+        return frames[a].stream != frames[b].stream ? frames[a].stream < frames[b].stream : frames[a].start < frames[b].start;
+    });
+    const size_t desc_off = ((n_streams + 1) * sizeof(uint32_t) + 15) & ~(size_t)15;
+    std::vector<uint8_t> blob(desc_off + sizeof(TxFrameDesc) * n_frames, 0);
+    uint32_t *row_ptr = reinterpret_cast<uint32_t *>(blob.data());
+    TxFrameDesc *desc = reinterpret_cast<TxFrameDesc *>(blob.data() + desc_off);
+    for (size_t k = 0; k < n_frames; k++) {
+        const lora_b200_tx_frame &fr = frames[order[k]];
+        if (k && frames[order[k - 1]].stream == fr.stream) {
+            const lora_b200_tx_frame &pr = frames[order[k - 1]];
+            if (pr.start + tx_frame_samples(pr.n_symbols, d->sps) > fr.start)
+                return fail(LORA_B200_EINVAL, "frames %u and %u overlap in stream %u", order[k - 1], order[k], fr.stream);
+        }
+        const uint32_t sync = ((((fr.sync_word >> 4) & 15u) * 8u) % d->n_bins) | ((((fr.sync_word & 15u) * 8u) % d->n_bins) << 16);
+        desc[k] = TxFrameDesc{fr.start, fr.n_symbols, fr.cfo_hz, order[k], sync};
+        row_ptr[fr.stream + 1]++;
+    }
+    for (size_t s = 0; s < n_streams; s++) row_ptr[s + 1] += row_ptr[s];
+    CU(cudaSetDevice(d->device));
+    if (n_streams == 0 || n_items == 0) return LORA_B200_OK;
+    const cudaStream_t st = (cudaStream_t)stream;
+    if (int rc = tx_upload(d, blob.data(), blob.size(), st)) return rc;
+    const float2 *up = up_table ? (const float2 *)up_table : tab<float2>(d, d->toff.up);
+    const size_t threads = n_streams * (n_items / 2);
+    const int grid = (int)std::min<size_t>((threads + 255) / 256, (size_t)d->n_sms * 16);
+    tx_frames_kernel<<<grid, 256, 0, st>>>(up, d->sps, d->decim, d->n_bins, (const uint32_t *)d->d_tx,
+                                           (const TxFrameDesc *)((const uint8_t *)d->d_tx + desc_off), shifts, max_symbols,
+                                           1.0 / (double)d->cfg.samp_rate, noise_sigma, (unsigned long long)seed, n_items, n_streams,
+                                           (float2 *)out);
+    return tx_launched(d, st);
 }
 
 int lora_b200_work_batch_sc8(lora_b200_decoder *d, const void *iq_sc8, float scale, size_t n_items, size_t stride_items,

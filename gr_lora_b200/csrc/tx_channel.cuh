@@ -6,7 +6,9 @@
 //                         + sigma (N(0,1) + j N(0,1)) -- the cyclic-shift modulator of gr_lora_b200/tx.py::modulate_shifts
 //                         (bit-identical to it when given the same chirp table and no noise / CFO);
 //   * tx_expand_kernel    a batch of concurrent channels from K base captures: out[s] = base[s mod K] + the stream's own
-//                         noise (64 channels that replay one capture would correlate perfectly).
+//                         noise (64 channels that replay one capture would correlate perfectly);
+//   * tx_frames_kernel    whole streams of placed frames (preamble, sync word, SFD, the data symbols tx_encode_kernel of
+//                         tx_encode.cuh produced), per-frame CFO, the noise of tx_expand_kernel: every stream its own payloads.
 // Noise: Philox4x32-10 keyed by the seed, counter = (sample pair, row), Box-Muller on the four 32-bit outputs -- a
 // counter-based generator, so the result does not depend on the launch geometry.  Both kernels are HBM-write bound.
 #pragma once
@@ -89,6 +91,78 @@ __global__ void tx_expand_kernel(const float2 *__restrict__ base, uint32_t k, si
         if (sigma != 0.0f) {
             const float4 z = philox_normal4(seed, s, i / 2);
             o = make_float4(fmaf(sigma, z.x, v.x), fmaf(sigma, z.y, v.y), fmaf(sigma, z.z, v.z), fmaf(sigma, z.w, v.w));
+        }
+        __stcs(reinterpret_cast<float4 *>(out + s * n_items + i), o);
+    }
+}
+
+// one placed frame of tx_frames_kernel; a row's frames are sorted by start and do not overlap
+struct TxFrameDesc {
+    unsigned long long start;   // first preamble sample in the row
+    uint32_t n_symbols;         // data symbols, shifts[shift_row * max_symbols ..]
+    float cfo_hz;
+    uint32_t shift_row;
+    uint32_t sync;              // bins of the two sync symbols, low and high half
+};
+
+// samples of a frame: 8 preamble up-chirps, 2 sync symbols, 2.25 down-chirps (conj(up)), then the data symbols
+LB_HD unsigned long long tx_frame_samples(uint32_t n_symbols, uint32_t sps) { return (12ull + n_symbols) * sps + sps / 4u; }
+
+// sample o (< tx_frame_samples) of frame fr, before the CFO rotation
+LB_D float2 tx_frame_sample(const float2 *__restrict__ up, uint32_t sps, uint32_t decim, const TxFrameDesc &fr,
+                            const uint32_t *__restrict__ shifts, uint32_t max_symbols, uint32_t n_bins, uint32_t o) {
+    const uint32_t q = o / sps, r = o - q * sps;
+    if (q < 8u) return __ldg(up + r);
+    if (q < 10u) return __ldg(up + (r + ((q == 8u ? fr.sync : fr.sync >> 16) & 0xFFFFu) * decim) % sps);
+    const uint32_t sfd_end = 12u * sps + sps / 4u;
+    if (o < sfd_end) {                 // conj(up), with +0 for a zero imaginary part, as tx.channel's complex scaling leaves it
+        const float2 u = __ldg(up + r);
+        return make_float2(u.x, __fsub_rn(0.0f, u.y));
+    }
+    const uint32_t d = o - sfd_end, k = d / sps, rr = d - k * sps;
+    const uint32_t sh = __ldg(shifts + (size_t)fr.shift_row * max_symbols + k) % n_bins;
+    return __ldg(up + (rr + sh * decim) % sps);
+}
+
+// whole streams of frames: out[s][n] = frame sample (0 outside every frame) * e^{j 2 pi cfo n / fs} + noise(seed, s, n), the
+// noise exactly tx_expand_kernel's, so that with sigma > 0 the output equals tx_expand over the sigma = 0 output.  One thread
+// = one sample pair; the covering frame comes from a binary search of the row's sorted list (row_ptr: CSR over rows).
+__global__ void tx_frames_kernel(const float2 *__restrict__ up, uint32_t sps, uint32_t decim, uint32_t n_bins,
+                                 const uint32_t *__restrict__ row_ptr, const TxFrameDesc *__restrict__ frames,
+                                 const uint32_t *__restrict__ shifts, uint32_t max_symbols, double inv_fs, float sigma,
+                                 unsigned long long seed, size_t n_items, size_t n_streams, float2 *__restrict__ out) {
+    const size_t pairs = n_items / 2, total = n_streams * pairs;
+    for (size_t g = (size_t)blockIdx.x * blockDim.x + threadIdx.x; g < total; g += (size_t)gridDim.x * blockDim.x) {
+        const size_t s = g / pairs, i = (g - s * pairs) * 2;
+        // last frame of the row that starts at or before sample i + 1
+        uint32_t lo = __ldg(row_ptr + s), hi = __ldg(row_ptr + s + 1);
+        const uint32_t first = lo;
+        while (lo < hi) {
+            const uint32_t mid = (lo + hi) >> 1;
+            if (frames[mid].start <= i + 1) lo = mid + 1; else hi = mid;
+        }
+        float2 v[2] = {make_float2(0.f, 0.f), make_float2(0.f, 0.f)};
+        for (int e = 0; e < 2 && lo > first; e++) {
+            const size_t n = i + e;
+            // sample i may still belong to the frame before one that starts at i + 1
+            const uint32_t k = (e == 0 && frames[lo - 1].start > n) ? lo - 2 : lo - 1;
+            if (k < first || k == 0xFFFFFFFFu) continue;
+            const TxFrameDesc fr = frames[k];
+            if (n < fr.start || n - fr.start >= tx_frame_samples(fr.n_symbols, sps)) continue;
+            float2 a = tx_frame_sample(up, sps, decim, fr, shifts, max_symbols, n_bins, (uint32_t)(n - fr.start));
+            if (fr.cfo_hz != 0.0f) {                                 // as tx_symbols_kernel: phase reduced in double
+                double t = (double)fr.cfo_hz * inv_fs * (double)n;
+                t -= floor(t);
+                float sn, cs;
+                sincospif(2.0f * (float)t, &sn, &cs);
+                a = make_float2(a.x * cs - a.y * sn, a.x * sn + a.y * cs);
+            }
+            v[e] = a;
+        }
+        float4 o = make_float4(v[0].x, v[0].y, v[1].x, v[1].y);
+        if (sigma != 0.0f) {
+            const float4 z = philox_normal4(seed, s, i / 2);
+            o = make_float4(fmaf(sigma, z.x, o.x), fmaf(sigma, z.y, o.y), fmaf(sigma, z.z, o.z), fmaf(sigma, z.w, o.w));
         }
         __stcs(reinterpret_cast<float4 *>(out + s * n_items + i), o);
     }

@@ -268,6 +268,69 @@ class decoder:
         N.check(self._L.lora_b200_tx_expand_dev(self._h, _dev_ptr(base_dev), int(k), int(n_items), float(noise_sigma), int(seed),
                                                int(n_streams), _dev_ptr(out_dev), int(cuda_stream)), "lora_b200_tx_expand_dev")
 
+    TX_FRAME_DTYPE = np.dtype([("start", "<u8"), ("stream", "<u4"), ("n_symbols", "<u4"), ("cfo_hz", "<f4"), ("sync_word", "u1"),
+                               ("pad", "u1", (3,))])     # struct lora_b200_tx_frame
+
+    def tx_encode(self, payloads_dev, offsets, lengths, shifts_dev, max_symbols, cuda_stream=0):
+        """Frame encoder on the device: frame f = payloads_dev[offsets[f] .. + lengths[f]) (host arrays offsets, lengths) ->
+        chirp shifts_dev[f * max_symbols + i] for its tx_frame_symbols() data symbols, as tx.encode_frame gives them."""
+        off = np.ascontiguousarray(offsets, dtype=np.uint32)
+        ln = np.ascontiguousarray(lengths, dtype=np.uint32)
+        assert off.shape == ln.shape and off.ndim == 1
+        N.check(self._L.lora_b200_tx_encode_dev(self._h, _dev_ptr(payloads_dev), off.ctypes.data, ln.ctypes.data, ln.size,
+                                               _dev_ptr(shifts_dev), int(max_symbols), int(cuda_stream)), "lora_b200_tx_encode_dev")
+
+    def tx_frames(self, frames, shifts_dev, max_symbols, n_streams, n_items, out_dev, noise_sigma=0.0, seed=0, up_table_dev=None,
+                  cuda_stream=0):
+        """Whole streams of frames on the device: out_dev [n_streams, n_items] cf32.  frames: structured array of TX_FRAME_DTYPE
+        (host, any order); frame f's data symbols are shifts_dev[f * max_symbols ..]."""
+        fr = np.ascontiguousarray(frames, dtype=self.TX_FRAME_DTYPE)
+        N.check(self._L.lora_b200_tx_frames_dev(self._h, _dev_ptr(up_table_dev), C.cast(fr.ctypes.data, C.POINTER(N.TxFrame)), fr.size,
+                                               _dev_ptr(shifts_dev), int(max_symbols), float(noise_sigma), int(seed), int(n_streams),
+                                               int(n_items), _dev_ptr(out_dev), int(cuda_stream)), "lora_b200_tx_frames_dev")
+
+    def synth_streams(self, payloads_per_stream, n_items, *, lead_symbols=3.0, gap_symbols=4.0, sync_word=0x12, cfo_hz=0.0,
+                      noise_sigma=0.0, seed=0, up_table_dev=None):
+        """Stream s of a [len(payloads_per_stream), n_items] cf32 device tensor carries the frames of payloads_per_stream[s]
+        under this decoder's sf / cr / implicit / crc / reduced_rate, laid out as tx.channel does it: int(lead_symbols * sps)
+        of silence, then every frame followed by int(gap_symbols * sps) of silence.  A frame is placed while it and the gap
+        after it fit in the row.  cfo_hz: one value for every frame, or a sequence per stream with one value per payload.
+        Encoding (tx_encode) and modulation (tx_frames) run on the device, on torch's current stream.
+        Returns (tensor, [(stream, start, payload) of every placed frame])."""
+        import torch
+        sps, lead, gap = self.sps, int(lead_symbols * self.sps), int(gap_symbols * self.sps)
+        n_sym = {}
+        placed, rows = [], []
+        for s, pays in enumerate(payloads_per_stream):
+            pos = lead
+            for k, p in enumerate(pays):
+                p = bytes(p)
+                if len(p) not in n_sym:
+                    n_sym[len(p)] = int(self._L.lora_b200_tx_frame_symbols(C.byref(self.cfg), len(p)))
+                    if n_sym[len(p)] == 0:
+                        raise ValueError(f"payload length {len(p)} is not encodable under this configuration")
+                flen = (12 + n_sym[len(p)]) * sps + sps // 4
+                if pos + flen + gap > n_items:
+                    break
+                placed.append((s, pos, p))
+                rows.append((pos, s, n_sym[len(p)], float(cfo_hz if np.isscalar(cfo_hz) else cfo_hz[s][k]), int(sync_word) & 0xFF))
+                pos += flen + gap
+        dev = torch.device("cuda", self.cfg.device if self.cfg.device >= 0 else torch.cuda.current_device())
+        stream = torch.cuda.current_stream(dev).cuda_stream
+        lengths = np.array([len(p) for _, _, p in placed], np.uint32)
+        offsets = (np.cumsum(lengths, dtype=np.uint64) - lengths).astype(np.uint32)
+        max_symbols = max([n for _, _, n, _, _ in rows], default=8)
+        blob = b"".join(p for _, _, p in placed)
+        pay = torch.from_numpy(np.frombuffer(blob, np.uint8).copy()).to(dev) if blob else torch.zeros(1, dtype=torch.uint8, device=dev)
+        shifts = torch.empty(max(len(placed), 1) * max_symbols, dtype=torch.int32, device=dev)
+        self.tx_encode(pay, offsets, lengths, shifts, max_symbols, stream)
+        frames = np.zeros(len(rows), self.TX_FRAME_DTYPE)
+        for f, (start, s, n, cfo, sw) in enumerate(rows):
+            frames[f] = (start, s, n, cfo, sw, (0, 0, 0))
+        out = torch.empty((len(payloads_per_stream), n_items), dtype=torch.complex64, device=dev)
+        self.tx_frames(frames, shifts, max_symbols, len(payloads_per_stream), n_items, out, noise_sigma, seed, up_table_dev, stream)
+        return out, placed
+
     def ifreq(self, iq_dev, n_windows, window, out_dev, cuda_stream=0):
         """A3 instantaneous_frequency of n_windows windows of `window` samples (device tensors)."""
         N.check(self._L.lora_b200_ifreq_dev(self._h, _dev_ptr(iq_dev), int(n_windows), int(window), _dev_ptr(out_dev),
@@ -327,6 +390,14 @@ def tables_build_host(samp_rate=1e6, bandwidth=125000, sf=7) -> np.ndarray:
     out = np.empty(n, np.uint8)
     L.lora_b200_tables_build_host(C.byref(cfg), out.ctypes.data, out.size)
     return out
+
+
+def tx_frame_symbols(payload_len, sf, cr, implicit, crc, reduced_rate, samp_rate=1e6, bandwidth=125000) -> int:
+    """Data symbols (8-symbol header block + payload blocks) of one frame carrying payload_len bytes; 0 for an unsupported
+    configuration or length (host only, lora_b200_tx_frame_symbols)."""
+    cfg = N.Config(samp_rate=float(samp_rate), bandwidth=int(bandwidth), sf=int(sf), implicit=int(bool(implicit)), cr=int(cr),
+                   crc=int(bool(crc)), reduced_rate=int(bool(reduced_rate)), n_streams=1)
+    return int(N.lib().lora_b200_tx_frame_symbols(C.byref(cfg), int(payload_len)))
 
 
 def split_tables(blob: np.ndarray, sps: int) -> dict:

@@ -149,6 +149,45 @@ int lora_b200_tx_symbols_dev(lora_b200_decoder *d, const void *up_table, const u
 int lora_b200_tx_expand_dev(lora_b200_decoder *d, const void *base, uint32_t k, size_t n_items, float noise_sigma, uint64_t seed,
                             size_t n_streams, void *out, void *cuda_stream);
 
+/* ---- frame encoder and frame modulator on the device (the inverse of B1-B5 + chirp synthesis + sync word + SFD) ----
+ * The specification is the host encoder gr_lora_b200/tx.py: encode_frame, modulate_frame and channel.
+ *
+ * tx_frame_symbols (host only, no device needed): data symbols (the 8-symbol header block + the payload blocks) of one frame
+ *   carrying payload_len bytes under cfg's sf / cr / implicit / crc / reduced_rate; the whole frame is
+ *   (8 + 2 + 2) * sps + sps / 4 + that * sps samples.  0 for an unsupported configuration or length.
+ * tx_encode: payload bytes -> chirp shifts.  Frame f = payloads[offsets[f] .. + lengths[f]) (payloads, shifts: device;
+ *   offsets, lengths: host arrays, validated and uploaded inside the call); shifts[f * max_symbols + i] for
+ *   i < tx_frame_symbols(lengths[f]) equals tx.encode_frame(payload, sf, cr, explicit=not implicit, has_crc=crc,
+ *   reduced_rate).shifts, the rest of each row is not written.  A payload is the bytes the receiver prints after the header:
+ *   with CRC on, the caller supplies the two CRC bytes at its end (no payload CRC is computed).  Supported for SF7..SF12 and
+ *   CR 1..4 at the decoder's own settings, else LORA_B200_EUNSUPPORTED.  LORA_B200_EINVAL, before any launch, for a length
+ *   above 255 + 2 * crc, below 2 with CRC on and an explicit header, or needing more than max_symbols symbols.
+ *   One thread per (frame, data symbol).  Async on cuda_stream.
+ * tx_frames: whole streams of frames.  out = device cf32 [n_streams][n_items] (n_items even, 16-byte aligned), every sample
+ *   written once: frame samples at [start, start + frame length) of row `stream` -- 8 preamble up-chirps, 2 sync symbols,
+ *   2.25 down-chirps (conj(up)), then data symbol k = up[(n + decim * shifts[f * max_symbols + k]) mod sps] -- rotated by
+ *   e^{j 2 pi cfo_hz n / fs} (n = sample index in the row, phase reduced in double as tx_symbols does), 0 outside every
+ *   frame, then noise_sigma * (N(0,1) + j N(0,1)) added exactly as tx_expand adds it: tx_frames(sigma, seed) equals
+ *   tx_expand(base = tx_frames(0), k = n_streams, sigma, seed) bit for bit.  up_table as for tx_symbols (NULL: the decoder's
+ *   own ideal up-chirp).  frames (host) may come in any order; LORA_B200_EINVAL, before any launch, for frames that overlap
+ *   in one row, a frame that runs past n_items, stream >= n_streams or n_symbols > max_symbols.  The per-frame tables of
+ *   tx_encode / tx_frames are uploaded on cuda_stream into one buffer per decoder: a call first waits (on the host) for the
+ *   previous such call's kernel to finish. */
+typedef struct lora_b200_tx_frame {
+    uint64_t start;      /* first preamble sample, index into its row (may be odd)                                   */
+    uint32_t stream;     /* row of out                                                                               */
+    uint32_t n_symbols;  /* data symbols, read from shifts[f * max_symbols ..], f = index of this descriptor          */
+    float    cfo_hz;     /* rotation e^{j 2 pi cfo_hz n / fs}, n = sample index in the row (as tx.channel)            */
+    uint8_t  sync_word;  /* two symbols of ((sw >> 4) & 15) * 8 and (sw & 15) * 8 bins (tx.modulate_frame)            */
+    uint8_t  pad[3];
+} lora_b200_tx_frame;
+uint32_t lora_b200_tx_frame_symbols(const lora_b200_config *cfg, uint32_t payload_len);
+int lora_b200_tx_encode_dev(lora_b200_decoder *d, const uint8_t *payloads, const uint32_t *offsets, const uint32_t *lengths,
+                            size_t n_frames, uint32_t *shifts, uint32_t max_symbols, void *cuda_stream);
+int lora_b200_tx_frames_dev(lora_b200_decoder *d, const void *up_table, const lora_b200_tx_frame *frames, size_t n_frames,
+                            const uint32_t *shifts, uint32_t max_symbols, float noise_sigma, uint64_t seed, size_t n_streams,
+                            size_t n_items, void *out, void *cuda_stream);
+
 /* ---- K8: integer decode of whole code-word vectors (decode(), :567-586, B2-B4) ----
  * For each of n_vec vectors: codewords[i*stride .. +lengths[i]) -> deshuffle, dewhiten,
  * Hamming decode.  out[i*out_stride ..]; out_len[i] = bytes produced.  cr[i] = d_phdr.cr,
