@@ -7,6 +7,7 @@
 #include "k1_sf10.cuh"
 #include "k1_rows.cuh"
 #include "int_chain.cuh"
+#include "rx_stream.cuh"
 #include "tx_channel.cuh"
 #include "tx_encode.cuh"
 
@@ -92,5 +93,40 @@ uint32_t lb_emul_tx_encode(const uint8_t *payload, uint32_t len, uint32_t sf, ui
     return n;
 }
 uint32_t lb_emul_header_checksum(uint32_t length, uint32_t cr, uint32_t crc) { return lb::header_checksum(length, cr, crc); }
+
+// the stream kernels' per-step bookkeeping (rx_stream.cuh) over a recorded step sequence: state at the start of step i,
+// its metric (DETECT: autocorrelation, FIND_SFD: downchirp correlation) and its bin (-1: not demodulated).  next[i] gets
+// the state step i leads to (-1 for SYNC, PAUSE and STOP steps, which need no bookkeeping), frames the queued records
+// with their code words; returns the number of frames (at most cap are written)
+uint32_t lb_emul_rx_replay(const int32_t *states, const float *metrics, const int32_t *bins, size_t n_steps, uint32_t sf,
+                           int implicit, uint32_t cr, int crc, int reduced_rate, int32_t *next, lb::RxFrameRec *frames, uint32_t cap) {
+    lb::RxParams p;
+    memset(&p, 0, sizeof p);
+    p.sf = sf; p.n_bins_hdr = 1u << (sf - 2); p.implicit = implicit; p.reduced_rate = reduced_rate;
+    lb::RxStreamState st;
+    lb::rx_state_init(&st, (uint8_t)(((cr & 7u) << 5) | (crc ? 1u << 4 : 0u)));
+    uint32_t n_frames = 0;
+    for (size_t i = 0; i < n_steps; i++) {
+        const int s = states[i];
+        next[i] = -1;
+        if (s == LORA_B200_DETECT) next[i] = lb::rx_detect_commit(&st, 1.0f, 1.0f, 1u, metrics[i]);   // (no energies recorded)
+        else if (s == LORA_B200_FIND_SFD) next[i] = lb::rx_sfd_commit(&st, metrics[i]);
+        else if (s == LORA_B200_DECODE_HEADER || s == LORA_B200_DECODE_PAYLOAD) {
+            const lb::RxSymbolResult r = lb::rx_symbol_commit(&st, p, s == LORA_B200_DECODE_HEADER, bins[i] >= 0, bins[i]);
+            next[i] = r == lb::RX_HEADER_DONE ? LORA_B200_DECODE_PAYLOAD : r == lb::RX_FRAME_DONE ? LORA_B200_DETECT : s;
+            if (r == lb::RX_FRAME_DONE) {
+                if (n_frames < cap) {
+                    lb::RxFrameRec *fr = frames + n_frames;
+                    memcpy(fr->cw, st.demodulated, st.n_demod);
+                    lb::rx_frame_record(fr, &st, 0, implicit);
+                }
+                n_frames++;
+                lb::rx_frame_reset(&st);
+            }
+        }
+    }
+    return n_frames;
+}
+uint32_t lb_emul_rx_frame_rec_size(void) { return (uint32_t)sizeof(lb::RxFrameRec); }
 
 }

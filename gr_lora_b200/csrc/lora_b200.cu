@@ -356,7 +356,9 @@ int launch_rx_t(lora_b200_decoder *d, const RxParams &p, int grid, cudaStream_t 
     return LORA_B200_OK;
 }
 
-// SF7 at fs / bw = 8: one warp per stream (rx_warp.cuh); LORA_B200_RX=cta keeps the CTA-per-stream kernel (A/B runs)
+// SF7 at fs / bw = 8 runs rx_warp_kernel (one warp per stream); every other configuration rx_stream_kernel (one CTA per stream)
+bool rx_warp_path(const lora_b200_decoder *d) { return d->cfg.sf == 7 && d->sps == (uint32_t)RW_SPS && d->n_bins == (uint32_t)RW_N; }
+
 template <bool FFT>
 int launch_rx_warp(lora_b200_decoder *d, const RxParams &p, int n_streams, cudaStream_t st) {
     static bool attr_set[64] = {};
@@ -373,12 +375,9 @@ int launch_rx_warp(lora_b200_decoder *d, const RxParams &p, int n_streams, cudaS
 
 int launch_rx(lora_b200_decoder *d, const RxParams &p, int grid, cudaStream_t st) {
     const bool fft = d->cfg.demod == LORA_B200_DEMOD_FFT;
-    static const char *rxk = getenv("LORA_B200_RX");
-    if (d->cfg.sf == 7 && d->sps == (uint32_t)RW_SPS && d->n_bins == (uint32_t)RW_N && !(rxk && !strcmp(rxk, "cta")))
-        return fft ? launch_rx_warp<true>(d, p, grid, st) : launch_rx_warp<false>(d, p, grid, st);
+    if (rx_warp_path(d)) return fft ? launch_rx_warp<true>(d, p, grid, st) : launch_rx_warp<false>(d, p, grid, st);
     if (!fft) return launch_rx_t<7, false>(d, p, grid, st);       // SF is a run-time value on the gradient path
-    switch (d->cfg.sf) {
-    case 7: return launch_rx_t<7, true>(d, p, grid, st);
+    switch (d->cfg.sf) {                                          // (the FFT demodulator at SF7 always has sps = RW_SPS)
     case 8: return launch_rx_t<8, true>(d, p, grid, st);
     case 9: return launch_rx_t<9, true>(d, p, grid, st);
     case 10: return launch_rx_t<10, true>(d, p, grid, st);
@@ -537,12 +536,7 @@ int lora_b200_abi_version(void) { return LORA_B200_ABI_VERSION; }
 static cudaError_t init_states(lora_b200_decoder *d) {
     const uint32_t ns = d->cfg.n_streams;
     std::vector<RxStreamState> init(ns);
-    memset(init.data(), 0, sizeof(RxStreamState) * ns);
-    for (auto &s : init) {
-        s.state = LORA_B200_DETECT;                                      // :55
-        s.snr = 1.0f;                                                    // reference leaves d_snr uninitialised (oracle D4)
-        s.phdr[1] = d->phdr1_init;
-    }
+    for (auto &s : init) rx_state_init(&s, d->phdr1_init);
     return cudaMemcpy(d->d_states, init.data(), sizeof(RxStreamState) * ns, cudaMemcpyHostToDevice);
 }
 
@@ -902,8 +896,7 @@ static int work_batch_any(lora_b200_decoder *d, const void *iq, size_t elem, flo
     // groups: one launch each; a group should fill the machine about once (rx_warp_kernel: RW_WARPS streams per CTA, one CTA per
     // SM; rx_stream_kernel: one stream per CTA, two CTAs per SM), small batches stay whole.  Consecutive groups run on two
     // alternating compute streams so that the tail of one launch overlaps the head of the next.
-    const bool warp_kernel = d->cfg.sf == 7 && d->sps == (uint32_t)RW_SPS;
-    const uint32_t per_wave = (uint32_t)d->n_sms * (warp_kernel ? (uint32_t)RW_WARPS : 2u);
+    const uint32_t per_wave = (uint32_t)d->n_sms * (rx_warp_path(d) ? (uint32_t)RW_WARPS : 2u);
     // (a group of per_wave + 1 streams would take two waves: round the number of groups UP, so that the last group -- the
     // only one whose state machine is not hidden under a copy -- is a single wave)
     const uint32_t n_groups = std::max<uint32_t>(1u, std::min<uint32_t>(8u, (ns + per_wave - 1) / per_wave));

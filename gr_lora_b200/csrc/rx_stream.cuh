@@ -15,9 +15,10 @@
 //   fine_sync_block      fine_sync                          :300-338
 //   demod (gradient)     max_frequency_gradient_idx         :466-491
 //   demod (FFT)          get_shift_fft via the K1 phase functions :430-464
-// The integer tail (Gray, deinterleave, header parse) runs on thread 0 with int_chain.cuh;
-// completed frames are queued for the follow-on K8 kernel.
+// The scalar bookkeeping after each step (rx_detect_commit .. rx_frame_record below, shared with
+// rx_warp_kernel and the CPU tests) runs on thread 0; completed frames are queued for the K8 kernel.
 #pragma once
+#include <string.h>
 #include "int_chain.cuh"
 #include "k1_fft.cuh"
 #include "../../include/lora_b200.h"
@@ -93,6 +94,108 @@ struct RxParams {
     uint32_t trace_cap;
     uint32_t *trace_n;                 // per stream
 };
+
+// ---- the scalar bookkeeping of work() after each step -----------------------------------------------------------------
+// One thread per stream runs these (thread 0 of rx_stream_kernel, lane 0 of rx_warp_kernel); the host replays them in the
+// CPU tests (host_emul.cu).  The kernels differ only in how they compute each step's sums, arg()s and correlations.
+
+enum RxSymbolResult { RX_SYMBOL_NEXT = 0, RX_FRAME_DONE = 1, RX_HEADER_DONE = 2 };
+
+// decoder_impl's members as the constructor leaves them (:55-66, :72-73)
+inline void rx_state_init(RxStreamState *s, uint8_t phdr1) {
+    memset(s, 0, sizeof *s);
+    s->state = LORA_B200_DETECT;                                  // :55
+    s->snr = 1.0f;                                                // the reference leaves d_snr uninitialised (oracle D4)
+    s->phdr[1] = phdr1;
+}
+
+// detect_preamble_autocorr (:340-366) from the window sums re, im of a * conj(b) and the energies of its two halves
+LB_HD float rx_detect_corr(float re, float im, float e_a, float e_b) {
+    const float s = sqrtf(e_a * e_b);
+    return hypotf(re / s, im / s);                                // :363
+}
+
+// DETECT (:752-768): energy threshold, the 4-deep power ring, determine_snr (:377-383); returns the next state
+LB_HD int rx_detect_commit(RxStreamState *st, float e_a, float e_b, uint32_t sps, float corr) {
+    st->energy_threshold = e_b / 2.0f;                            // :357
+    const float pw = e_a / (float)sps;                            // :360 push_back on the 4-deep ring
+    if (st->pwr_n < 4) { st->pwr_queue[(st->pwr_head + st->pwr_n) & 3] = pw; st->pwr_n++; }
+    else { st->pwr_queue[st->pwr_head] = pw; st->pwr_head = (st->pwr_head + 1) & 3; }
+    if (!(corr >= 0.90f)) return LORA_B200_DETECT;                // :755
+    if (st->pwr_n >= 2) st->snr = st->pwr_queue[(st->pwr_head + st->pwr_n - 1) & 3] / st->pwr_queue[st->pwr_head];
+    st->corr_fails = 0u;
+    return LORA_B200_SYNC;
+}
+
+// FIND_SFD (:799-816): another up-chirp, which fine_sync(ifreq, -1, decim * 4) realigns to (:801-803) ...
+LB_HD bool rx_sfd_up_again(float c) { return !(c > 0.96f) && c < -0.97f; }
+// ... and the step's verdict: the SFD, another try, or back to DETECT after five failures (:805-813)
+LB_HD int rx_sfd_commit(RxStreamState *st, float c) {
+    if (c > 0.96f) return LORA_B200_PAUSE;                        // :799
+    if (!rx_sfd_up_again(c)) st->corr_fails++;                    // :805
+    return st->corr_fails > 4u ? LORA_B200_DETECT : LORA_B200_FIND_SFD;   // :808-813
+}
+
+// DECODE_HEADER / DECODE_PAYLOAD after demodulate() (:826-886): `bin` is the demodulated bin, or nothing when the implicit
+// energy gate (:861) skipped the symbol
+LB_HD RxSymbolResult rx_symbol_commit(RxStreamState *st, const RxParams &p, bool is_first, bool demodulated, int bin) {
+    bool block_done = false;
+    uint32_t cr = st->phdr[1] >> 5;
+    if (demodulated) {
+        const bool reduced = is_first || p.reduced_rate;          // :495
+        uint32_t b = (uint32_t)bin;
+        if (reduced) b = reduce_bin(b, p.n_bins_hdr);             // :507-509
+        if (st->n_words < 8u) st->words[st->n_words] = gray_encode(b);   // :512,:517
+        st->n_words++;
+        if (st->n_words == 4u + (is_first ? 4u : cr)) {          // :521
+            const uint32_t ppm = reduced ? p.sf - 2u : p.sf;
+            uint8_t cwb[16];
+            deinterleave_block(st->words, st->n_words, ppm, cwb);
+            for (uint32_t k = 0; k < ppm; k++)
+                if (st->n_demod < (uint32_t)LB_MAX_CW) st->demodulated[st->n_demod++] = cwb[k];
+            st->n_words = 0;
+            block_done = true;
+        }
+    } else {
+        st->payload_symbols = 0;                                  // :862-864
+        st->payload_length = st->n_demod / 2u;
+    }
+    if (is_first) {
+        if (!block_done) return RX_SYMBOL_NEXT;
+        if (p.implicit) {
+            st->payload_symbols = 1;                              // :829
+        } else {
+            const uint32_t nb = decode_len_bytes(6u, cr);         // decode(true) :831
+            uint8_t hb[4] = {0, 0, 0, 0};
+            for (uint32_t k = 0; k < nb && k < 4u; k++) hb[k] = decode_byte(st->demodulated, st->n_demod, 1, cr, k);
+            st->n_hdr_print = (uint8_t)(nb < 4u ? nb : 4u);       // :832 prints d_decoded
+            for (int k = 0; k < 4; k++) st->hdr_print[k] = hb[k];
+            const uint32_t erase = st->n_demod < 5u ? st->n_demod : 5u;   // :632
+            for (uint32_t k = erase; k < st->n_demod; k++) st->demodulated[k - erase] = st->demodulated[k];
+            st->n_demod -= erase;
+            st->phdr[0] = hb[0]; st->phdr[1] = hb[1]; st->phdr[2] = hb[2];   // :833
+            if ((st->phdr[1] >> 5) > 4) st->phdr[1] = (uint8_t)((st->phdr[1] & 0x1f) | (4u << 5));   // :834-835
+            cr = st->phdr[1] >> 5;
+            st->payload_length = st->phdr[0] + 2u * ((st->phdr[1] >> 4) & 1u);   // :838
+            st->payload_symbols = payload_symbols(st->payload_length, cr, p.sf, p.reduced_rate);
+        }
+        return RX_HEADER_DONE;                                    // -> DECODE_PAYLOAD, :853
+    }
+    if (block_done && !p.implicit) st->payload_symbols -= (int32_t)(4u + cr);   // :866-867
+    return st->payload_symbols <= 0 ? RX_FRAME_DONE : RX_SYMBOL_NEXT;          // :870
+}
+
+// the queued frame record of a completed frame (decode(false) and msg_lora_frame follow in K8), all but its code words
+LB_HD void rx_frame_record(RxFrameRec *fr, RxStreamState *st, uint32_t stream, int implicit) {
+    fr->stream = stream; fr->seq = st->frame_seq++; fr->n_cw = st->n_demod; fr->cr = st->phdr[1] >> 5;
+    fr->payload_length = st->payload_length; fr->snr = st->snr;
+    fr->phdr[0] = st->phdr[0]; fr->phdr[1] = st->phdr[1]; fr->phdr[2] = st->phdr[2];
+    fr->n_hdr_print = implicit ? 0 : st->n_hdr_print;
+    for (int k = 0; k < 4; k++) fr->hdr_print[k] = st->hdr_print[k];
+}
+
+// after the frame (:875-880): back to DETECT with empty buffers
+LB_HD void rx_frame_reset(RxStreamState *st) { st->n_words = 0; st->n_demod = 0; }
 
 #ifdef __CUDACC__
 
@@ -210,6 +313,37 @@ LB_D int fine_sync_block(const RxParams &p, const float *scr, int bin_idx, int s
     return -lag;                                                  // :321
 }
 
+// A5 max_frequency_gradient_idx (:466-491) on the instantaneous frequency ifq[0, N * decim); avg takes N floats
+LB_D int grad_demod_block(const float *ifq, float *avg, int N, int decim, RxShared &sh) {
+    for (int i = threadIdx.x; i < N; i += RX_THREADS) {
+        float acc = 0.0f;
+        for (int k = 0; k < decim; k++) acc += ifq[i * decim + k];    // :475
+        avg[i] = acc / (float)decim;                              // :476
+    }
+    __syncthreads();
+    unsigned long long best = 0ull;
+    for (int i = 1 + threadIdx.x; i < N; i += RX_THREADS) {
+        const float g = avg[i - 1] - avg[i];                      // :483
+        if (g > 0.1f) { const unsigned long long k = pack_key(g, (uint32_t)i); best = k > best ? k : best; }
+    }
+    best = block_max_key(best, sh);
+    const int max_index = best ? (int)key_idx(best) + 1 : 0;       // :486
+    return (N - max_index) % N;                                   // :490
+}
+
+// experimental_determine_cfo(&input[i], sps) (:730-738; the reference's call at :774 is commented out) on xi = &input[i]:
+// instantaneous frequency of samples * down-chirp at the hard-coded index 256, in Hz.  Bookkeeping thread only.
+LB_D void rx_cfo_estimate(const RxParams &p, RxStreamState *st, const float2 *xi) {
+    if (p.sps <= 257) return;
+    const float2 m0 = cmul(xi[256], __ldg(p.down + 256)), m1 = cmul(xi[257], __ldg(p.down + 257));
+    const float p1 = atan2f(m0.y, m0.x);
+    float p2 = atan2f(m1.y, m1.x);
+    while (p2 - p1 > LB_PI_BELOW) p2 = (float)((double)p2 - 6.283185307179586);
+    while (p2 - p1 < -LB_PI_BELOW) p2 = (float)((double)p2 + 6.283185307179586);
+    st->cfo_est = (float)((double)(p2 - p1) / (2.0 * 3.14159265358979323846) * (double)p.samples_per_second);
+    st->cfo_count++;
+}
+
 template <int SF, bool FFT>
 __global__ void __launch_bounds__(RX_THREADS)
 rx_stream_kernel(RxParams p) {
@@ -247,21 +381,9 @@ rx_stream_kernel(RxParams p) {
             }
             block_sum<4>(v, sh);
             if (tid == 0) {
-                st->energy_threshold = v[3] / 2.0f;               // :357
-                const float pw = v[2] / (float)p.sps;             // :360 push_back on the 4-deep ring
-                if (st->pwr_n < 4) { st->pwr_queue[(st->pwr_head + st->pwr_n) & 3] = pw; st->pwr_n++; }
-                else { st->pwr_queue[st->pwr_head] = pw; st->pwr_head = (st->pwr_head + 1) & 3; }
-                const float s = sqrtf(v[2] * v[3]);
-                const float corr = hypotf(v[0] / s, v[1] / s);    // :363
-                sh.metric = corr;
-                if (corr >= 0.90f) {                              // :755
-                    if (st->pwr_n >= 2)                           // determine_snr :377-383
-                        st->snr = st->pwr_queue[(st->pwr_head + st->pwr_n - 1) & 3] / st->pwr_queue[st->pwr_head];
-                    st->corr_fails = 0u;
-                    sh.state = LORA_B200_SYNC;
-                } else {
-                    sh.consumed = sps;
-                }
+                sh.metric = rx_detect_corr(v[0], v[1], v[2], v[3]);
+                sh.state = rx_detect_commit(st, v[2], v[3], p.sps, sh.metric);
+                if (sh.state == LORA_B200_DETECT) sh.consumed = sps;
             }
             break;
         }
@@ -287,18 +409,7 @@ rx_stream_kernel(RxParams p) {
                 sh.metric = best ? key_mag2(best) : 0.0f;
                 sh.consumed = best ? (int)key_idx(best) : 0;      // :780 consume_each(i)
                 sh.state = LORA_B200_FIND_SFD;
-                if (p.cfo_estimate && sps > 257) {
-                    // experimental_determine_cfo(&input[i], sps) (:730-738, call site :774 commented out in the reference):
-                    // instantaneous frequency of samples * downchirp at the hard-coded index 256, in Hz
-                    const float2 *xi = x + sh.consumed;
-                    const float2 m0 = cmul(xi[256], __ldg(p.down + 256)), m1 = cmul(xi[257], __ldg(p.down + 257));
-                    const float p1 = atan2f(m0.y, m0.x);
-                    float p2 = atan2f(m1.y, m1.x);
-                    while (p2 - p1 > LB_PI_BELOW) p2 = (float)((double)p2 - 6.283185307179586);
-                    while (p2 - p1 < -LB_PI_BELOW) p2 = (float)((double)p2 + 6.283185307179586);
-                    st->cfo_est = (float)((double)(p2 - p1) / (2.0 * 3.14159265358979323846) * (double)p.samples_per_second);
-                    st->cfo_count++;
-                }
+                if (p.cfo_estimate) rx_cfo_estimate(p, st, x + sh.consumed);
             }
             break;
         }
@@ -319,16 +430,10 @@ rx_stream_kernel(RxParams p) {
             const float sd = sqrtf(v2[0] / (float)to_idx) * p.down_ifreq_sd;   // :288-289
             const float c = v2[1] / sd / (float)to_idx;           // :291-295
             int fs = 0;
-            const bool up_again = !(c > 0.96f) && (c < -0.97f);
-            if (up_again) fs = fine_sync_block(p, scr, -1, (int)p.decim * 4, sh);   // :803
+            if (rx_sfd_up_again(c)) fs = fine_sync_block(p, scr, -1, (int)p.decim * 4, sh);   // :803
             if (tid == 0) {
                 sh.metric = c;
-                if (c > 0.96f) {
-                    sh.state = LORA_B200_PAUSE;                   // :799
-                } else {
-                    if (!up_again) st->corr_fails++;              // :805
-                    if (st->corr_fails > 4u) sh.state = LORA_B200_DETECT;   // :808-813
-                }
+                sh.state = rx_sfd_commit(st, c);
                 sh.fine_sync = fs;
                 sh.consumed = sps + fs;                           // :816
             }
@@ -370,23 +475,8 @@ rx_stream_kernel(RxParams p) {
                     }
                     best = block_max_key(best, sh);
                     bin = ((int)key_idx(best) + N - 1) % N;       // gradient-index convention (SURVEY A7)
-                } else {                                          // A5 :466-491
-                    float *avg = scr + 2 * sps;
-                    const int decim = (int)p.decim;
-                    for (int i = tid; i < N; i += RX_THREADS) {
-                        float acc = 0.0f;
-                        for (int k = 0; k < decim; k++) acc += scr[i * decim + k];   // :475
-                        avg[i] = acc / (float)decim;              // :476
-                    }
-                    __syncthreads();
-                    unsigned long long best = 0ull;
-                    for (int i = 1 + tid; i < N; i += RX_THREADS) {
-                        const float g = avg[i - 1] - avg[i];      // :483
-                        if (g > 0.1f) { const unsigned long long k = pack_key(g, (uint32_t)i); best = k > best ? k : best; }
-                    }
-                    best = block_max_key(best, sh);
-                    const int max_index = best ? (int)key_idx(best) + 1 : 0;   // :486
-                    bin = (N - max_index) % N;                    // :490
+                } else {
+                    bin = grad_demod_block(scr, scr + 2 * sps, N, (int)p.decim, sh);
                 }
                 if (p.enable_fine_sync) {                         // :501-502
                     int s = (int)p.decim / 4; if (s < 2) s = 2;
@@ -394,53 +484,11 @@ rx_stream_kernel(RxParams p) {
                 }
             }
             if (tid == 0) {
-                bool block_done = false;
-                uint32_t cr = st->phdr[1] >> 5;
-                if (do_demod) {
-                    const bool reduced = is_first || p.reduced_rate;      // :495
-                    uint32_t b = (uint32_t)bin;
-                    if (reduced) b = reduce_bin(b, p.n_bins_hdr);  // :507-509
-                    st->words[st->n_words++] = gray_encode(b);    // :512,:517
-                    if (st->n_words == 4u + (is_first ? 4u : cr)) {       // :521
-                        const uint32_t ppm = reduced ? p.sf - 2u : p.sf;
-                        uint8_t cwb[16];
-                        deinterleave_block(st->words, st->n_words, ppm, cwb);
-                        for (uint32_t k = 0; k < ppm; k++)
-                            if (st->n_demod < (uint32_t)LB_MAX_CW) st->demodulated[st->n_demod++] = cwb[k];
-                        st->n_words = 0;
-                        block_done = true;
-                    }
-                } else {
-                    st->payload_symbols = 0;                      // :862-864
-                    st->payload_length = st->n_demod / 2u;
-                }
-                if (is_first) {
-                    if (block_done) {
-                        if (p.implicit) {
-                            st->payload_symbols = 1;              // :829
-                        } else {
-                            const uint32_t nb = decode_len_bytes(6u, cr);            // decode(true) :831
-                            uint8_t hb[4] = {0, 0, 0, 0};
-                            for (uint32_t k = 0; k < nb && k < 4u; k++) hb[k] = decode_byte(st->demodulated, st->n_demod, 1, cr, k);
-                            st->n_hdr_print = (uint8_t)(nb < 4u ? nb : 4u);          // :832 prints d_decoded
-                            for (int k = 0; k < 4; k++) st->hdr_print[k] = hb[k];
-                            const uint32_t erase = st->n_demod < 5u ? st->n_demod : 5u;   // :632
-                            for (uint32_t k = erase; k < st->n_demod; k++) st->demodulated[k - erase] = st->demodulated[k];
-                            st->n_demod -= erase;
-                            st->phdr[0] = hb[0]; st->phdr[1] = hb[1]; st->phdr[2] = hb[2];   // :833
-                            if ((st->phdr[1] >> 5) > 4) st->phdr[1] = (uint8_t)((st->phdr[1] & 0x1f) | (4u << 5));   // :834-835
-                            cr = st->phdr[1] >> 5;
-                            st->payload_length = st->phdr[0] + 2u * ((st->phdr[1] >> 4) & 1u);   // :838
-                            st->payload_symbols = payload_symbols(st->payload_length, cr, p.sf, p.reduced_rate);
-                        }
-                        sh.state = LORA_B200_DECODE_PAYLOAD;      // :853
-                    }
-                } else {
-                    if (block_done && !p.implicit) st->payload_symbols -= (int32_t)(4u + cr);   // :866-867
-                    if (st->payload_symbols <= 0) {               // :870
-                        sh.flag = 1;
-                        sh.frame_slot = atomicAdd(p.n_frames, 1u);
-                    }
+                const RxSymbolResult r = rx_symbol_commit(st, p, is_first, do_demod, bin);
+                if (r == RX_HEADER_DONE) sh.state = LORA_B200_DECODE_PAYLOAD;
+                if (r == RX_FRAME_DONE) {
+                    sh.flag = 1;
+                    sh.frame_slot = atomicAdd(p.n_frames, 1u);
                 }
                 sh.bin = bin;
                 sh.fine_sync = fs;
@@ -453,18 +501,12 @@ rx_stream_kernel(RxParams p) {
                     RxFrameRec *fr = p.frames + slot;
                     const uint32_t n = st->n_demod;
                     for (uint32_t k = tid; k < n; k += RX_THREADS) fr->cw[k] = st->demodulated[k];
-                    if (tid == 0) {
-                        fr->stream = stream; fr->seq = st->frame_seq++; fr->n_cw = n; fr->cr = st->phdr[1] >> 5;
-                        fr->payload_length = st->payload_length; fr->snr = st->snr;
-                        fr->phdr[0] = st->phdr[0]; fr->phdr[1] = st->phdr[1]; fr->phdr[2] = st->phdr[2];
-                        fr->n_hdr_print = p.implicit ? 0 : st->n_hdr_print;
-                        for (int k = 0; k < 4; k++) fr->hdr_print[k] = st->hdr_print[k];
-                    }
+                    if (tid == 0) rx_frame_record(fr, st, stream, p.implicit);
                 }
                 __syncthreads();
                 if (tid == 0) {
                     sh.state = LORA_B200_DETECT;                  // :875-880
-                    st->n_words = 0; st->n_demod = 0;
+                    rx_frame_reset(st);
                     sh.frames_here++;
                 }
             }
@@ -500,25 +542,10 @@ k2_gradient_kernel(const float2 *__restrict__ iq, size_t n_symbols, uint32_t sps
                    float *__restrict__ scratch /* gridDim.x * (sps + n_bins) */, uint32_t *__restrict__ bins) {
     __shared__ RxShared sh;
     float *scr = scratch + (size_t)blockIdx.x * (sps + n_bins);
-    float *avg = scr + sps;
     for (size_t sym = blockIdx.x; sym < n_symbols; sym += gridDim.x) {
         ifreq_block(iq + sym * sps, scr, (int)sps);
-        for (int i = threadIdx.x; i < (int)n_bins; i += RX_THREADS) {
-            float acc = 0.0f;
-            for (uint32_t k = 0; k < decim; k++) acc += scr[i * decim + k];
-            avg[i] = acc / (float)decim;
-        }
-        __syncthreads();
-        unsigned long long best = 0ull;
-        for (int i = 1 + threadIdx.x; i < (int)n_bins; i += RX_THREADS) {
-            const float g = avg[i - 1] - avg[i];
-            if (g > 0.1f) { const unsigned long long k = pack_key(g, (uint32_t)i); best = k > best ? k : best; }
-        }
-        best = block_max_key(best, sh);
-        if (threadIdx.x == 0) {
-            const int max_index = best ? (int)key_idx(best) + 1 : 0;
-            bins[sym] = (uint32_t)(((int)n_bins - max_index) % (int)n_bins);
-        }
+        const int bin = grad_demod_block(scr, scr + sps, (int)n_bins, (int)decim, sh);
+        if (threadIdx.x == 0) bins[sym] = (uint32_t)bin;
         __syncthreads();
     }
 }

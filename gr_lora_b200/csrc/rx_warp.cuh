@@ -21,8 +21,10 @@
 //     issue slots 42 % active, stalls wait 24 %, long scoreboard 18 %); 4 700 warp
 //     instructions per window, a third of them the per-sample arg() and unwrap.  The kernel alone runs 4096 streams x 256
 //     windows in 12 ms (8.7e7 windows/s).
-// Same observable behaviour as rx_stream_kernel: frames, consume amounts, per-step trace.  Other SFs and sample rates use
-// rx_stream_kernel.
+// What only one thread does after a step -- the decoder_impl members, the integer tail, the frame record -- is the
+// rx_stream_kernel's code too: lane 0 calls the shared bookkeeping functions of rx_stream.cuh (rx_detect_commit ..
+// rx_frame_reset) and the warp learns the next state by a shuffle.  Same observable behaviour as rx_stream_kernel: frames,
+// consume amounts, per-step trace.  Other SFs and sample rates use rx_stream_kernel (rx_warp_path(), lora_b200.cu).
 #pragma once
 #include "rx_stream.cuh"
 #include "k1_warp.cuh"
@@ -298,21 +300,10 @@ rx_warp_kernel(RxParams p) {
                 v3 += b.x * b.x + b.y * b.y;
             }
             v0 = warp_sum(v0); v1 = warp_sum(v1); v2 = warp_sum(v2); v3 = warp_sum(v3);
-            const float s = sqrtf(v2 * v3);
-            const float corr = hypotf(v0 / s, v1 / s);            // :363
-            metric = corr;
-            if (lane == 0) {
-                st->energy_threshold = v3 / 2.0f;                 // :357
-                const float pw = v2 / (float)sps;                 // :360 push_back on the 4-deep ring
-                if (st->pwr_n < 4) { st->pwr_queue[(st->pwr_head + st->pwr_n) & 3] = pw; st->pwr_n++; }
-                else { st->pwr_queue[st->pwr_head] = pw; st->pwr_head = (st->pwr_head + 1) & 3; }
-                if (corr >= 0.90f) {                              // :755
-                    if (st->pwr_n >= 2)                           // determine_snr :377-383
-                        st->snr = st->pwr_queue[(st->pwr_head + st->pwr_n - 1) & 3] / st->pwr_queue[st->pwr_head];
-                    st->corr_fails = 0u;
-                }
-            }
-            if (corr >= 0.90f) next_state = LORA_B200_SYNC; else consumed = sps;
+            metric = rx_detect_corr(v0, v1, v2, v3);
+            if (lane == 0) next_state = rx_detect_commit(st, v2, v3, sps, metric);
+            next_state = __shfl_sync(0xffffffffu, next_state, 0);
+            if (next_state == LORA_B200_DETECT) consumed = sps;
             break;
         }
         case LORA_B200_SYNC: {                                    // :770-783, A9 :392-413
@@ -323,15 +314,7 @@ rx_warp_kernel(RxParams p) {
             metric = best ? key_mag2(best) : 0.0f;
             consumed = best ? (int)key_idx(best) : 0;             // :780 consume_each(i)
             next_state = LORA_B200_FIND_SFD;
-            if (p.cfo_estimate && lane == 0) {                    // experimental_determine_cfo(&input[i], sps), :730-738,774
-                const float2 m0 = cmul(x[consumed + 256], __ldg(p.down + 256)), m1 = cmul(x[consumed + 257], __ldg(p.down + 257));
-                const float p1 = atan2f(m0.y, m0.x);
-                float p2 = atan2f(m1.y, m1.x);
-                while (p2 - p1 > LB_PI_BELOW) p2 = (float)((double)p2 - 6.283185307179586);
-                while (p2 - p1 < -LB_PI_BELOW) p2 = (float)((double)p2 + 6.283185307179586);
-                st->cfo_est = (float)((double)(p2 - p1) / (2.0 * 3.14159265358979323846) * (double)p.samples_per_second);
-                st->cfo_count++;
-            }
+            if (p.cfo_estimate && lane == 0) rx_cfo_estimate(p, st, x + consumed);
             break;
         }
         case LORA_B200_FIND_SFD: {                                // :785-818, A10
@@ -354,18 +337,10 @@ rx_warp_kernel(RxParams p) {
             q0 = warp_sum(q0); q1 = warp_sum(q1);
             const float sd = sqrtf(q0 / (float)to_idx) * p.down_ifreq_sd;   // :288-289
             const float cc = q1 / sd / (float)to_idx;             // :291-295
-            const bool up_again = !(cc > 0.96f) && (cc < -0.97f);
-            if (up_again) fine = rw_fine_sync63(ifq, sm.up_ifreq_v, reinterpret_cast<float *>(ws.win), lane);   // :803, fine_sync(ifreq, -1, decim * 4)
+            if (rx_sfd_up_again(cc)) fine = rw_fine_sync63(ifq, sm.up_ifreq_v, reinterpret_cast<float *>(ws.win), lane);   // :803, fine_sync(ifreq, -1, decim * 4)
             metric = cc;
-            if (cc > 0.96f) {
-                next_state = LORA_B200_PAUSE;                     // :799
-            } else {
-                unsigned int fails = st->corr_fails;
-                if (!up_again) fails++;                           // :805
-                __syncwarp();
-                if (lane == 0) st->corr_fails = fails;
-                if (fails > 4u) next_state = LORA_B200_DETECT;    // :808-813
-            }
+            if (lane == 0) next_state = rx_sfd_commit(st, cc);
+            next_state = __shfl_sync(0xffffffffu, next_state, 0);
             consumed = sps + fine;                                // :816
             break;
         }
@@ -441,76 +416,23 @@ rx_warp_kernel(RxParams p) {
             int flag = 0;
             unsigned int frame_slot = 0;
             if (lane == 0) {
-                bool block_done = false;
-                uint32_t cr = st->phdr[1] >> 5;
-                if (do_demod) {
-                    const bool reduced = is_first || p.reduced_rate;      // :495
-                    uint32_t b = (uint32_t)bin;
-                    if (reduced) b = reduce_bin(b, p.n_bins_hdr);  // :507-509
-                    if (st->n_words < 8u) st->words[st->n_words] = gray_encode(b);    // :512,:517
-                    st->n_words++;
-                    if (st->n_words == 4u + (is_first ? 4u : cr)) {       // :521
-                        const uint32_t ppm = reduced ? p.sf - 2u : p.sf;
-                        uint8_t cwb[16];
-                        deinterleave_block(st->words, st->n_words, ppm, cwb);
-                        for (uint32_t k = 0; k < ppm; k++)
-                            if (st->n_demod < (uint32_t)LB_MAX_CW) st->demodulated[st->n_demod++] = cwb[k];
-                        st->n_words = 0;
-                        block_done = true;
-                    }
-                } else {
-                    st->payload_symbols = 0;                      // :862-864
-                    st->payload_length = st->n_demod / 2u;
-                }
-                if (is_first) {
-                    if (block_done) {
-                        if (p.implicit) {
-                            st->payload_symbols = 1;              // :829
-                        } else {
-                            const uint32_t nb = decode_len_bytes(6u, cr);            // decode(true) :831
-                            uint8_t hb[4] = {0, 0, 0, 0};
-                            for (uint32_t k = 0; k < nb && k < 4u; k++) hb[k] = decode_byte(st->demodulated, st->n_demod, 1, cr, k);
-                            st->n_hdr_print = (uint8_t)(nb < 4u ? nb : 4u);          // :832 prints d_decoded
-                            for (int k = 0; k < 4; k++) st->hdr_print[k] = hb[k];
-                            const uint32_t erase = st->n_demod < 5u ? st->n_demod : 5u;   // :632
-                            for (uint32_t k = erase; k < st->n_demod; k++) st->demodulated[k - erase] = st->demodulated[k];
-                            st->n_demod -= erase;
-                            st->phdr[0] = hb[0]; st->phdr[1] = hb[1]; st->phdr[2] = hb[2];   // :833
-                            if ((st->phdr[1] >> 5) > 4) st->phdr[1] = (uint8_t)((st->phdr[1] & 0x1f) | (4u << 5));   // :834-835
-                            cr = st->phdr[1] >> 5;
-                            st->payload_length = st->phdr[0] + 2u * ((st->phdr[1] >> 4) & 1u);   // :838
-                            st->payload_symbols = payload_symbols(st->payload_length, cr, p.sf, p.reduced_rate);
-                        }
-                        flag = 2;                                 // -> DECODE_PAYLOAD, :853
-                    }
-                } else {
-                    if (block_done && !p.implicit) st->payload_symbols -= (int32_t)(4u + cr);   // :866-867
-                    if (st->payload_symbols <= 0) {               // :870
-                        flag = 1;
-                        frame_slot = atomicAdd(p.n_frames, 1u);
-                    }
-                }
+                flag = rx_symbol_commit(st, p, is_first, do_demod, bin);
+                if (flag == RX_FRAME_DONE) frame_slot = atomicAdd(p.n_frames, 1u);
             }
             __syncwarp();                                         // lane 0's stores to the decoder state above -> every lane's reads below
             flag = __shfl_sync(0xffffffffu, flag, 0);
             frame_slot = __shfl_sync(0xffffffffu, frame_slot, 0);
-            if (flag == 2) next_state = LORA_B200_DECODE_PAYLOAD;
+            if (flag == RX_HEADER_DONE) next_state = LORA_B200_DECODE_PAYLOAD;
             consumed = sps + fine;                                // :856,:883
-            if (flag == 1) {                                      // decode(false) + msg_lora_frame happen in K8
+            if (flag == RX_FRAME_DONE) {                          // decode(false) + msg_lora_frame happen in K8
                 if (frame_slot < p.frame_cap) {
                     RxFrameRec *fr = p.frames + frame_slot;
                     const uint32_t n = st->n_demod;
                     for (uint32_t k = lane; k < n; k += 32) fr->cw[k] = st->demodulated[k];
-                    if (lane == 0) {
-                        fr->stream = stream; fr->seq = st->frame_seq++; fr->n_cw = n; fr->cr = st->phdr[1] >> 5;
-                        fr->payload_length = st->payload_length; fr->snr = st->snr;
-                        fr->phdr[0] = st->phdr[0]; fr->phdr[1] = st->phdr[1]; fr->phdr[2] = st->phdr[2];
-                        fr->n_hdr_print = p.implicit ? 0 : st->n_hdr_print;
-                        for (int k = 0; k < 4; k++) fr->hdr_print[k] = st->hdr_print[k];
-                    }
+                    if (lane == 0) rx_frame_record(fr, st, stream, p.implicit);
                 }
                 __syncwarp();
-                if (lane == 0) { st->n_words = 0; st->n_demod = 0; }     // :875-880
+                if (lane == 0) rx_frame_reset(st);                // :875-880
                 next_state = LORA_B200_DETECT;
                 frames_here++;
             }

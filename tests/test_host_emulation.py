@@ -8,7 +8,7 @@ from pathlib import Path
 import numpy as np
 import pytest
 
-from conftest import twiddle_table
+from conftest import FRAME_CASES, case_decoder_args, make_case_iq, twiddle_table
 from gr_lora_b200 import build as B, tx, whitening
 
 GOLD = json.loads((Path(__file__).parent / "golden" / "golden.json").read_text())
@@ -36,6 +36,10 @@ def emul():
     L.lb_emul_payload_symbols.argtypes = [C.c_uint32, C.c_uint32, C.c_uint32, C.c_int]
     L.lb_emul_atan2f.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t]
     L.lb_emul_philox4x32_10.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p]
+    L.lb_emul_rx_replay.restype = C.c_uint32
+    L.lb_emul_rx_replay.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_uint32, C.c_int, C.c_uint32, C.c_int, C.c_int,
+                                    C.c_void_p, C.c_void_p, C.c_uint32]
+    L.lb_emul_rx_frame_rec_size.restype = C.c_uint32
     return L
 
 
@@ -161,6 +165,68 @@ def test_tx_inverts_the_integer_chain(emul):
                 assert got == payload
             else:
                 assert got == payload
+
+
+# lb::RxFrameRec (rx_stream.cuh)
+FRAME_REC = np.dtype([("stream", "<u4"), ("seq", "<u4"), ("n_cw", "<u4"), ("cr", "<u4"), ("payload_length", "<u4"), ("snr", "<f4"),
+                      ("phdr", "u1", 3), ("n_hdr_print", "u1"), ("hdr_print", "u1", 4), ("cw", "u1", 1024)])
+
+
+def _hex(v):
+    return "".join(f" {int(b):02x}" for b in v)
+
+
+@pytest.mark.parametrize("case", FRAME_CASES, ids=[c[0] for c in FRAME_CASES])
+def test_rx_bookkeeping_replays_the_oracle(emul, oracle, case):
+    """The stream kernels' bookkeeping after each step (rx_stream.cuh: DETECT and FIND_SFD verdicts, reduced-rate fold,
+    Gray, deinterleave, header parse with the erase of 5, payload countdown, frame record) replayed on the host over the
+    oracle's steps (state, metric, bin): every next state is the oracle's, and the frames' header and payload bytes
+    (decoded by decode_byte, as K8 does) and printed lines are the oracle's.  The SNR byte is not compared: the steps
+    carry no energies."""
+    x, _, _ = make_case_iq(case)
+    _replay_matches_oracle(emul, oracle, x, case_decoder_args(case))
+
+
+def test_rx_bookkeeping_clamps_the_header_cr(emul, oracle):
+    """A header whose CR field reads 7 (the reference never checks the header checksum): the bookkeeping clamps it to 4
+    (:834-835) as the oracle does, and the CR 4/8 payload after it decodes."""
+    payload = bytes.fromhex("0badc0ffee0102")
+    fs = tx.encode_frame(payload, 8, 4, has_crc=True, header=tx.header_bytes(len(payload) - 2, 7, 1))
+    x = tx.channel([tx.modulate_frame(fs, 8)] * 2, sf=8, snr_db=40.0, seed=23)
+    frames = _replay_matches_oracle(emul, oracle, x, dict(sf=8, implicit=False, cr=4, crc=True, reduced_rate=False))
+    assert [f[16] >> 5 for f in frames] == [4, 4] and [f[18:] for f in frames] == [payload] * 2
+
+
+def _replay_matches_oracle(emul, oracle, x, args):
+    sf, implicit, cr, crc, rr = args["sf"], args["implicit"], args["cr"], args["crc"], args["reduced_rate"]
+    d = oracle.Decoder(**args)
+    _, steps = d.run(x)
+    want = d.frames()
+    states = np.ascontiguousarray(steps["state"])
+    metrics = np.ascontiguousarray(steps["metric"])
+    bins = np.ascontiguousarray(steps["bin"])
+    nxt = np.empty(states.size, np.int32)
+    recs = np.zeros(4, FRAME_REC)
+    assert emul.lb_emul_rx_frame_rec_size() == FRAME_REC.itemsize
+    k = emul.lb_emul_rx_replay(states.ctypes.data, metrics.ctypes.data, bins.ctypes.data, states.size, sf, int(implicit), cr,
+                               int(crc), int(rr), nxt.ctypes.data, recs.ctypes.data, len(recs))
+    after = np.append(states[1:], d.state)
+    replayed = nxt >= 0
+    assert np.count_nonzero(np.isin(states[replayed], (4, 5))) > 0
+    assert np.array_equal(nxt[replayed], after[replayed])
+    assert k == len(want) == 2
+    text = ""
+    for r, f in zip(recs[:k], want):
+        cw = np.ascontiguousarray(r["cw"][:r["n_cw"]])
+        dec = np.zeros(1024, np.uint8)
+        m = emul.lb_emul_decode(cw.ctypes.data, int(r["n_cw"]), 0, int(r["cr"]), dec.ctypes.data, dec.size)
+        plen = int(r["payload_length"])
+        payload = bytes(dec[:min(m, plen)]) + bytes(max(0, plen - m))      # missing bytes read 0 (oracle D5)
+        assert bytes(r["phdr"]) + payload == f[15:]
+        text += _hex(r["hdr_print"][:r["n_hdr_print"]]) + _hex(payload)
+        text += " (" + "".join(chr(b) for b in payload if 32 <= b <= 126) + ")\n"
+    assert d.stdout.endswith(text)
+    return want
 
 
 @pytest.mark.parametrize("sf", [11, 12])
