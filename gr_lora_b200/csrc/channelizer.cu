@@ -10,6 +10,7 @@
 // Here every channel of channel_list is produced (one FIR bank launch, the wideband input is staged in
 // shared memory once per tile and reused by all channels), output stays in HBM for the decoder.
 #include "../../include/lora_b200.h"
+#include "device_once.h"
 #include <cuda_runtime.h>
 #include <cmath>
 #include <cstdio>
@@ -211,12 +212,10 @@ int lora_b200_channelizer_work_dev(lora_b200_channelizer *c, const void *in_dev,
     cudaStreamSynchronize(st);                       // dph is a stack vector
     const uint32_t seg = (CH_TN - 1) * c->decimation + c->ntaps;
     const size_t smem = sizeof(float2) * ((size_t)seg + (size_t)CH_CT * c->ntaps);
-    static bool attr_set[64] = {};
-    if (smem > 48 * 1024 && !attr_set[c->device & 63]) {
-        if (cudaFuncSetAttribute(chan_fir_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024) != cudaSuccess)
-            return cfail(c, LORA_B200_ECUDA, "channelizer_work: shared memory attribute");
-        attr_set[c->device & 63] = true;
-    }
+    static lb::DeviceOnce once;
+    if (smem > 48 * 1024 &&
+        once(c->device, [] { return cudaFuncSetAttribute(chan_fir_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024); }) != cudaSuccess)
+        return cfail(c, LORA_B200_ECUDA, "channelizer_work: shared memory attribute");
     if (smem > 200 * 1024) return cfail(c, LORA_B200_EUNSUPPORTED, "channelizer_work: filter too long for one tile");
     dim3 grid((unsigned)((no + CH_TN - 1) / CH_TN), (c->n_channels + CH_CT - 1) / CH_CT);
     chan_fir_kernel<<<grid, CH_TN, smem, st>>>(c->d_hist, (const float2 *)in_dev, n_in, c->decimation, c->ntaps, c->d_ctaps,

@@ -37,7 +37,6 @@ int lb_k1_emulate_warp_sf7(const float2 *x, size_t n_symbols, const float2 *chir
 int lb_k1_emulate_group(int sf, const float2 *x, size_t n_symbols, const float2 *chirp, const float2 *tw, uint32_t *bins, float *mags) {
     lb::K1Args a{x, chirp, tw, n_symbols};
     switch (sf) {
-    case 7: lb::g_emulate<7>(a, bins, mags); break;
     case 8: lb::g_emulate<8>(a, bins, mags); break;
     case 9: lb::g_emulate<9>(a, bins, mags); break;
     case 10: lb::s10_emulate(a, bins, mags); break;

@@ -85,6 +85,25 @@ LB_HD float2 k1_ld_table(const float2 *p) {
 #endif
 }
 
+// Horner evaluation of the twiddled branch sum sum_r w^r g[r] over NB branches, g[NB-1] first
+template <int NB>
+LB_HD float2 horner(const float2 *g, float2 w) {
+    float2 acc = g[NB - 1];
+#pragma unroll
+    for (int r = NB - 2; r >= 0; r--) acc = cfma(acc, w, g[r]);
+    return acc;
+}
+// tmp[N/2] += F[N/2] (:450): bin N/2 is summed a second time with the conjugate twiddle, over gq (its branches, or what
+// stands for them)
+template <int NB>
+LB_HD float2 plus_quirk(float2 acc, const float2 *gq, float2 w) { return cadd(acc, horner<NB>(gq, cconj(w))); }
+
+// result of symbol i from its argmax key: the bin and, when asked for, the magnitude
+LB_HD void k1_store(uint32_t *bins, float *mags, size_t i, unsigned long long key) {
+    bins[i] = key_idx(key);
+    if (mags) mags[i] = sqrtf(key_mag2(key));
+}
+
 // ---- pass 0: global -> registers -> radix-16 -> shared ---------------------------------
 template <int SF, bool AL16 = true>
 LB_HD void k1_pass0(const K1Args &a, size_t batch, int s, int tid, float2 *buf) {
@@ -215,16 +234,8 @@ LB_HD unsigned long long k1_combine(const K1Args &a, int s, int tid, const float
         float2 gv[8];
 #pragma unroll
         for (int r = 0; r < 8; r++) gv[r] = bs[r * C::SB + pp];
-        float2 acc = gv[7];
-#pragma unroll
-        for (int r = 6; r >= 0; r--) acc = cfma(acc, w, gv[r]);
-        if (s == 0 && q == C::NP / 2) {                    // tmp[N/2] += F[N/2]  (:450)
-            const float2 wc = cconj(w);
-            float2 acc2 = gv[7];
-#pragma unroll
-            for (int r = 6; r >= 0; r--) acc2 = cfma(acc2, wc, gv[r]);
-            acc = cadd(acc, acc2);
-        }
+        float2 acc = horner<8>(gv, w);
+        if (s == 0 && q == C::NP / 2) acc = plus_quirk<8>(acc, gv, w);
         const int kp = C::S * qs + s;
         const uint32_t idx = (uint32_t)(kp >= 0 ? kp : C::N + kp);
         const unsigned long long key = pack_key(cnorm2(acc), idx);
@@ -274,25 +285,11 @@ k1_fft_kernel(K1Args a, uint32_t *__restrict__ bins, float *__restrict__ mags,
             }
             const size_t sym = batch * C::G + tid;
             if (sym < a.n_symbols) {
-                if (C::S == 1) {
-                    bins[sym] = key_idx(bb);
-                    if (mags) mags[sym] = sqrtf(key_mag2(bb));
-                } else {
-                    atomicMax(packed + sym, bb);
-                }
+                if (C::S == 1) k1_store(bins, mags, sym, bb);
+                else atomicMax(packed + sym, bb);
             }
         }
         // warp_best and buf are rewritten only after the next pass0 + __syncthreads
-    }
-}
-
-static __global__ void k1_finalize_kernel(const unsigned long long *__restrict__ packed, size_t n,
-                                   uint32_t *__restrict__ bins, float *__restrict__ mags) {
-    const size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x;
-    if (i < n) {
-        const unsigned long long k = packed[i];
-        bins[i] = key_idx(k);
-        if (mags) mags[i] = sqrtf(key_mag2(k));
     }
 }
 #endif  // __CUDACC__
@@ -320,10 +317,7 @@ inline void k1_emulate(const K1Args &a, uint32_t *bins, float *mags) {
             }
         }
     }
-    for (size_t i = 0; i < a.n_symbols; i++) {
-        bins[i] = key_idx(packed[i]);
-        if (mags) mags[i] = sqrtf(key_mag2(packed[i]));
-    }
+    for (size_t i = 0; i < a.n_symbols; i++) k1_store(bins, mags, i, packed[i]);
     delete[] buf;
     delete[] packed;
 }

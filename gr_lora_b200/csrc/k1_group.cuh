@@ -6,15 +6,18 @@
 //            inter-pass twiddle u^kc (u = W_N^a lane invariant, powers kept in registers)
 //   exch 1   XOR-swizzled 128-bit exchange through the consumed slot: thread (kc, h) receives its
 //            NR = 4/W polyphase branches of output column kc, all M0 = 8 W points
-//   pass 1   NR radix-M0 FFTs in registers (radix 16 at SF8, radix 32 at SF9)
-//   exch 2   second swizzled exchange ([bin][branch]) so that each thread holds all 8 branches of 4 bins
-//   combine  Horner over the 8 branches with ONE lane-invariant twiddle per bin, |.|^2, group argmax
+//   pass 1   NR radix-M0 FFTs in registers (radix 16 at SF8, radix 32 at SF9), branch pairs combined
+//   exch 2   second swizzled exchange ([bin][branch pair]) so that each thread holds all 4 pair sums of 4 bins
+//   combine  Horner over the 4 pairs with ONE lane-invariant twiddle per bin, |.|^2, group argmax
 // Same arithmetic as get_shift_fft (lib/decoder_impl.cc:430-464); see k1_fft.cuh for the derivation.
 // Shared-memory traffic per symbol: 6 x 8*sps bytes (slot read, chirp read, two exchanges).  The down-chirp is one
 // shared-memory table per CTA, read by every group (the samples a thread multiplies with are symbol-invariant).
 #pragma once
-#include "k1_warp.cuh"
+#include "k1_ring.cuh"
 #include "k1_group_consts.h"
+#include "k1_launch.h"
+
+#include <algorithm>
 
 namespace lb {
 
@@ -24,20 +27,18 @@ struct GCfg {
     static constexpr int T = 32 * W;                 // threads per group
     static constexpr int N = 1 << SF, SPS = 8 * N;
     static constexpr int M0 = 8 * W;                 // points of the second FFT (columns)
-    static constexpr int NR = 4 / W;                 // branches per thread in pass 1: 4, 2, 1
+    static constexpr int NR = 4 / W;                 // branches per thread in pass 1: 2, 1
     static constexpr int LPK = 2 * W;                // lanes per output column kc
     static constexpr int SLOT_F4 = 16 * T;           // float4 per slot
-    static constexpr uint32_t SLOT_BYTES = 8u * SPS;
-    static_assert(SF >= 7 && SF <= 9, "group kernel: SF7..SF9");
+    static_assert(SF == 8 || SF == 9, "group kernel: SF8, SF9");
 };
 
-template <int SF> LB_HD int g_swz1(int kc) { return SF == 7 ? ((kc & 1) | ((kc & 2) << 1)) : ((kc & 1) << 2); }
+LB_HD int g_swz1(int kc) { return (kc & 1) << 2; }
 template <int SF> LB_HD int g_signed_bin(int q) { return q < GCfg<SF>::N / 2 ? q : q - GCfg<SF>::N; }
 
 template <int SF>
 struct GConsts {
     float2 twk[16];          // W_N^{a kc}, a = t >> 2 (pass-0 output twiddle), twk[0] = 1
-    float2 wq[4];            // W_sps^{q'} for the thread's bins q = t + T i
     float2 wq2[4];           // wq^2 (Horner over branch PAIRS)
     float2 wb;               // pair-twiddle base of this lane: W_sps^{kc} (times the upper-half factor at SF9)
 };
@@ -47,7 +48,6 @@ LB_HD void g_consts(int t, const float2 *tw, GConsts<SF> &c) {
     using C = GCfg<SF>;
     const int a = t >> 2;
     for (int kc = 0; kc < 16; kc++) c.twk[kc] = k1_ld_table(tw + ((a * kc * 8) & (C::SPS - 1)));     // W_N = W_sps^8
-    for (int i = 0; i < 4; i++) c.wq[i] = k1_ld_table(tw + (g_signed_bin<SF>(t + C::T * i) & (C::SPS - 1)));
     for (int i = 0; i < 4; i++) c.wq2[i] = k1_ld_table(tw + ((2 * g_signed_bin<SF>(t + C::T * i)) & (C::SPS - 1)));
     {   // w[ka] = W_sps^{q'} with q = kc + 16 ka = wb * g_cc[ka]; at SF9 the odd lane of a pair owns ka >= M0/2:
         // g_cc[ka] = g_cc[ka - M0/2] * W_sps^{16 M0/2 - N}, folded into its wb
@@ -94,7 +94,7 @@ LB_HD void g_store1(int t, float4 *slot, const float2 *v0, const float2 *v1) {
 #pragma unroll
     for (int kc = 0; kc < 16; kc++) {
         const int br = bitrev<16>(kc);
-        slot[kc * C::T + (t ^ g_swz1<SF>(kc))] = make_float4(v0[br].x, v0[br].y, v1[br].x, v1[br].y);
+        slot[kc * C::T + (t ^ g_swz1(kc))] = make_float4(v0[br].x, v0[br].y, v1[br].x, v1[br].y);
     }
 }
 
@@ -104,18 +104,11 @@ template <int SF>
 LB_HD void g_pass1(int t, const float4 *slot, float2 (*g)[GCfg<SF>::M0]) {
     using C = GCfg<SF>;
     const int kc = t / C::LPK, h = t % C::LPK;
-    const int sw = g_swz1<SF>(kc);
+    const int sw = g_swz1(kc);
     const float4 *row = slot + kc * C::T;
 #pragma unroll
     for (int a = 0; a < C::M0; a++) {
-        if constexpr (C::NR == 4) {
-#pragma unroll
-            for (int e = 0; e < 2; e++) {
-                const float4 u = row[(4 * a + 2 * h + e) ^ sw];
-                g[2 * e][a] = make_float2(u.x, u.y);
-                g[2 * e + 1][a] = make_float2(u.z, u.w);
-            }
-        } else if constexpr (C::NR == 2) {
+        if constexpr (C::NR == 2) {
             const float4 u = row[(4 * a + h) ^ sw];
             g[0][a] = make_float2(u.x, u.y);
             g[C::NR - 1][a] = make_float2(u.z, u.w);
@@ -128,62 +121,7 @@ LB_HD void g_pass1(int t, const float4 *slot, float2 (*g)[GCfg<SF>::M0]) {
     for (int i = 0; i < C::NR; i++) dft_dif<C::M0>(g[i]);
 }
 
-// exchange 2: [bin q][16-byte unit u = r/2], unit position XOR ((q >> 1) & 3); 4 units (64 B) per bin
-LB_HD int g_unit2(int q, int u) { return q * 4 + (u ^ ((q >> 1) & 3)); }
-
-template <int SF>
-LB_HD void g_store2(int t, float4 *slot, float2 (*g)[GCfg<SF>::M0]) {
-    using C = GCfg<SF>;
-    const int kc = t / C::LPK, h = t % C::LPK;
-#pragma unroll
-    for (int ka = 0; ka < C::M0; ka++) {
-        const int br = bitrev<C::M0>(ka);
-        const int q = kc + 16 * ka;
-        if constexpr (C::NR == 4) {
-            slot[g_unit2(q, 2 * h)] = make_float4(g[0][br].x, g[0][br].y, g[1][br].x, g[1][br].y);
-            slot[g_unit2(q, 2 * h + 1)] = make_float4(g[2][br].x, g[2][br].y, g[3][br].x, g[3][br].y);
-        } else if constexpr (C::NR == 2) {
-            slot[g_unit2(q, h)] = make_float4(g[0][br].x, g[0][br].y, g[C::NR - 1][br].x, g[C::NR - 1][br].y);
-        } else {
-            float2 *p2 = reinterpret_cast<float2 *>(slot + g_unit2(q, h >> 1));
-            p2[h & 1] = g[0][br];
-        }
-    }
-}
-
-// combine: bins q = t + T i, i = 0..3: all 8 branches, Horner with w = W_sps^{q'}
-template <int SF>
-LB_HD unsigned long long g_combine(int t, const float4 *slot, const GConsts<SF> &c) {
-    using C = GCfg<SF>;
-    unsigned long long best = 0ull;
-#pragma unroll
-    for (int i = 0; i < 4; i++) {
-        const int q = t + C::T * i;
-        float2 gv[8];
-#pragma unroll
-        for (int u = 0; u < 4; u++) {
-            const float4 v = slot[g_unit2(q, u)];
-            gv[2 * u] = make_float2(v.x, v.y);
-            gv[2 * u + 1] = make_float2(v.z, v.w);
-        }
-        const float2 w = c.wq[i];
-        float2 acc = gv[7];
-#pragma unroll
-        for (int r = 6; r >= 0; r--) acc = cfma(acc, w, gv[r]);
-        if (q == C::N / 2) {                             // tmp[N/2] += F[N/2]  (:450); thread 0, i = 2
-            const float2 wc = cconj(w);
-            float2 acc2 = gv[7];
-#pragma unroll
-            for (int r = 6; r >= 0; r--) acc2 = cfma(acc2, wc, gv[r]);
-            acc = cadd(acc, acc2);
-        }
-        const unsigned long long key = pack_key(cnorm2(acc), (uint32_t)q);
-        best = key > best ? key : best;
-    }
-    return best;
-}
-
-// ---- pair variant (SF8, SF9): combine branch pairs BEFORE the second exchange ---------------------
+// ---- combine branch pairs BEFORE the second exchange ----------------------------------------------
 // P_pr[q] = G_{2pr}[q] + w[q] G_{2pr+1}[q].  SF8 (NR = 2): both branches are in the thread.  SF9 (NR = 1):
 // the partner lane t^1 holds the other branch; the even lane finishes ka < M0/2, the odd lane ka >= M0/2
 // (own = this lane's G, bit-reversed; other = what the partner sent for this lane's half).
@@ -251,17 +189,8 @@ LB_HD unsigned long long g_combine_p(int t, const float2 *slot2, const float2 *q
             pv[2 * u] = make_float2(v.x, v.y);
             pv[2 * u + 1] = make_float2(v.z, v.w);
         }
-        const float2 w2 = c.wq2[i];
-        float2 acc = cfma(pv[3], w2, pv[2]);
-        acc = cfma(acc, w2, pv[1]);
-        acc = cfma(acc, w2, pv[0]);
-        if (q == C::N / 2) {                             // tmp[N/2] += F[N/2]  (:450)
-            const float2 wc = cconj(w2);
-            float2 a2 = cfma(quirk[3], wc, quirk[2]);
-            a2 = cfma(a2, wc, quirk[1]);
-            a2 = cfma(a2, wc, quirk[0]);
-            acc = cadd(acc, a2);
-        }
+        float2 acc = horner<4>(pv, c.wq2[i]);
+        if (q == C::N / 2) acc = plus_quirk<4>(acc, quirk, c.wq2[i]);
         const unsigned long long key = pack_key(cnorm2(acc), (uint32_t)q);
         best = key > best ? key : best;
     }
@@ -291,32 +220,18 @@ k1_group_kernel(K1Args a, uint32_t *__restrict__ bins, float *__restrict__ mags)
     const int bar_id = 1 + grp;                         // named barrier of this group (0 = __syncthreads)
     const size_t gg = (size_t)blockIdx.x * NGROUPS + grp, g_total = (size_t)gridDim.x * NGROUPS;
 
-    if (t == 0) {
-#pragma unroll
-        for (int s = 0; s < NSLOT; s++) mbar_init(&sm.bars[grp][s], 1);
-        fence_mbar_init();
-    }
+    const SymbolRing<float4, C::SLOT_F4, NSLOT> ring{sm.slots[grp], sm.bars[grp], a.x, gg, g_total, a.n_symbols};
+
+    if (t == 0) ring.init();
     for (int i = threadIdx.x; i < C::SLOT_F4; i += NGROUPS * C::T) sm.chirp[i] = k1_ld_table4(a.chirp + 2 * i);
     __syncthreads();
-    if (t == 0) {
-#pragma unroll
-        for (int s = 0; s < NSLOT; s++) {
-            const size_t sym = gg + (size_t)s * g_total;
-            if (sym < a.n_symbols) {
-                mbar_expect_tx(&sm.bars[grp][s], C::SLOT_BYTES);
-                bulk_g2s(sm.slots[grp][s], a.x + sym * C::SPS, C::SLOT_BYTES, &sm.bars[grp][s]);
-            }
-        }
-    }
+    if (t == 0) ring.fill();
     GConsts<SF> c;
     g_consts<SF>(t, a.tw, c);
 
     uint32_t it = 0;
     for (size_t sym = gg; sym < a.n_symbols; sym += g_total, it++) {
-        const int s = it % NSLOT;
-        const uint32_t parity = (it / NSLOT) & 1u;
-        float4 *slot = sm.slots[grp][s];
-        mbar_wait(&sm.bars[grp][s], parity);
+        float4 *slot = ring.wait(it);
         {
             float2 v0[16], v1[16];
             g_pass0<SF>(t, slot, sm.chirp, c, v0, v1);
@@ -326,52 +241,52 @@ k1_group_kernel(K1Args a, uint32_t *__restrict__ bins, float *__restrict__ mags)
         group_bar(bar_id, C::T);
         float2 g[C::NR][C::M0];
         g_pass1<SF>(t, slot, g);
-        unsigned long long best;
-        if constexpr (C::NR == 4) {
-            group_bar(bar_id, C::T);                    // exchange-1 reads done
-            g_store2<SF>(t, slot, g);
-            group_bar(bar_id, C::T);
-            best = g_combine<SF>(t, slot, c);
+        float2 P[GPair<SF>::NP], Pq;
+        if constexpr (C::NR == 2) {
+            g_pair_sf8<SF>(t, g, c, P, Pq);
         } else {
-            float2 P[GPair<SF>::NP], Pq;
-            if constexpr (C::NR == 2) {
-                g_pair_sf8<SF>(t, g, c, P, Pq);
-            } else {
-                const int odd = t & 1;
-                float2 keep[C::M0 / 2], recv[C::M0 / 2];
+            const int odd = t & 1;
+            float2 keep[C::M0 / 2], recv[C::M0 / 2];
 #pragma unroll
-                for (int j = 0; j < C::M0 / 2; j++) {
-                    const float2 lo = g[0][bitrev<C::M0>(j)], hi = g[0][bitrev<C::M0>(j + C::M0 / 2)];
-                    keep[j] = odd ? hi : lo;
-                    const float2 send = odd ? lo : hi;
-                    recv[j].x = __shfl_xor_sync(0xffffffffu, send.x, 1);
-                    recv[j].y = __shfl_xor_sync(0xffffffffu, send.y, 1);
-                }
-                g_pair_sf9<SF>(t, keep, recv, c, P, Pq);
+            for (int j = 0; j < C::M0 / 2; j++) {
+                const float2 lo = g[0][bitrev<C::M0>(j)], hi = g[0][bitrev<C::M0>(j + C::M0 / 2)];
+                keep[j] = odd ? hi : lo;
+                const float2 send = odd ? lo : hi;
+                recv[j].x = __shfl_xor_sync(0xffffffffu, send.x, 1);
+                recv[j].y = __shfl_xor_sync(0xffffffffu, send.y, 1);
             }
-            group_bar(bar_id, C::T);                    // exchange-1 reads done
-            g_store2p<SF>(t, reinterpret_cast<float2 *>(slot), P, Pq, sm.quirk[grp]);
-            group_bar(bar_id, C::T);
-            best = g_combine_p<SF>(t, reinterpret_cast<const float2 *>(slot), sm.quirk[grp], c);
+            g_pair_sf9<SF>(t, keep, recv, c, P, Pq);
         }
+        group_bar(bar_id, C::T);                        // exchange-1 reads done
+        g_store2p<SF>(t, reinterpret_cast<float2 *>(slot), P, Pq, sm.quirk[grp]);
+        group_bar(bar_id, C::T);
+        unsigned long long best = g_combine_p<SF>(t, reinterpret_cast<const float2 *>(slot), sm.quirk[grp], c);
         best = warp_max_key(best);
         if (lane == 0) sm.keys[grp][wig] = best;
         group_bar(bar_id, C::T);                        // exchange-2 reads done + keys visible
         if (t == 0) {
-            const size_t nxt = sym + (size_t)NSLOT * g_total;
-            if (nxt < a.n_symbols) {
-                fence_proxy_async();
-                mbar_expect_tx(&sm.bars[grp][s], C::SLOT_BYTES);
-                bulk_g2s(slot, a.x + nxt * C::SPS, C::SLOT_BYTES, &sm.bars[grp][s]);
-            }
+            ring.refill(it, sym);
             unsigned long long bb = sm.keys[grp][0];
 #pragma unroll
             for (int k = 1; k < C::W; k++) bb = sm.keys[grp][k] > bb ? sm.keys[grp][k] : bb;
-            bins[sym] = key_idx(bb);
-            if (mags) mags[sym] = sqrtf(key_mag2(bb));
+            k1_store(bins, mags, sym, bb);
         }
         // keys[] is rewritten only after four more group barriers: no hazard with thread 0's read
     }
+}
+
+// instantiated in the translation unit that owns the SF's kernel: SF8 lora_b200.cu, SF9 k1_packed.cu
+template <int SF, int NGROUPS, int NSLOT>
+int k1_launch_group(const K1Launch &k) {
+    static DeviceOnce once;
+    const size_t smem = sizeof(GSmem<SF, NGROUPS, NSLOT>);
+    K1_CU(once(k.device, [&] {
+        return cudaFuncSetAttribute(k1_group_kernel<SF, NGROUPS, NSLOT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    }));
+    const int grid = (int)std::min((k.a.n_symbols + NGROUPS - 1) / NGROUPS, (size_t)k.n_sms);
+    k1_group_kernel<SF, NGROUPS, NSLOT><<<grid, NGROUPS * GCfg<SF>::T, smem, k.st>>>(k.a, k.bins, k.mags);
+    K1_CU(cudaGetLastError());
+    return 0;
 }
 #endif  // __CUDACC__
 
@@ -395,39 +310,30 @@ inline void g_emulate(const K1Args &a, uint32_t *bins, float *mags) {
         for (int t = 0; t < C::T; t++) g_store1<SF>(t, slot, v0[t], v1[t]);
         for (int t = 0; t < C::T; t++) g_pass1<SF>(t, slot, g[t]);
         for (int i = 0; i < C::SLOT_F4; i++) slot[i] = make_float4(NAN, NAN, NAN, NAN);
-        unsigned long long best = 0ull;
-        if constexpr (C::NR == 4) {
-            for (int t = 0; t < C::T; t++) g_store2<SF>(t, slot, g[t]);
-            for (int t = 0; t < C::T; t++) {
-                const unsigned long long k = g_combine<SF>(t, slot, c[t]);
-                best = k > best ? k : best;
-            }
-        } else {
-            float2 quirk[4] = {};
-            float2 *slot2 = reinterpret_cast<float2 *>(slot);
-            for (int t = 0; t < C::T; t++) {
-                float2 P[GPair<SF>::NP], Pq;
-                if constexpr (C::NR == 2) {
-                    g_pair_sf8<SF>(t, g[t], c[t], P, Pq);
-                } else {
-                    const int odd = t & 1;
-                    float2 keep[C::M0 / 2], recv[C::M0 / 2];
-                    for (int j = 0; j < C::M0 / 2; j++) {
-                        const int mine = bitrev<C::M0>(j + (odd ? C::M0 / 2 : 0));
-                        keep[j] = g[t][0][mine];
-                        recv[j] = g[t ^ 1][0][mine];          // what the partner sends: its value at MY ka
-                    }
-                    g_pair_sf9<SF>(t, keep, recv, c[t], P, Pq);
+        float2 quirk[4] = {};
+        float2 *slot2 = reinterpret_cast<float2 *>(slot);
+        for (int t = 0; t < C::T; t++) {
+            float2 P[GPair<SF>::NP], Pq;
+            if constexpr (C::NR == 2) {
+                g_pair_sf8<SF>(t, g[t], c[t], P, Pq);
+            } else {
+                const int odd = t & 1;
+                float2 keep[C::M0 / 2], recv[C::M0 / 2];
+                for (int j = 0; j < C::M0 / 2; j++) {
+                    const int mine = bitrev<C::M0>(j + (odd ? C::M0 / 2 : 0));
+                    keep[j] = g[t][0][mine];
+                    recv[j] = g[t ^ 1][0][mine];          // what the partner sends: its value at MY ka
                 }
-                g_store2p<SF>(t, slot2, P, Pq, quirk);
+                g_pair_sf9<SF>(t, keep, recv, c[t], P, Pq);
             }
-            for (int t = 0; t < C::T; t++) {
-                const unsigned long long k = g_combine_p<SF>(t, slot2, quirk, c[t]);
-                best = k > best ? k : best;
-            }
+            g_store2p<SF>(t, slot2, P, Pq, quirk);
         }
-        bins[sym] = key_idx(best);
-        if (mags) mags[sym] = sqrtf(key_mag2(best));
+        unsigned long long best = 0ull;
+        for (int t = 0; t < C::T; t++) {
+            const unsigned long long k = g_combine_p<SF>(t, slot2, quirk, c[t]);
+            best = k > best ? k : best;
+        }
+        k1_store(bins, mags, sym, best);
     }
     delete[] slot; delete[] chirp; delete[] c; delete[] v0; delete[] v1; delete[] g;
 }

@@ -2,9 +2,8 @@
 // the IQ batch (SF12) and the launch (SF12: clusters of two CTAs).
 #define LB_PACKED_CMUL 1
 #include "k1_rows.cuh"
-#include "k1_rows.h"
+#include "k1_launch.h"
 
-#include <cstdio>
 #include <cstring>
 
 namespace lb {
@@ -27,55 +26,49 @@ encode_tiled_fn get_encoder() {
     return fn;
 }
 
-#define RCU(call)                                                                     \
-    do {                                                                              \
-        cudaError_t e_ = (call);                                                      \
-        if (e_ != cudaSuccess) {                                                      \
-            snprintf(err, err_cap, "%s: %s", #call, cudaGetErrorString(e_));          \
-            return (int)e_;                                                           \
-        }                                                                             \
-    } while (0)
+}  // namespace
 
+// SF11 writes bins / mags directly; SF12 merges the two CTAs' argmax keys into k.packed
 template <int SF>
-int launch(int device, int n_sms, const float2 *iq, const float2 *chirp, const float2 *tw, const float2 *tw_host, size_t n_symbols,
-           uint32_t *bins, float *mags, unsigned long long *packed, cudaStream_t st, char *err, size_t err_cap) {
+int k1_launch_rows(const K1Launch &k) {
     using C = RCfg<SF>;
-    static bool ready[64] = {};
+    static DeviceOnce once;
     const size_t smem = sizeof(RSmem<SF>);
-    if (!ready[device & 63]) {
-        RCU(cudaFuncSetAttribute(k1_rows_kernel<SF>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        if (C::CL > 1) RCU(cudaFuncSetAttribute(k1_rows_kernel<SF>, cudaFuncAttributeNonPortableClusterSizeAllowed, 0));
+    K1_CU(once(k.device, [&] {      // the shared-memory and cluster opt-ins, and the per-q2 constants from the host table
+        cudaError_t e = cudaFuncSetAttribute(k1_rows_kernel<SF>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+        if (e == cudaSuccess && C::CL > 1) e = cudaFuncSetAttribute(k1_rows_kernel<SF>, cudaFuncAttributeNonPortableClusterSizeAllowed, 0);
+        if (e != cudaSuccess) return e;
         RConsts rc;
-        r_build_consts<SF>(tw_host, rc);
-        RCU(cudaMemcpyToSymbol(r_consts_dev, &rc, sizeof rc, sizeof(RConsts) * (SF - 11)));
-        ready[device & 63] = true;
-    }
+        r_build_consts<SF>(k.tw_host, rc);
+        return cudaMemcpyToSymbol(r_consts_dev, &rc, sizeof rc, sizeof(RConsts) * (SF - 11));
+    }));
+    const size_t n_symbols = k.a.n_symbols;
     RParams P;
     memset(&P, 0, sizeof P);
-    P.a = K1Args{iq, chirp, tw, n_symbols};
-    P.packed = packed; P.bins = bins; P.mags = mags;
+    P.a = k.a;
+    P.packed = k.packed; P.bins = k.bins; P.mags = k.mags;
     if (C::CL == 2) {
         encode_tiled_fn enc = get_encoder();
-        if (!enc) { snprintf(err, err_cap, "cuTensorMapEncodeTiled is not available from this driver"); return (int)cudaErrorNotSupported; }
+        if (!enc) { snprintf(k.err, k.err_cap, "cuTensorMapEncodeTiled is not available from this driver"); return (int)cudaErrorNotSupported; }
         // the batch as a 2-D float array: 16 floats (8 branches x re/im) per n1, n_symbols * L values of n1;
         // a box = 8 floats (this CTA's 4 branches) x 256 n1 = one row of 8 KiB, dense in shared memory
         const cuuint64_t dims[2] = {16, (cuuint64_t)n_symbols * C::L};
         const cuuint64_t strides[1] = {64};
         const cuuint32_t box[2] = {8, (cuuint32_t)C::A};
         const cuuint32_t estr[2] = {1, 1};
-        const CUresult r = enc(&P.tmap, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, const_cast<float2 *>(iq), dims, strides, box, estr,
+        const CUresult r = enc(&P.tmap, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, const_cast<float2 *>(k.a.x), dims, strides, box, estr,
                                CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_NONE,
                                CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-        if (r != CUDA_SUCCESS) { snprintf(err, err_cap, "cuTensorMapEncodeTiled failed (%d)", (int)r); return (int)cudaErrorInvalidValue; }
+        if (r != CUDA_SUCCESS) { snprintf(k.err, k.err_cap, "cuTensorMapEncodeTiled failed (%d)", (int)r); return (int)cudaErrorInvalidValue; }
     }
-    size_t units = (size_t)n_sms / C::CL;
+    size_t units = (size_t)k.n_sms / C::CL;
     if (units > n_symbols) units = n_symbols;
     if (units == 0) return 0;
     cudaLaunchConfig_t cfg = {};
     cfg.gridDim = dim3((unsigned)(units * C::CL));
     cfg.blockDim = dim3(C::T);
     cfg.dynamicSmemBytes = smem;
-    cfg.stream = st;
+    cfg.stream = k.st;
     cudaLaunchAttribute attr[1];
     attr[0].id = cudaLaunchAttributeClusterDimension;
     attr[0].val.clusterDim.x = C::CL;
@@ -83,12 +76,12 @@ int launch(int device, int n_sms, const float2 *iq, const float2 *chirp, const f
     attr[0].val.clusterDim.z = 1;
     cfg.attrs = attr;
     cfg.numAttrs = 1;
-    RCU(cudaLaunchKernelEx(&cfg, k1_rows_kernel<SF>, P));
+    K1_CU(cudaLaunchKernelEx(&cfg, k1_rows_kernel<SF>, P));
 #ifdef LB_ROWS_TIMING
     {   // diagnosis build: mean cycles per symbol and warp class spent in each wait
-        RCU(cudaStreamSynchronize(st));
+        K1_CU(cudaStreamSynchronize(k.st));
         static unsigned int h[160 * 16 * 8];
-        RCU(cudaMemcpyFromSymbol(h, r_timing_dev, sizeof h));
+        K1_CU(cudaMemcpyFromSymbol(h, r_timing_dev, sizeof h));
         const char *names[6] = {"x_full", "x_free", "sym_full", "sym_late", "barrier", "-"};
         for (int rank = 0; rank < C::CL; rank++)
             for (int half = 0; half < 2; half++) {
@@ -112,15 +105,7 @@ int launch(int device, int n_sms, const float2 *iq, const float2 *chirp, const f
     return 0;
 }
 
-}  // namespace
-
-int k1_rows_launch(int sf, int device, int n_sms, const float2 *iq, const float2 *chirp, const float2 *tw, const float2 *tw_host,
-                   size_t n_symbols, uint32_t *bins, float *mags, unsigned long long *packed, cudaStream_t st, char *err,
-                   size_t err_cap) {
-    if (sf == 11) return launch<11>(device, n_sms, iq, chirp, tw, tw_host, n_symbols, bins, mags, packed, st, err, err_cap);
-    if (sf == 12) return launch<12>(device, n_sms, iq, chirp, tw, tw_host, n_symbols, bins, mags, packed, st, err, err_cap);
-    snprintf(err, err_cap, "rows kernel: SF11 / SF12 only");
-    return (int)cudaErrorInvalidValue;
-}
+template int k1_launch_rows<11>(const K1Launch &k);
+template int k1_launch_rows<12>(const K1Launch &k);
 
 }  // namespace lb

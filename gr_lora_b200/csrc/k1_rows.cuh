@@ -33,7 +33,7 @@
 // The index arithmetic and the butterflies are __host__ __device__ (r_emulate below runs them on the CPU for the
 // non-GPU tests, with shared memory and the peer exchange modelled as plain arrays).
 #pragma once
-#include "k1_warp.cuh"
+#include "k1_ring.cuh"
 #ifdef __CUDACC__
 #include <cuda.h>      // CUtensorMap (type only; the encoder is fetched through cudaGetDriverEntryPoint)
 #endif
@@ -627,8 +627,7 @@ inline void r_emulate(const K1Args &a, uint32_t *bins, float *mags) {
             const unsigned long long key = pack_key(cnorm2(f), (uint32_t)k);
             best = key > best ? key : best;
         }
-        bins[s] = key_idx(best);
-        if (mags) mags[s] = sqrtf(key_mag2(best));
+        k1_store(bins, mags, s, best);
     }
     for (int c = 0; c < C::CL; c++) { delete[] slots[c]; delete[] part[c]; }
     delete[] keys;

@@ -9,13 +9,12 @@
 // The 32 down-chirp samples a thread multiplies with are the same for every symbol; the CTA keeps the chirp as a
 // 64 KiB shared-memory table next to a ring of two TMA slots (64 + 2 x 64 KiB).
 #pragma once
-#include "k1_group.cuh"
+#include "k1_ring.cuh"
 
 namespace lb {
 
 constexpr int S10_T = 256, S10_N = 1024, S10_SPS = 8192;
 constexpr int S10_SLOT_F2 = 8192;                    // float2 per slot
-constexpr uint32_t S10_SLOT_BYTES = 65536u;
 
 struct S10Consts {
     float2 tl[4];            // W_N^{a j},   j = 0..3
@@ -87,17 +86,8 @@ LB_HD unsigned long long s10_combine(int t, const float2 *slot, const S10Consts 
             gv[2 * u] = make_float2(v.x, v.y);
             gv[2 * u + 1] = make_float2(v.z, v.w);
         }
-        const float2 w = c.wq[i];
-        float2 acc = gv[7];
-#pragma unroll
-        for (int r = 6; r >= 0; r--) acc = cfma(acc, w, gv[r]);
-        if (q == S10_N / 2) {                            // tmp[N/2] += F[N/2]  (:450)
-            const float2 wc = cconj(w);
-            float2 acc2 = gv[7];
-#pragma unroll
-            for (int r = 6; r >= 0; r--) acc2 = cfma(acc2, wc, gv[r]);
-            acc = cadd(acc, acc2);
-        }
+        float2 acc = horner<8>(gv, c.wq[i]);
+        if (q == S10_N / 2) acc = plus_quirk<8>(acc, gv, c.wq[i]);
         const unsigned long long key = pack_key(cnorm2(acc), (uint32_t)q);
         best = key > best ? key : best;
     }
@@ -120,30 +110,16 @@ k1_sf10_kernel(K1Args a, uint32_t *__restrict__ bins, float *__restrict__ mags) 
     S10Smem<NSLOT> &sm = *reinterpret_cast<S10Smem<NSLOT> *>(s10_raw);
     const int t = threadIdx.x, lane = t & 31, warp = t >> 5;
     const size_t g0 = blockIdx.x, g_total = gridDim.x;
-    if (t == 0) {
-#pragma unroll
-        for (int s = 0; s < NSLOT; s++) mbar_init(&sm.bars[s], 1);
-        fence_mbar_init();
-    }
+    const SymbolRing<float2, S10_SLOT_F2, NSLOT> ring{sm.slots, sm.bars, a.x, g0, g_total, a.n_symbols};
+    if (t == 0) ring.init();
     for (int i = t; i < S10_SLOT_F2; i += S10_T) sm.chirp[i] = k1_ld_table(a.chirp + i);
     __syncthreads();
-    if (t == 0) {
-#pragma unroll
-        for (int s = 0; s < NSLOT; s++) {
-            const size_t sym = g0 + (size_t)s * g_total;
-            if (sym < a.n_symbols) {
-                mbar_expect_tx(&sm.bars[s], S10_SLOT_BYTES);
-                bulk_g2s(sm.slots[s], a.x + sym * S10_SPS, S10_SLOT_BYTES, &sm.bars[s]);
-            }
-        }
-    }
+    if (t == 0) ring.fill();
     S10Consts c;
     s10_consts(t, a.tw, c);
     uint32_t it = 0;
     for (size_t sym = g0; sym < a.n_symbols; sym += g_total, it++) {
-        const int s = it % NSLOT;
-        float2 *slot = sm.slots[s];
-        mbar_wait(&sm.bars[s], (it / NSLOT) & 1u);
+        float2 *slot = ring.wait(it);
         float2 v[32];
         s10_pass0(t, slot, sm.chirp, c, v);
         __syncthreads();
@@ -158,17 +134,11 @@ k1_sf10_kernel(K1Args a, uint32_t *__restrict__ bins, float *__restrict__ mags) 
         if (lane == 0) sm.keys[warp] = best;
         __syncthreads();
         if (t == 0) {
-            const size_t nxt = sym + (size_t)NSLOT * g_total;
-            if (nxt < a.n_symbols) {
-                fence_proxy_async();
-                mbar_expect_tx(&sm.bars[s], S10_SLOT_BYTES);
-                bulk_g2s(slot, a.x + nxt * S10_SPS, S10_SLOT_BYTES, &sm.bars[s]);
-            }
+            ring.refill(it, sym);
             unsigned long long bb = sm.keys[0];
 #pragma unroll
             for (int k = 1; k < S10_T / 32; k++) bb = sm.keys[k] > bb ? sm.keys[k] : bb;
-            bins[sym] = key_idx(bb);
-            if (mags) mags[sym] = sqrtf(key_mag2(bb));
+            k1_store(bins, mags, sym, bb);
         }
     }
 }
@@ -193,8 +163,7 @@ inline void s10_emulate(const K1Args &a, uint32_t *bins, float *mags) {
             const unsigned long long k = s10_combine(t, slot, c[t]);
             best = k > best ? k : best;
         }
-        bins[sym] = key_idx(best);
-        if (mags) mags[sym] = sqrtf(key_mag2(best));
+        k1_store(bins, mags, sym, best);
     }
     delete[] slot; delete[] c; delete[] v;
 }

@@ -18,7 +18,7 @@
 //     partner lane, |.|^2, warp argmax.
 // Shared-memory traffic per symbol: 4 x 8 KB (read data, read chirp, exchange write + read).
 #pragma once
-#include "k1_fft.cuh"
+#include "k1_ring.cuh"
 
 namespace lb {
 
@@ -87,21 +87,14 @@ LB_HD void w7_pass1(int lane, const float4 *slot, const W7Consts &c, float2 *P, 
 #pragma unroll
     for (int ka = 0; ka < 8; ka++) {
         const int br = bitrev<8>(ka);
-        float2 acc = g[3][br];
-        acc = cfma(acc, c.wq[ka], g[2][br]);
-        acc = cfma(acc, c.wq[ka], g[1][br]);
-        acc = cfma(acc, c.wq[ka], g[0][br]);
-        P[ka] = acc;
+        const float2 gv[4] = {g[0][br], g[1][br], g[2][br], g[3][br]};
+        P[ka] = horner<4>(gv, c.wq[ka]);
     }
     Pq = make_float2(0.f, 0.f);
     if (kc == 0) {                                   // bin q = 64: tmp[N/2] += F[N/2] (:450)
-        const float2 wc = cconj(c.wq[4]);
         const int br = bitrev<8>(4);
-        float2 acc = g[3][br];
-        acc = cfma(acc, wc, g[2][br]);
-        acc = cfma(acc, wc, g[1][br]);
-        acc = cfma(acc, wc, g[0][br]);
-        Pq = acc;
+        const float2 gv[4] = {g[0][br], g[1][br], g[2][br], g[3][br]};
+        Pq = horner<4>(gv, cconj(c.wq[4]));
     }
 }
 
@@ -129,27 +122,23 @@ LB_HD unsigned long long w7_final(int lane, const W7Consts &c, const float2 *own
 }
 
 #ifdef __CUDACC__
-// ---- TMA bulk copy + mbarrier primitives (sm_90+ PTX, UBLKCP / SYNCS in SASS) -----------------
-LB_D uint32_t smem_u32(const void *p) { return (uint32_t)__cvta_generic_to_shared(p); }
-LB_D void mbar_init(uint64_t *bar, uint32_t count) {
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count));
+// the end of a symbol: lane h of each pair keeps ka = 4h..4h+3 of P and sends the other half to its partner, w7_final, and
+// the warp's argmax key in every lane
+LB_D unsigned long long w7_reduce(int lane, const W7Consts &c, const float2 *P, float2 Pq) {
+    const int h = lane & 1;
+    float2 own[4], other[4];
+#pragma unroll
+    for (int j = 0; j < 4; j++) {
+        const float2 send = h ? P[j] : P[4 + j];
+        own[j] = h ? P[4 + j] : P[j];
+        other[j].x = __shfl_xor_sync(0xffffffffu, send.x, 1);
+        other[j].y = __shfl_xor_sync(0xffffffffu, send.y, 1);
+    }
+    float2 other_q;
+    other_q.x = __shfl_xor_sync(0xffffffffu, Pq.x, 1);
+    other_q.y = __shfl_xor_sync(0xffffffffu, Pq.y, 1);
+    return warp_max_key(w7_final(lane, c, own, other, Pq, other_q));
 }
-LB_D void mbar_expect_tx(uint64_t *bar, uint32_t bytes) {
-    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
-}
-LB_D void mbar_wait(uint64_t *bar, uint32_t parity) {
-    uint32_t ok;
-    do {
-        asm volatile("{\n.reg .pred p;\nmbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\nselp.u32 %0, 1, 0, p;\n}\n"
-                     : "=r"(ok) : "r"(smem_u32(bar)), "r"(parity) : "memory");
-    } while (!ok);
-}
-LB_D void bulk_g2s(void *dst_smem, const void *src_gmem, uint32_t bytes, uint64_t *bar) {
-    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
-                 ::"r"(smem_u32(dst_smem)), "l"(src_gmem), "r"(bytes), "r"(smem_u32(bar)) : "memory");
-}
-LB_D void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-LB_D void fence_mbar_init() { asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
 
 template <int NWARPS, int NSLOT>
 struct W7Smem {
@@ -166,34 +155,18 @@ k1_sf7_warp_kernel(K1Args a, uint32_t *__restrict__ bins, float *__restrict__ ma
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     const size_t gw = (size_t)blockIdx.x * NWARPS + warp, tw_total = (size_t)gridDim.x * NWARPS;
 
-    if (lane == 0) {
-#pragma unroll
-        for (int s = 0; s < NSLOT; s++) mbar_init(&sm.bars[warp][s], 1);
-        fence_mbar_init();
-    }
+    const SymbolRing<float4, W7_SLOT_F4, NSLOT> ring{sm.slots[warp], sm.bars[warp], a.x, gw, tw_total, a.n_symbols};
+
+    if (lane == 0) ring.init();
     for (int i = threadIdx.x; i < W7_SLOT_F4; i += NWARPS * 32) sm.chirp[i] = k1_ld_table4(a.chirp + 2 * i);
     __syncthreads();
-
-    // prologue: fill the ring
-    if (lane == 0) {
-#pragma unroll
-        for (int s = 0; s < NSLOT; s++) {
-            const size_t sym = gw + (size_t)s * tw_total;
-            if (sym < a.n_symbols) {
-                mbar_expect_tx(&sm.bars[warp][s], 8192);
-                bulk_g2s(sm.slots[warp][s], a.x + sym * W7_SPS, 8192, &sm.bars[warp][s]);
-            }
-        }
-    }
+    if (lane == 0) ring.fill();
     W7Consts c;
     w7_consts(lane, a.tw, c);
 
     uint32_t it = 0;
     for (size_t sym = gw; sym < a.n_symbols; sym += tw_total, it++) {
-        const int s = it % NSLOT;
-        const uint32_t parity = (it / NSLOT) & 1u;
-        float4 *slot = sm.slots[warp][s];
-        mbar_wait(&sm.bars[warp][s], parity);
+        float4 *slot = ring.wait(it);
         float2 v0[16], v1[16];
         w7_pass0(lane, slot, sm.chirp, v0, v1);
         __syncwarp();                                   // every lane has read the slot
@@ -202,33 +175,9 @@ k1_sf7_warp_kernel(K1Args a, uint32_t *__restrict__ bins, float *__restrict__ ma
         float2 P[8], Pq;
         w7_pass1(lane, slot, c, P, Pq);
         __syncwarp();                                   // exchange reads done: the slot can be refilled
-        if (lane == 0) {
-            const size_t nxt = sym + (size_t)NSLOT * tw_total;
-            if (nxt < a.n_symbols) {
-                fence_proxy_async();                    // generic-proxy accesses before the async-proxy write
-                mbar_expect_tx(&sm.bars[warp][s], 8192);
-                bulk_g2s(slot, a.x + nxt * W7_SPS, 8192, &sm.bars[warp][s]);
-            }
-        }
-        // partner exchange: lane h keeps ka = 4h..4h+3 and sends the other half
-        const int h = lane & 1;
-        float2 own[4], other[4];
-#pragma unroll
-        for (int j = 0; j < 4; j++) {
-            const float2 send = h ? P[j] : P[4 + j];
-            own[j] = h ? P[4 + j] : P[j];
-            other[j].x = __shfl_xor_sync(0xffffffffu, send.x, 1);
-            other[j].y = __shfl_xor_sync(0xffffffffu, send.y, 1);
-        }
-        float2 other_q;
-        other_q.x = __shfl_xor_sync(0xffffffffu, Pq.x, 1);
-        other_q.y = __shfl_xor_sync(0xffffffffu, Pq.y, 1);
-        unsigned long long best = w7_final(lane, c, own, other, Pq, other_q);
-        best = warp_max_key(best);
-        if (lane == 0) {
-            bins[sym] = key_idx(best);
-            if (mags) mags[sym] = sqrtf(key_mag2(best));
-        }
+        if (lane == 0) ring.refill(it, sym);
+        const unsigned long long best = w7_reduce(lane, c, P, Pq);
+        if (lane == 0) k1_store(bins, mags, sym, best);
     }
 }
 #endif  // __CUDACC__
@@ -259,8 +208,7 @@ inline void w7_emulate(const K1Args &a, uint32_t *bins, float *mags) {
             const unsigned long long k = w7_final(l, c[l], own, other, Pq[l], Pq[l ^ 1]);
             best = k > best ? k : best;
         }
-        bins[sym] = key_idx(best);
-        if (mags) mags[sym] = sqrtf(key_mag2(best));
+        k1_store(bins, mags, sym, best);
     }
     delete[] slot;
     delete[] chirp;

@@ -4,15 +4,13 @@
 // pinned staging and kernel launches.  There is no CPU compute path in this file.
 #include "../../include/lora_b200.h"
 #include "k1_fft.cuh"
-#include "k1_warp.cuh"
 #include "k1_group.cuh"
 #include "k1_sf10.cuh"
+#include "k1_launch.h"
 #include "rx_stream.cuh"
 #include "rx_warp.cuh"
 #include "tx_channel.cuh"
 #include "tx_encode.cuh"
-#include "k1_rows.h"
-#include "k1_packed.h"
 
 #include <algorithm>
 #include <cmath>
@@ -49,15 +47,13 @@ struct Tables {          // offsets (bytes) inside the device blob, see lora_b20
     size_t down, up, down_ifreq, up_ifreq, up_ifreq_v, tw, total;
 };
 
-// Scratch of one K1 launch in flight: the 64-bit argmax keys that the split kernels merge with atomicMax and the
-// L2-resident exchange image + flags of the team kernels.  A launch zeroes it on its stream first, so two launches that
-// share one K1Scratch must not overlap: slot 0 (lora_b200_demod_fft_dev) is ordered across user streams by `done`,
-// and every slot of the host pipeline (lora_b200_demod_fft_host) owns its own.
+// Scratch of one K1 launch in flight: the 64-bit argmax keys that the split kernels merge with atomicMax.  A launch
+// zeroes it on its stream first, so two launches that share one K1Scratch must not overlap: slot 0
+// (lora_b200_demod_fft_dev) is ordered across user streams by `done`, and every slot of the host pipeline
+// (lora_b200_demod_fft_host) owns its own.
 struct K1Scratch {
     unsigned long long *packed = nullptr;
     size_t packed_cap = 0;
-    void *xs = nullptr;
-    size_t xs_cap = 0;
     cudaEvent_t done = nullptr;
     cudaStream_t last = nullptr;
     bool used = false;
@@ -193,102 +189,33 @@ const T *tab(const lora_b200_decoder *d, size_t off) { return (const T *)(d->d_t
 
 // ---- K1 launch -----------------------------------------------------------------------------
 template <int SF>
-int launch_k1(lora_b200_decoder *d, K1Scratch &ks, const float2 *iq, size_t n_symbols, uint32_t *bins, float *mags, cudaStream_t st) {
+int k1_launch_generic(const K1Launch &k) {
     using C = K1Cfg<SF>;
-    static bool attr_set[64] = {};
+    static DeviceOnce once;
     const size_t smem = sizeof(float2) * C::SMEM_ELEMS;
-    if (!attr_set[d->device & 63]) {
-        CU(cudaFuncSetAttribute(k1_fft_kernel<SF>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        attr_set[d->device & 63] = true;
-    }
-    K1Args a{iq, tab<float2>(d, d->toff.down), tab<float2>(d, d->toff.tw), n_symbols};
-    const size_t n_work = ((n_symbols + C::G - 1) / C::G) * C::S;
-    const int grid = (int)std::min<size_t>(n_work, (size_t)d->n_sms * 2);
-    if (C::S > 1) {
-        if (ks.packed_cap < n_symbols) {
-            if (ks.packed) cudaFree(ks.packed);
-            ks.packed = nullptr; ks.packed_cap = 0;
-            CU(cudaMalloc(&ks.packed, sizeof(unsigned long long) * n_symbols));
-            ks.packed_cap = n_symbols;
-        }
-        CU(cudaMemsetAsync(ks.packed, 0, sizeof(unsigned long long) * n_symbols, st));
-    }
-    k1_fft_kernel<SF><<<grid, K1_THREADS, smem, st>>>(a, bins, mags, ks.packed);
-    d->launches++;
-    if (C::S > 1) {
-        k1_finalize_kernel<<<(unsigned)((n_symbols + 255) / 256), 256, 0, st>>>(ks.packed, n_symbols, bins, mags);
-        d->launches++;
-    }
-    CU(cudaGetLastError());
-    return LORA_B200_OK;
-}
-
-// SF8: a group of 2 warps per symbol (k1_group.cuh; the SF7 warp kernel and the SF9 group kernel are launched from k1_packed.cu)
-template <int SF, int NGROUPS, int NSLOT>
-int launch_k1_group(lora_b200_decoder *d, K1Scratch &ks, const float2 *iq, size_t n_symbols, uint32_t *bins, float *mags, cudaStream_t st) {
-    static bool attr_set[64] = {};
-    const size_t smem = sizeof(GSmem<SF, NGROUPS, NSLOT>);
-    if (!attr_set[d->device & 63]) {
-        CU(cudaFuncSetAttribute(k1_group_kernel<SF, NGROUPS, NSLOT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        attr_set[d->device & 63] = true;
-    }
-    K1Args a{iq, tab<float2>(d, d->toff.down), tab<float2>(d, d->toff.tw), n_symbols};
-    const int grid = (int)std::min<size_t>((n_symbols + NGROUPS - 1) / NGROUPS, (size_t)d->n_sms);
-    k1_group_kernel<SF, NGROUPS, NSLOT><<<grid, NGROUPS * GCfg<SF>::T, smem, st>>>(a, bins, mags);
-    d->launches++;
-    CU(cudaGetLastError());
-    return LORA_B200_OK;
+    K1_CU(once(k.device, [&] { return cudaFuncSetAttribute(k1_fft_kernel<SF>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem); }));
+    const size_t n_work = ((k.a.n_symbols + C::G - 1) / C::G) * C::S;
+    const int grid = (int)std::min<size_t>(n_work, (size_t)k.n_sms * 2);
+    k1_fft_kernel<SF><<<grid, K1_THREADS, smem, k.st>>>(k.a, k.bins, k.mags, k.packed);
+    K1_CU(cudaGetLastError());
+    return 0;
 }
 
 // SF10: one 256-thread group per symbol, two radix-32 passes (k1_sf10.cuh)
-int launch_k1_sf10(lora_b200_decoder *d, K1Scratch &ks, const float2 *iq, size_t n_symbols, uint32_t *bins, float *mags, cudaStream_t st) {
-    static bool attr_set[64] = {};
+int k1_launch_sf10(const K1Launch &k) {
+    static DeviceOnce once;
     const size_t smem = sizeof(S10Smem<2>);
-    if (!attr_set[d->device & 63]) {
-        CU(cudaFuncSetAttribute(k1_sf10_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        attr_set[d->device & 63] = true;
-    }
-    K1Args a{iq, tab<float2>(d, d->toff.down), tab<float2>(d, d->toff.tw), n_symbols};
-    const int grid = (int)std::min<size_t>(n_symbols, (size_t)d->n_sms);
-    k1_sf10_kernel<2><<<grid, S10_T, smem, st>>>(a, bins, mags);
-    d->launches++;
-    CU(cudaGetLastError());
-    return LORA_B200_OK;
+    K1_CU(once(k.device, [&] { return cudaFuncSetAttribute(k1_sf10_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem); }));
+    const int grid = (int)std::min<size_t>(k.a.n_symbols, (size_t)k.n_sms);
+    k1_sf10_kernel<2><<<grid, S10_T, smem, k.st>>>(k.a, k.bins, k.mags);
+    K1_CU(cudaGetLastError());
+    return 0;
 }
 
-// SF11 / SF12: every sample stays inside one SM (k1_rows.cuh; SF12 = cluster of two CTAs per symbol); own translation unit
-int launch_k1_rows(lora_b200_decoder *d, K1Scratch &ks, const float2 *iq, size_t n_symbols, uint32_t *bins, float *mags, cudaStream_t st) {
-    const int sf = d->cfg.sf;
-    if (sf == 12) {
-        if (ks.packed_cap < n_symbols) {
-            if (ks.packed) cudaFree(ks.packed);
-            ks.packed = nullptr; ks.packed_cap = 0;
-            CU(cudaMalloc(&ks.packed, sizeof(unsigned long long) * n_symbols));
-            ks.packed_cap = n_symbols;
-        }
-        CU(cudaMemsetAsync(ks.packed, 0, sizeof(unsigned long long) * n_symbols, st));
-    }
-    char err[256] = {0};
-    const int rc = k1_rows_launch(sf, d->device, d->n_sms, iq, tab<float2>(d, d->toff.down), tab<float2>(d, d->toff.tw),
-                                  (const float2 *)(d->h_tables.data() + d->toff.tw), n_symbols, bins, mags, ks.packed, st, err, sizeof err);
-    if (rc) return fail(LORA_B200_ECUDA, "k1_rows: %s", err);
-    d->launches++;
-    if (sf == 12) {
-        k1_finalize_kernel<<<(unsigned)((n_symbols + 255) / 256), 256, 0, st>>>(ks.packed, n_symbols, bins, mags);
-        d->launches++;
-        CU(cudaGetLastError());
-    }
-    return LORA_B200_OK;
-}
-
-// SF7 / SF9: the warp / group kernels built with the packed complex product (k1_packed.cu)
-int launch_k1_packed(lora_b200_decoder *d, const float2 *iq, size_t n_symbols, uint32_t *bins, float *mags, cudaStream_t st) {
-    char err[256] = {0};
-    const int rc = k1_packed_launch(d->cfg.sf, d->device, d->n_sms, iq, tab<float2>(d, d->toff.down), tab<float2>(d, d->toff.tw), n_symbols,
-                                    bins, mags, st, err, sizeof err);
-    if (rc) return fail(LORA_B200_ECUDA, "k1_packed: %s", err);
-    d->launches++;
-    return LORA_B200_OK;
+__global__ void k1_finalize_kernel(const unsigned long long *__restrict__ packed, size_t n, uint32_t *__restrict__ bins,
+                                   float *__restrict__ mags) {
+    const size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x;
+    if (i < n) k1_store(bins, mags, i, packed[i]);
 }
 
 // LORA_B200_K1=generic selects k1_fft_kernel (the CTA-wide kernel the stream state machine also uses) for every SF;
@@ -300,30 +227,55 @@ bool k1_generic() {
     return v == 1;
 }
 
+K1Launcher k1_launcher(int sf, bool generic) {
+    switch (generic ? -sf : sf) {
+    case 7: return k1_launch_warp7;                  // k1_packed.cu
+    case 8: return k1_launch_group<8, 6, 2>;         // a group of 2 warps per symbol (k1_group.cuh)
+    case 9: return k1_launch_group9;                 // k1_packed.cu
+    case 10: return k1_launch_sf10;
+    case 11: return k1_launch_rows<11>;              // every sample stays inside one SM (k1_rows.cuh, k1_rows.cu)
+    case 12: return k1_launch_rows<12>;              // a cluster of two CTAs per symbol
+    case -7: return k1_launch_generic<7>;
+    case -8: return k1_launch_generic<8>;
+    case -9: return k1_launch_generic<9>;
+    case -10: return k1_launch_generic<10>;
+    case -11: return k1_launch_generic<11>;
+    case -12: return k1_launch_generic<12>;
+    }
+    return nullptr;
+}
+
 int dispatch_k1_impl(lora_b200_decoder *d, K1Scratch &ks, const float2 *iq, size_t n, uint32_t *bins, float *mags, cudaStream_t st) {
     if (!d->k1_ok) return fail(LORA_B200_EUNSUPPORTED, "FFT demodulator needs samp_rate/bandwidth == 8 and SF7..SF12");
     if (n == 0) return LORA_B200_OK;
-    if (!k1_generic()) {
-        static const char *rows = getenv("LORA_B200_K1_ROWS");
-        switch (d->cfg.sf) {
-        case 7: return launch_k1_packed(d, iq, n, bins, mags, st);
-        case 8: return launch_k1_group<8, 6, 2>(d, ks, iq, n, bins, mags, st);
-        case 9: return launch_k1_packed(d, iq, n, bins, mags, st);
-        case 10: return launch_k1_sf10(d, ks, iq, n, bins, mags, st);
-        case 11: case 12:
-            if (!(rows && rows[0] == '0')) return launch_k1_rows(d, ks, iq, n, bins, mags, st);
-            break;
+    static const char *rows = getenv("LORA_B200_K1_ROWS");
+    const int sf = (int)d->cfg.sf;
+    const bool generic = k1_generic() || (sf >= 11 && rows && rows[0] == '0');
+    const K1Launcher launch = k1_launcher(sf, generic);
+    if (!launch) return fail(LORA_B200_EUNSUPPORTED, "unsupported SF %u", d->cfg.sf);
+    // the kernels that split a symbol (every SF12 kernel, the generic one at SF11) merge partial argmax keys in ks.packed
+    const bool split = sf == 12 || (sf == 11 && generic);
+    if (split) {
+        if (ks.packed_cap < n) {
+            if (ks.packed) cudaFree(ks.packed);
+            ks.packed = nullptr; ks.packed_cap = 0;
+            CU(cudaMalloc(&ks.packed, sizeof(unsigned long long) * n));
+            ks.packed_cap = n;
         }
+        CU(cudaMemsetAsync(ks.packed, 0, sizeof(unsigned long long) * n, st));
     }
-    switch (d->cfg.sf) {
-    case 7: return launch_k1<7>(d, ks, iq, n, bins, mags, st);
-    case 8: return launch_k1<8>(d, ks, iq, n, bins, mags, st);
-    case 9: return launch_k1<9>(d, ks, iq, n, bins, mags, st);
-    case 10: return launch_k1<10>(d, ks, iq, n, bins, mags, st);
-    case 11: return launch_k1<11>(d, ks, iq, n, bins, mags, st);
-    case 12: return launch_k1<12>(d, ks, iq, n, bins, mags, st);
+    char err[256] = {0};
+    const K1Launch k{K1Args{iq, tab<float2>(d, d->toff.down), tab<float2>(d, d->toff.tw), n},
+                     (const float2 *)(d->h_tables.data() + d->toff.tw), bins, mags, split ? ks.packed : nullptr,
+                     d->device, d->n_sms, st, err, sizeof err};
+    if (launch(k)) return fail(LORA_B200_ECUDA, "K1: %s", err);
+    d->launches++;
+    if (split) {
+        k1_finalize_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(ks.packed, n, bins, mags);
+        d->launches++;
+        CU(cudaGetLastError());
     }
-    return fail(LORA_B200_EUNSUPPORTED, "unsupported SF %u", d->cfg.sf);
+    return LORA_B200_OK;
 }
 
 // K1 on stream `st` with scratch `ks`: a launch that follows one on ANOTHER stream with the same scratch waits for it
@@ -344,11 +296,8 @@ int launch_rx_t(lora_b200_decoder *d, const RxParams &p, int grid, cudaStream_t 
     size_t smem = 0;
     if (FFT) {
         smem = sizeof(float2) * K1Cfg<SF>::SMEM_ELEMS;
-        static bool attr_set[64] = {};
-        if (!attr_set[d->device & 63]) {
-            CU(cudaFuncSetAttribute(rx_stream_kernel<SF, FFT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-            attr_set[d->device & 63] = true;
-        }
+        static DeviceOnce once;
+        CU(once(d->device, [&] { return cudaFuncSetAttribute(rx_stream_kernel<SF, FFT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem); }));
     }
     rx_stream_kernel<SF, FFT><<<grid, RX_THREADS, smem, st>>>(p);
     d->launches++;
@@ -361,12 +310,9 @@ bool rx_warp_path(const lora_b200_decoder *d) { return d->cfg.sf == 7 && d->sps 
 
 template <bool FFT>
 int launch_rx_warp(lora_b200_decoder *d, const RxParams &p, int n_streams, cudaStream_t st) {
-    static bool attr_set[64] = {};
+    static DeviceOnce once;
     const size_t smem = sizeof(RWSmem);
-    if (!attr_set[d->device & 63]) {
-        CU(cudaFuncSetAttribute(rx_warp_kernel<FFT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        attr_set[d->device & 63] = true;
-    }
+    CU(once(d->device, [&] { return cudaFuncSetAttribute(rx_warp_kernel<FFT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem); }));
     rx_warp_kernel<FFT><<<(n_streams + RW_WARPS - 1) / RW_WARPS, RW_WARPS * 32, smem, st>>>(p);
     d->launches++;
     CU(cudaGetLastError());
@@ -634,7 +580,7 @@ void lora_b200_destroy(lora_b200_decoder *d) {
     cudaDeviceSynchronize();
     cudaFree(d->d_tables); cudaFree(d->d_k2_scratch);
     for (auto &ks : d->k1s) {
-        cudaFree(ks.packed); cudaFree(ks.xs);
+        cudaFree(ks.packed);
         if (ks.done) cudaEventDestroy(ks.done);
     }
     for (int i = 0; i < 2; i++) {

@@ -372,21 +372,8 @@ rx_warp_kernel(RxParams p) {
                     __syncwarp();
                     float2 P[8], Pq;
                     w7_pass1(lane, ws.win, kc, P, Pq);
-                    const int h = lane & 1;
-                    float2 own[4], other[4];
-#pragma unroll
-                    for (int j = 0; j < 4; j++) {
-                        const float2 send = h ? P[j] : P[4 + j];
-                        own[j] = h ? P[4 + j] : P[j];
-                        other[j].x = __shfl_xor_sync(0xffffffffu, send.x, 1);
-                        other[j].y = __shfl_xor_sync(0xffffffffu, send.y, 1);
-                    }
-                    float2 other_q;
-                    other_q.x = __shfl_xor_sync(0xffffffffu, Pq.x, 1);
-                    other_q.y = __shfl_xor_sync(0xffffffffu, Pq.y, 1);
-                    unsigned long long best = w7_final(lane, kc, own, other, Pq, other_q);
-                    best = warp_max_key(best);
-                    bin = ((int)key_idx(best) + N - 1) % N;       // gradient-index convention (SURVEY A7)
+                    const unsigned long long best = w7_reduce(lane, kc, P, Pq);
+                    bin =((int)key_idx(best) + N - 1) % N;       // gradient-index convention (SURVEY A7)
                 } else {                                          // A5 :466-491
                     float *avg = ifq + sps;
 #pragma unroll

@@ -59,9 +59,9 @@ def test_k1_emulation_matches_oracle(emul, oracle, sf):
     np.testing.assert_allclose(mags, om, rtol=1e-5)
 
 
-@pytest.mark.parametrize("which", ["warp7", "group7", "group8", "group9", "group10"])
+@pytest.mark.parametrize("which", ["warp7", "group8", "group9", "group10"])
 def test_k1_fast_kernels_emulation_matches_oracle(emul, oracle, which):
-    """k1_warp.cuh (SF7, warp per symbol) and k1_group.cuh (SF7-9, group per symbol): lane/thread
+    """k1_warp.cuh (SF7, warp per symbol), k1_group.cuh (SF8-9, group per symbol) and k1_sf10.cuh: lane/thread
     functions run on the host; bins must equal the oracle on the fixture, the edge bins and on noise."""
     from golden.make_golden import k1_case
     sf = int(which[-2:]) if which[-2:].isdigit() else int(which[-1])

@@ -59,7 +59,7 @@ def _emulations(sf):
     out = [("generic", lambda L, *a: L.lb_k1_emulate(sf, *a))]
     if sf == 7:
         out.append(("warp7", lambda L, *a: L.lb_k1_emulate_warp_sf7(*a)))
-    if sf <= 10:
+    elif sf <= 10:
         out.append((f"group{sf}", lambda L, *a: L.lb_k1_emulate_group(sf, *a)))
     else:
         out.append((f"rows{sf}", lambda L, *a: L.lb_k1_emulate_rows(sf, *a)))
