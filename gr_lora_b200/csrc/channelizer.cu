@@ -10,6 +10,7 @@
 // Here every channel of channel_list is produced (one FIR bank launch, the wideband input is staged in
 // shared memory once per tile and reused by all channels), output stays in HBM for the decoder.
 #include "../../include/lora_b200.h"
+#include "cuda_owned.h"
 #include "device_once.h"
 #include <cuda_runtime.h>
 #include <cmath>
@@ -29,14 +30,15 @@ struct lora_b200_channelizer {
     int device;
     std::vector<float> channel_list, taps;
     std::vector<double> cfo, w, phase;            // per channel: applied CFO, rad/sample, rotator phase at the next output
-    float2 *d_ctaps = nullptr;                    // [n_channels][ntaps]
-    float2 *d_hist = nullptr;                     // last ntaps-1 input samples
-    double *d_phase = nullptr, *d_dphase = nullptr;
-    float2 *d_in = nullptr, *d_out = nullptr;     // internal staging for the host entry point
-    size_t in_cap = 0, out_cap = 0;               // items
+    // device memory, owned by the members and freed by the destructor (cuda_owned.h)
+    lb::DeviceBuffer<float2> d_ctaps;             // [n_channels][ntaps]
+    lb::DeviceBuffer<float2> d_hist;              // last ntaps-1 input samples
+    lb::DeviceBuffer<double> d_phase, d_dphase;
+    lb::DeviceBuffer<float2> d_in, d_out;         // internal staging for the host entry point; d_out is [n_channels][out_cap()]
     uint64_t launches = 0;
     bool conj_out = false;                        // conjugate every output sample (the hier block's optional conjugate_cc)
     std::string err;
+    size_t out_cap() const { return d_out.capacity() / n_channels; }     // items per channel
 };
 
 namespace {
@@ -155,21 +157,19 @@ lora_b200_channelizer *lora_b200_channelizer_create(float samp_rate, float cente
     c->taps = firdes_low_pass(samp_rate, (double)(bandwidth / 2) + 15000.0, 10000.0);      // lib/channelizer_impl.cc:46
     c->ntaps = (uint32_t)c->taps.size();
     c->cfo.assign(n_channels, 0.0); c->w.assign(n_channels, 0.0); c->phase.assign(n_channels, 0.0);
-    bool ok = cudaMalloc(&c->d_ctaps, sizeof(float2) * (size_t)n_channels * c->ntaps) == cudaSuccess &&
-              cudaMalloc(&c->d_hist, sizeof(float2) * c->ntaps) == cudaSuccess &&
-              cudaMalloc(&c->d_phase, sizeof(double) * n_channels) == cudaSuccess &&
-              cudaMalloc(&c->d_dphase, sizeof(double) * n_channels) == cudaSuccess &&
+    bool ok = c->d_ctaps.reserve((size_t)n_channels * c->ntaps) == cudaSuccess &&
+              c->d_hist.reserve(c->ntaps) == cudaSuccess &&
+              c->d_phase.reserve(n_channels) == cudaSuccess &&
+              c->d_dphase.reserve(n_channels) == cudaSuccess &&
               cudaMemset(c->d_hist, 0, sizeof(float2) * c->ntaps) == cudaSuccess;
     for (uint32_t ch = 0; ok && ch < n_channels; ch++) ok = upload_channel(c, ch) == LORA_B200_OK;
-    if (!ok) { cfail(nullptr, LORA_B200_ECUDA, "channelizer: device allocation failed"); lora_b200_channelizer_destroy(c); return nullptr; }
+    if (!ok) { cfail(nullptr, LORA_B200_ECUDA, "channelizer: device allocation failed"); delete c; return nullptr; }
     return c;
 }
 
 void lora_b200_channelizer_destroy(lora_b200_channelizer *c) {
     if (!c) return;
     cudaSetDevice(c->device);
-    cudaFree(c->d_ctaps); cudaFree(c->d_hist); cudaFree(c->d_phase); cudaFree(c->d_dphase);
-    cudaFree(c->d_in); cudaFree(c->d_out);
     delete c;
 }
 
@@ -228,14 +228,14 @@ int lora_b200_channelizer_work_dev(lora_b200_channelizer *c, const void *in_dev,
         if (cudaMemcpyAsync(c->d_hist, (const float2 *)in_dev + (n_in - h), sizeof(float2) * h, cudaMemcpyDeviceToDevice, st) != cudaSuccess)
             return cfail(c, LORA_B200_ECUDA, "channelizer_work: history copy failed");
     } else {
-        cudaStreamSynchronize(st);
-        std::vector<float2> tmp(h);
-        cudaMemcpy(tmp.data(), c->d_hist, sizeof(float2) * h, cudaMemcpyDeviceToHost);
-        std::vector<float2> in(n_in);
-        cudaMemcpy(in.data(), in_dev, sizeof(float2) * n_in, cudaMemcpyDeviceToHost);
-        std::vector<float2> nh(h);
+        std::vector<float2> tmp(h), in(n_in), nh(h);
+        if (cudaStreamSynchronize(st) != cudaSuccess ||
+            cudaMemcpy(tmp.data(), c->d_hist, sizeof(float2) * h, cudaMemcpyDeviceToHost) != cudaSuccess ||
+            cudaMemcpy(in.data(), in_dev, sizeof(float2) * n_in, cudaMemcpyDeviceToHost) != cudaSuccess)
+            return cfail(c, LORA_B200_ECUDA, "channelizer_work: history copy failed");
         for (size_t i = 0; i < h; i++) nh[i] = (i + n_in < h) ? tmp[i + n_in] : in[i + n_in - h];
-        cudaMemcpy(c->d_hist, nh.data(), sizeof(float2) * h, cudaMemcpyHostToDevice);
+        if (cudaMemcpy(c->d_hist, nh.data(), sizeof(float2) * h, cudaMemcpyHostToDevice) != cudaSuccess)
+            return cfail(c, LORA_B200_ECUDA, "channelizer_work: history copy failed");
     }
     for (uint32_t ch = 0; ch < c->n_channels; ch++) c->phase[ch] = fmod(c->phase[ch] + dph[ch] * (double)no, 2.0 * M_PI);
     return LORA_B200_OK;
@@ -245,19 +245,11 @@ int lora_b200_channelizer_work_host(lora_b200_channelizer *c, const void *in_hos
     if (!c || (!in_host && n_in) || !n_out) return cfail(c, LORA_B200_EINVAL, "channelizer_work_host: null argument");
     cudaSetDevice(c->device);
     const size_t no = n_in / c->decimation;
-    if (n_in > c->in_cap) {
-        cudaFree(c->d_in); c->d_in = nullptr; c->in_cap = 0;
-        if (cudaMalloc(&c->d_in, sizeof(float2) * n_in) != cudaSuccess) return cfail(c, LORA_B200_ENOMEM, "channelizer: input staging");
-        c->in_cap = n_in;
-    }
-    if (no > c->out_cap) {
-        cudaFree(c->d_out); c->d_out = nullptr; c->out_cap = 0;
-        if (cudaMalloc(&c->d_out, sizeof(float2) * no * c->n_channels) != cudaSuccess) return cfail(c, LORA_B200_ENOMEM, "channelizer: output buffer");
-        c->out_cap = no;
-    }
+    if (c->d_in.reserve(n_in) != cudaSuccess) return cfail(c, LORA_B200_ENOMEM, "channelizer: input staging");
+    if (c->d_out.reserve(no * c->n_channels) != cudaSuccess) return cfail(c, LORA_B200_ENOMEM, "channelizer: output buffer");
     if (n_in && cudaMemcpy(c->d_in, in_host, sizeof(float2) * n_in, cudaMemcpyHostToDevice) != cudaSuccess)
         return cfail(c, LORA_B200_ECUDA, "channelizer: H2D failed");
-    int rc = lora_b200_channelizer_work_dev(c, c->d_in, n_in, c->d_out, c->out_cap, n_out, nullptr);
+    int rc = lora_b200_channelizer_work_dev(c, c->d_in, n_in, c->d_out, c->out_cap(), n_out, nullptr);
     if (rc) return rc;
     if (cudaDeviceSynchronize() != cudaSuccess) return cfail(c, LORA_B200_ECUDA, "channelizer: kernel failed");
     return LORA_B200_OK;
@@ -265,15 +257,15 @@ int lora_b200_channelizer_work_host(lora_b200_channelizer *c, const void *in_hos
 
 const void *lora_b200_channelizer_output(const lora_b200_channelizer *c, uint32_t channel, size_t *stride_items) {
     if (!c || channel >= c->n_channels || !c->d_out) return nullptr;
-    if (stride_items) *stride_items = c->out_cap;
-    return c->d_out + (size_t)channel * c->out_cap;
+    if (stride_items) *stride_items = c->out_cap();
+    return c->d_out + (size_t)channel * c->out_cap();
 }
 
 int lora_b200_channelizer_read_output(const lora_b200_channelizer *c, uint32_t channel, void *host_dst, size_t n_items) {
     if (!c || channel >= c->n_channels || !c->d_out || (!host_dst && n_items)) return cfail(nullptr, LORA_B200_EINVAL, "channelizer_read_output: bad argument");
-    if (n_items > c->out_cap) return cfail(nullptr, LORA_B200_EINVAL, "channelizer_read_output: more items than the last call produced");
+    if (n_items > c->out_cap()) return cfail(nullptr, LORA_B200_EINVAL, "channelizer_read_output: more items than the last call produced");
     cudaSetDevice(c->device);
-    if (n_items && cudaMemcpy(host_dst, c->d_out + (size_t)channel * c->out_cap, sizeof(float2) * n_items, cudaMemcpyDeviceToHost) != cudaSuccess)
+    if (n_items && cudaMemcpy(host_dst, c->d_out + (size_t)channel * c->out_cap(), sizeof(float2) * n_items, cudaMemcpyDeviceToHost) != cudaSuccess)
         return cfail(nullptr, LORA_B200_ECUDA, "channelizer_read_output: D2H failed");
     return LORA_B200_OK;
 }

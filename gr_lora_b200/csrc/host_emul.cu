@@ -1,6 +1,8 @@
 // host_emul.cu -- CPU entry points for the __host__ __device__ phase functions (tests only).
 // Lets the non-GPU test-suite run the kernels' index arithmetic, twiddles and integer chain
-// on the host and compare them with the oracle.  Not part of liblora_b200.so.
+// on the host and compare them with the oracle, and drive the owning buffer type of
+// cuda_owned.h.  Not part of liblora_b200.so.
+#include "cuda_owned.h"
 #include "k1_fft.cuh"
 #include "k1_warp.cuh"
 #include "k1_group.cuh"
@@ -127,5 +129,11 @@ uint32_t lb_emul_rx_replay(const int32_t *states, const float *metrics, const in
     return n_frames;
 }
 uint32_t lb_emul_rx_frame_rec_size(void) { return (uint32_t)sizeof(lb::RxFrameRec); }
+
+// reserve(bytes[i]) in turn on one DeviceBuffer (cuda_owned.h): the cudaError_t, pointer and capacity after each
+void lb_emul_buffer_reserve(const size_t *bytes, size_t n, int *rc, void **ptr, size_t *cap) {
+    lb::DeviceBuffer<uint8_t> b;
+    for (size_t i = 0; i < n; i++) { rc[i] = (int)b.reserve(bytes[i]); ptr[i] = b.get(); cap[i] = b.capacity(); }
+}
 
 }
