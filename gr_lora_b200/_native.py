@@ -29,6 +29,12 @@ class TxFrame(C.Structure):
                 ("sync_word", C.c_uint8), ("pad", C.c_uint8 * 3)]
 
 
+class RxParams(C.Structure):
+    """struct lora_b200_rx_params (include/lora_b200.h)."""
+    _fields_ = [("sync_word", C.c_uint8), ("reserved0", C.c_uint8 * 3), ("implicit_len", C.c_uint32), ("min_preamble", C.c_uint32),
+                ("max_cfo_hz", C.c_float), ("reserved", C.c_uint32 * 4)]
+
+
 FRAME_CB = C.CFUNCTYPE(None, C.c_void_p, C.c_uint32, C.POINTER(C.c_uint8), C.c_size_t)
 
 OK, EINVAL, ECUDA, ENOMEM, EUNSUPPORTED, EOVERFLOW = 0, -1, -2, -3, -4, -5
@@ -71,6 +77,8 @@ SIGNATURES = {
     "lora_b200_work_batch_sc16": (_i, [_vp, _vp, C.c_float, _sz, _sz, _i, C.POINTER(_sz), FRAME_CB, _vp]),
     "lora_b200_work_batch_sc8": (_i, [_vp, _vp, C.c_float, _sz, _sz, _i, C.POINTER(_sz), FRAME_CB, _vp]),
     "lora_b200_frames_last": (_sz, [_vp, C.POINTER(_vp)]),
+    "lora_b200_receive": (_i, [_vp, _vp, _sz, _sz, _i, C.POINTER(RxParams), C.POINTER(_sz)]),
+    "lora_b200_rx_info_last": (_sz, [_vp, C.POINTER(_vp), C.POINTER(C.c_uint32)]),
     "lora_b200_stream_state": (_i, [_vp, _u32]),
     "lora_b200_reset": (_i, [_vp]),
     "lora_b200_set_cfo_estimate": (_i, [_vp, _i]),

@@ -10,8 +10,13 @@
 #include "k1_rows.cuh"
 #include "int_chain.cuh"
 #include "rx_stream.cuh"
+#include "rx_sync.cuh"
 #include "tx_channel.cuh"
 #include "tx_encode.cuh"
+
+#include <algorithm>
+#include <cstring>
+#include <vector>
 
 extern "C" {
 
@@ -129,6 +134,116 @@ uint32_t lb_emul_rx_replay(const int32_t *states, const float *metrics, const in
     return n_frames;
 }
 uint32_t lb_emul_rx_frame_rec_size(void) { return (uint32_t)sizeof(lb::RxFrameRec); }
+
+}  // extern "C"
+
+namespace {
+
+// the windows of rs_synchronise on the host: K1 through its CPU emulation, the bin sums as plain loops in double
+struct RsHostOps {
+    const float2 *x;
+    long long n_items;
+    const float2 *down, *up, *tw;
+    uint32_t sps, sf;
+    bool in_range(long long pos) const { return pos >= 0 && pos + (long long)sps <= n_items; }
+    unsigned long long argmax(long long pos, bool use_up) {
+        uint32_t b;
+        float m;
+        lb_k1_emulate((int)sf, x + pos, 1, use_up ? up : down, tw, &b, &m);
+        return lb::pack_key(m * m, b);
+    }
+    float2 binval(long long pos, float F, bool use_up, int bin) {
+        const float2 *ch = use_up ? up : down;
+        double re = 0.0, im = 0.0;
+        for (uint32_t n = 0; n < sps; n++) {
+            const double a = -2.0 * M_PI * ((double)F * (double)(pos + n) / sps + (double)bin * n / sps);
+            const float2 v = lb::cmul(x[pos + n], ch[n]);
+            re += v.x * cos(a) - v.y * sin(a);
+            im += v.x * sin(a) + v.y * cos(a);
+        }
+        return make_float2((float)re, (float)im);
+    }
+    float energy(long long pos) {
+        double e = 0.0;
+        for (uint32_t n = 0; n < sps; n++) e += (double)x[pos + n].x * x[pos + n].x + (double)x[pos + n].y * x[pos + n].y;
+        return (float)e;
+    }
+};
+
+// windows start + k * sps (k < cnt) of one row, de-rotated by F bins, through K1
+void rs_host_bins(const RsHostOps &o, long long start, uint32_t cnt, float F, std::vector<uint32_t> &bins) {
+    std::vector<float2> w((size_t)cnt * o.sps);
+    for (size_t i = 0; i < w.size(); i++) {
+        const double a = -2.0 * M_PI * (double)F * (double)(start + (long long)i) / o.sps;
+        const float2 v = o.x[start + (long long)i];
+        w[i] = make_float2((float)(v.x * cos(a) - v.y * sin(a)), (float)(v.x * sin(a) + v.y * cos(a)));
+    }
+    bins.resize(cnt);
+    std::vector<float> mags(cnt);
+    lb_k1_emulate((int)o.sf, w.data(), cnt, o.down, o.tw, bins.data(), mags.data());
+}
+
+}  // namespace
+
+extern "C" {
+
+// The whole dechirp-synchronised receive path (rx_sync.cuh) of one row on the host: screen, detect, synchronise, header
+// and payload rounds, integer chain.  Per synchronised frame f (at most cap): start[f], cfo_bins[f], snr_db[f],
+// status[f] (0 published, 1 header checksum failed, 2 incomplete) and, when published, its payload in
+// payload[f * 256 ..] with length len[f].  Returns the number of synchronised frames.
+uint32_t lb_emul_rx_receive(const float2 *x, size_t n_items, const float2 *down, const float2 *up, const float2 *tw, uint32_t sf,
+                            uint32_t cr, int implicit, int crc, int reduced_rate, uint32_t sync_word, uint32_t implicit_len,
+                            uint32_t min_preamble, long long *start, float *cfo_bins, float *snr_db, int32_t *status,
+                            uint8_t *payload, uint32_t *len, uint32_t cap) {
+    const uint32_t N = 1u << sf, sps = 8u * N;
+    lb::RsParams p{sps, N, 8u, sf, min_preamble ? min_preamble : 5u, {((sync_word >> 4) & 15u) * 8u % N, (sync_word & 15u) * 8u % N},
+                   (float)N / 4.0f, 1e6f};
+    RsHostOps o{x, (long long)n_items, down, up, tw, sps, sf};
+    // screen
+    std::vector<uint32_t> bins[2];
+    std::vector<float> mags[2];
+    uint32_t n[2];
+    for (int ph = 0; ph < 2; ph++) {
+        n[ph] = n_items >= sps + ph * sps / 2 ? (uint32_t)((n_items - ph * sps / 2) / sps) : 0u;
+        bins[ph].resize(n[ph] + 1);
+        mags[ph].resize(n[ph] + 1);
+        if (n[ph]) lb_k1_emulate((int)sf, x + ph * sps / 2, n[ph], down, tw, bins[ph].data(), mags[ph].data());
+    }
+    const uint32_t *bp[2] = {bins[0].data(), bins[1].data()};
+    const float *mp[2] = {mags[0].data(), mags[1].data()};
+    std::vector<lb::RsCand> cands(64);
+    long long dropped;
+    const uint32_t nc = std::min<uint32_t>(lb::rs_detect_stream(bp, mp, n, p, cands.data(), 64, &dropped), 64u);
+    lb::RxParams rp;
+    memset(&rp, 0, sizeof rp);
+    rp.sf = sf; rp.n_bins = N; rp.n_bins_hdr = N / 4; rp.sps = sps; rp.decim = 8; rp.implicit = implicit; rp.reduced_rate = reduced_rate;
+    const uint8_t phdr1 = (uint8_t)(((cr & 7u) << 5) | (crc ? 1u << 4 : 0u));
+    uint32_t nf = 0;
+    for (uint32_t c = 0; c < nc && nf < cap; c++) {
+        const lb::RsFrame r = lb::rs_synchronise(o, cands[c], p, 0);
+        if (r.status == lb::RS_REJECT) continue;
+        start[nf] = r.start; cfo_bins[nf] = r.cfo_bins; snr_db[nf] = r.snr_db; status[nf] = 2; len[nf] = 0;
+        const long long d0 = lb::rs_data0(r.start, sps);
+        if (r.status == lb::RS_OK && d0 + 8ll * sps <= (long long)n_items) {
+            std::vector<uint32_t> hb, pb;
+            rs_host_bins(o, d0, 8, r.cfo_bins, hb);
+            lb::RxStreamState st;
+            const int32_t np = lb::rs_header(&st, rp, phdr1, hb.data(), implicit_len);
+            if (np < 0) status[nf] = 1;
+            else if (d0 + (8ll + np) * sps <= (long long)n_items) {
+                rs_host_bins(o, d0 + 8ll * sps, (uint32_t)np, r.cfo_bins, pb);
+                lb::RxFrameRec fr;
+                lb::rs_frame(&st, rp, pb.data(), np, &fr, 0, nf, 1.0f);
+                const uint32_t nd = lb::decode_len_bytes(lb::decode_len_words(fr.n_cw, 0), fr.cr);
+                len[nf] = std::min<uint32_t>(fr.payload_length, 256u);
+                for (uint32_t i = 0; i < len[nf]; i++) payload[(size_t)nf * 256 + i] = i < nd ? lb::decode_byte(fr.cw, fr.n_cw, 0, fr.cr, i) : 0;
+                status[nf] = 0;
+            }
+        }
+        nf++;
+    }
+    return nf;
+}
 
 // reserve(bytes[i]) in turn on one DeviceBuffer (cuda_owned.h): the cudaError_t, pointer and capacity after each
 void lb_emul_buffer_reserve(const size_t *bytes, size_t n, int *rc, void **ptr, size_t *cap) {

@@ -9,6 +9,7 @@
 #include "k1_sf10.cuh"
 #include "k1_launch.h"
 #include "rx_stream.cuh"
+#include "rx_sync.cuh"
 #include "rx_warp.cuh"
 #include "tx_channel.cuh"
 #include "tx_encode.cuh"
@@ -125,6 +126,18 @@ struct lora_b200_decoder : A1Params {
     // marks the end of the last launch that reads them, so the next upload waits for it on the host
     DeviceBuffer<uint8_t> d_tx;
     CudaEvent tx_done;
+    // lora_b200_receive (rx_sync.cuh), all on rx_stream
+    DeviceBuffer<float2> d_rs_stage, d_rs_win;
+    DeviceBuffer<uint32_t> d_rs_bins[2], d_rs_hbins, d_rs_pbins, d_rs_ncand, d_rs_nframes, d_rs_tab;
+    DeviceBuffer<float> d_rs_mags[2];
+    DeviceBuffer<RsCand> d_rs_cands;
+    DeviceBuffer<long long> d_rs_dropped;
+    DeviceBuffer<unsigned long long> d_rs_hold;
+    DeviceBuffer<RsFrame> d_rs_frames;
+    DeviceBuffer<RxFrameRec> d_rs_recs;
+    DeviceBuffer<RxFrameOut> d_rs_out;
+    std::vector<lora_b200_rx_info> rs_info;
+    uint32_t rs_hdr_drops = 0;
 };
 
 namespace {
@@ -412,6 +425,7 @@ int rx_finish(lora_b200_decoder *d, uint32_t stream_base, uint32_t n_launch, siz
         return x.stream != y.stream ? x.stream < y.stream : x.seq < y.seq;
     });
     d->h_sorted.resize(n_frames);
+    d->rs_info.clear();                           // (lora_b200_rx_info_last describes lora_b200_receive calls only)
     for (uint32_t k = 0; k < n_frames; k++) {
         const RxFrameOut &f = d->h_frames[order[k]];
         d->h_sorted[k] = f;
@@ -993,6 +1007,221 @@ int lora_b200_tx_frames_dev(lora_b200_decoder *d, const void *up_table, const lo
                                            1.0 / (double)d->cfg.samp_rate, noise_sigma, (unsigned long long)seed, n_items, n_streams,
                                            (float2 *)out);
     return tx_launched(d, st);
+}
+
+}  // extern "C"
+
+// ---- lora_b200_receive: the dechirp-synchronised receiver (rx_sync.cuh), every launch on rx_stream ----------------------
+template <int SF>
+static int rs_launch_sync(lora_b200_decoder *d, const float2 *x, size_t stride, size_t n_items, const RsParams &rp, uint32_t cap) {
+    static DeviceOnce once;
+    const size_t smem = sizeof(float2) * K1Cfg<SF>::SMEM_ELEMS;
+    CU(once(d->device, [&] { return cudaFuncSetAttribute(rs_sync_kernel<SF>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem); }));
+    rs_sync_kernel<SF><<<d->cfg.n_streams * cap, RX_THREADS, smem, d->rx_stream>>>(
+        x, stride, n_items, tab<float2>(d, d->toff.down), tab<float2>(d, d->toff.up), tab<float2>(d, d->toff.tw), rp, d->d_rs_cands,
+        d->d_rs_ncand, cap, d->d_rs_frames, d->d_rs_nframes, d->cfg.n_streams * cap, d->d_rs_hold);
+    return launched(d);
+}
+
+static int rs_sync(lora_b200_decoder *d, const float2 *x, size_t stride, size_t n_items, const RsParams &rp, uint32_t cap) {
+    switch (d->cfg.sf) {
+    case 7: return rs_launch_sync<7>(d, x, stride, n_items, rp, cap);
+    case 8: return rs_launch_sync<8>(d, x, stride, n_items, rp, cap);
+    case 9: return rs_launch_sync<9>(d, x, stride, n_items, rp, cap);
+    case 10: return rs_launch_sync<10>(d, x, stride, n_items, rp, cap);
+    case 11: return rs_launch_sync<11>(d, x, stride, n_items, rp, cap);
+    case 12: return rs_launch_sync<12>(d, x, stride, n_items, rp, cap);
+    }
+    return fail(LORA_B200_EUNSUPPORTED, "unsupported SF %u", d->cfg.sf);
+}
+
+extern "C" {
+
+int lora_b200_receive(lora_b200_decoder *d, const void *iq, size_t n_items, size_t stride_items, int host_ptr,
+                      const lora_b200_rx_params *prm, size_t *consumed) {
+    if (!d || !consumed || (!iq && n_items)) return fail(LORA_B200_EINVAL, "null argument");
+    if (stride_items < n_items) return fail(LORA_B200_EINVAL, "stride_items %zu < n_items %zu", stride_items, n_items);
+    if (!d->k1_ok) return fail(LORA_B200_EUNSUPPORTED, "the dechirp receiver needs samp_rate/bandwidth == 8 and SF7..SF12");
+    lora_b200_rx_params P;
+    memset(&P, 0, sizeof P);
+    if (prm) P = *prm;
+    const uint32_t crc2 = d->cfg.crc ? 2u : 0u;
+    if (d->cfg.implicit && (P.implicit_len == 0 || P.implicit_len > 255u + crc2))
+        return fail(LORA_B200_EINVAL, "an implicit-header decoder needs implicit_len in 1..%u, got %u", 255u + crc2, P.implicit_len);
+    CU(cudaSetDevice(d->device));
+    const uint32_t ns = d->cfg.n_streams, sps = d->sps, N = d->n_bins, cap = d->cfg.max_frames_per_call;
+    const uint8_t sw = P.sync_word ? P.sync_word : 0x12;
+    const float fs = (float)d->samples_per_second, bin_hz = fs / (float)sps;
+    const float max_cfo = P.max_cfo_hz > 0.f && P.max_cfo_hz < d->cfg.bandwidth / 4.0f ? P.max_cfo_hz : d->cfg.bandwidth / 4.0f;
+    RsParams rp{sps, N, d->decim, d->cfg.sf, P.min_preamble ? P.min_preamble : 5u, {((sw >> 4) & 15u) * 8u % N, (sw & 15u) * 8u % N},
+                max_cfo / bin_hz, fs};
+    d->rs_info.clear();
+    d->h_sorted.clear();
+    d->rs_hdr_drops = 0;
+    const size_t guard = (size_t)(rp.min_preamble + 4u) * sps, none = ~(size_t)0;
+    std::vector<size_t> end_pub(ns, 0), hold(ns, none);
+    auto finish = [&]() {
+        for (uint32_t s = 0; s < ns; s++) {
+            size_t c = n_items > guard ? n_items - guard : 0;
+            if (hold[s] < c) c = hold[s];
+            consumed[s] = std::max(c, end_pub[s]);
+        }
+        return LORA_B200_OK;
+    };
+    if (n_items < (size_t)sps + sps / 2) return finish();
+    cudaStream_t st = d->rx_stream;
+    // the screen runs K1 straight over the rows when a row is a whole number of windows, else over a padded copy
+    const float2 *x = (const float2 *)iq;
+    size_t stride = stride_items;
+    if (host_ptr || stride % sps || ((uintptr_t)iq & 15u)) {
+        stride = (n_items + sps - 1) / sps * sps;
+        CU(d->d_rs_stage.reserve(stride * ns));
+        CU(cudaMemcpy2DAsync(d->d_rs_stage, sizeof(float2) * stride, iq, sizeof(float2) * stride_items, sizeof(float2) * n_items, ns,
+                             host_ptr ? cudaMemcpyHostToDevice : cudaMemcpyDeviceToDevice, st));
+        x = d->d_rs_stage;
+    }
+    const size_t span = (ns - 1) * stride + n_items, nw[2] = {span / sps, (span - sps / 2) / sps};
+    for (int ph = 0; ph < 2; ph++) {
+        CU(d->d_rs_bins[ph].reserve(nw[ph] + 1));
+        CU(d->d_rs_mags[ph].reserve(nw[ph] + 1));
+        if (int rc = dispatch_k1(d, d->k1s[0], x + ph * (sps / 2), nw[ph], d->d_rs_bins[ph], d->d_rs_mags[ph], st)) return rc;
+    }
+    // detect, synchronise
+    const uint32_t fcap = ns * cap;
+    CU(d->d_rs_cands.reserve(fcap));
+    CU(d->d_rs_ncand.reserve(ns));
+    CU(d->d_rs_dropped.reserve(ns));
+    CU(d->d_rs_hold.reserve(ns));
+    CU(d->d_rs_frames.reserve(fcap));
+    CU(d->d_rs_nframes.reserve(1));
+    CU(cudaMemsetAsync(d->d_rs_hold, 0xFF, sizeof(unsigned long long) * ns, st));
+    CU(cudaMemsetAsync(d->d_rs_nframes, 0, sizeof(uint32_t), st));
+    rs_detect_kernel<<<(ns + 127) / 128, 128, 0, st>>>(d->d_rs_bins[0], d->d_rs_mags[0], d->d_rs_bins[1], d->d_rs_mags[1], stride, n_items,
+                                                       ns, rp, d->d_rs_cands, cap, d->d_rs_ncand, d->d_rs_dropped);
+    if (int rc = launched(d)) return rc;
+    if (int rc = rs_sync(d, x, stride, n_items, rp, cap)) return rc;
+    uint32_t n_sync = 0;
+    std::vector<long long> dropped(ns);
+    std::vector<unsigned long long> shold(ns);
+    CU(cudaMemcpyAsync(&n_sync, d->d_rs_nframes, sizeof n_sync, cudaMemcpyDeviceToHost, st));
+    CU(cudaMemcpyAsync(dropped.data(), d->d_rs_dropped, sizeof(long long) * ns, cudaMemcpyDeviceToHost, st));
+    CU(cudaMemcpyAsync(shold.data(), d->d_rs_hold, sizeof(unsigned long long) * ns, cudaMemcpyDeviceToHost, st));
+    CU(cudaStreamSynchronize(st));
+    for (uint32_t s = 0; s < ns; s++) {
+        if (dropped[s] >= 0) hold[s] = std::min(hold[s], (size_t)dropped[s]);
+        if (shold[s] != ~0ull) hold[s] = std::min(hold[s], (size_t)(shold[s] > sps ? shold[s] - sps : 0));
+    }
+    n_sync = std::min(n_sync, fcap);
+    if (n_sync == 0) return finish();
+    // header round: 8 windows per frame, assembled and demodulated in batches of at most 256 MiB of windows
+    const size_t win_cap = std::max<size_t>(1024, ((size_t)256 << 20) / (sizeof(float2) * sps));
+    CU(d->d_rs_win.reserve(win_cap * sps));
+    CU(d->d_rs_hbins.reserve((size_t)n_sync * 8));
+    const int agrid = d->n_sms * 8;
+    for (uint32_t f0 = 0; f0 < n_sync; f0 += (uint32_t)(win_cap / 8)) {
+        const uint32_t nb = (uint32_t)std::min<size_t>(win_cap / 8, n_sync - f0);
+        rs_assemble_kernel<<<std::min<int>((int)nb, agrid), 256, 0, st>>>(x, stride, (long long)n_items, d->d_rs_frames + f0, nb, nullptr, 0,
+                                                                          nullptr, 0, nullptr, sps, d->d_rs_win);
+        if (int rc = launched(d)) return rc;
+        if (int rc = dispatch_k1(d, d->k1s[0], d->d_rs_win, (size_t)nb * 8, d->d_rs_hbins + (size_t)f0 * 8, nullptr, st)) return rc;
+    }
+    RxParams rxp;
+    memset(&rxp, 0, sizeof rxp);
+    rxp.sps = sps; rxp.n_bins = N; rxp.n_bins_hdr = d->n_bins_hdr; rxp.decim = d->decim; rxp.sf = d->cfg.sf;
+    rxp.implicit = d->cfg.implicit; rxp.reduced_rate = d->cfg.reduced_rate;
+    rs_header_kernel<<<(n_sync + 127) / 128, 128, 0, st>>>(d->d_rs_frames, d->d_rs_nframes, fcap, rxp, d->phdr1_init, d->d_rs_hbins,
+                                                           P.implicit_len);
+    if (int rc = launched(d)) return rc;
+    std::vector<RsFrame> fr(n_sync);
+    CU(cudaMemcpyAsync(fr.data(), d->d_rs_frames, sizeof(RsFrame) * n_sync, cudaMemcpyDeviceToHost, st));
+    CU(cudaStreamSynchronize(st));
+    // one frame per preamble: candidates of one stream whose starts lie within a symbol of the previous synchronised one are
+    // the same preamble (found in both screen phases); the group keeps its best member -- a decodable header first, then
+    // the higher SNR -- and only that member is held back, dropped or published
+    std::vector<uint32_t> order(n_sync), reps, pub;
+    for (uint32_t f = 0; f < n_sync; f++) order[f] = f;
+    std::sort(order.begin(), order.end(), [&](uint32_t a, uint32_t b) {
+        return fr[a].stream != fr[b].stream ? fr[a].stream < fr[b].stream : fr[a].start < fr[b].start;
+    });
+    for (uint32_t k = 0; k < n_sync; k++) {
+        const uint32_t f = order[k], prev = k ? order[k - 1] : f;
+        if (k && fr[prev].stream == fr[f].stream && fr[f].start - fr[prev].start < (long long)sps) {
+            const RsFrame &a = fr[reps.back()], &b = fr[f];
+            if ((b.n_payload >= 0) > (a.n_payload >= 0) || ((b.n_payload >= 0) == (a.n_payload >= 0) && b.snr_db > a.snr_db)) reps.back() = f;
+            continue;
+        }
+        reps.push_back(f);
+    }
+    // which frames are whole inside this call
+    for (uint32_t f : reps) {
+        const RsFrame &r = fr[f];
+        const long long d0 = rs_data0(r.start, sps);
+        if (d0 + 8ll * sps > (long long)n_items || (r.n_payload >= 0 && d0 + (8ll + r.n_payload) * sps > (long long)n_items)) {
+            hold[r.stream] = std::min(hold[r.stream], (size_t)std::max<long long>(0, r.start - (long long)sps));
+            continue;
+        }
+        if (r.n_payload < 0) { d->rs_hdr_drops++; continue; }
+        pub.push_back(f);
+    }
+    const uint32_t np = (uint32_t)pub.size();
+    if (np == 0) return finish();
+    // payload round: table pub | seq | offs | cnts, windows in batches
+    std::vector<uint32_t> tabh(4 * (size_t)np);
+    uint32_t total = 0, seq = 0;
+    for (uint32_t k = 0; k < np; k++) {
+        const RsFrame &r = fr[pub[k]];
+        seq = (k && fr[pub[k - 1]].stream == r.stream) ? seq + 1 : 0;
+        tabh[k] = pub[k]; tabh[np + k] = seq; tabh[2 * np + k] = total; tabh[3 * np + k] = (uint32_t)r.n_payload;
+        total += (uint32_t)r.n_payload;
+    }
+    CU(d->d_rs_tab.reserve(tabh.size()));
+    CU(cudaMemcpyAsync(d->d_rs_tab, tabh.data(), sizeof(uint32_t) * tabh.size(), cudaMemcpyHostToDevice, st));
+    CU(d->d_rs_pbins.reserve(std::max<uint32_t>(total, 1u)));
+    // a batch holds whole frames: the window buffer grows to the longest frame if that is more than a batch
+    size_t pwin_cap = win_cap;
+    for (uint32_t k = 0; k < np; k++) pwin_cap = std::max<size_t>(pwin_cap, tabh[3 * np + k]);
+    CU(d->d_rs_win.reserve(pwin_cap * sps));
+    const uint32_t *t_pub = d->d_rs_tab, *t_seq = t_pub + np, *t_off = t_pub + 2 * np, *t_cnt = t_pub + 3 * np;
+    for (uint32_t g0 = 0; g0 < np;) {
+        uint32_t g1 = g0, w = 0;
+        while (g1 < np && w + tabh[3 * np + g1] <= pwin_cap) w += tabh[3 * np + g1++];
+        if (w) {
+            rs_assemble_kernel<<<std::min<int>((int)(g1 - g0), agrid), 256, 0, st>>>(x, stride, (long long)n_items, d->d_rs_frames, g1 - g0,
+                                                                                    t_pub + g0, 8, t_off + g0, tabh[2 * np + g0], t_cnt + g0,
+                                                                                    sps, d->d_rs_win);
+            if (int rc = launched(d)) return rc;
+            if (int rc = dispatch_k1(d, d->k1s[0], d->d_rs_win, w, d->d_rs_pbins + tabh[2 * np + g0], nullptr, st)) return rc;
+        }
+        g0 = g1;
+    }
+    CU(d->d_rs_recs.reserve(np));
+    CU(d->d_rs_out.reserve(np));
+    rs_frame_kernel<<<(np + 127) / 128, 128, 0, st>>>(d->d_rs_frames, t_pub, t_seq, np, rxp, d->phdr1_init, d->d_rs_hbins, d->d_rs_pbins,
+                                                      t_off, P.implicit_len, d->d_rs_recs);
+    if (int rc = launched(d)) return rc;
+    CU(cudaMemcpyAsync(d->d_rs_nframes, &np, sizeof np, cudaMemcpyHostToDevice, st));
+    k8_frames_kernel<<<(int)std::min<uint32_t>(np, (uint32_t)d->n_sms * 4u), 128, 0, st>>>(d->d_rs_recs, d->d_rs_nframes, np, d->d_rs_out);
+    if (int rc = launched(d)) return rc;
+    d->h_sorted.resize(np);
+    CU(cudaMemcpyAsync(d->h_sorted.data(), d->d_rs_out, sizeof(RxFrameOut) * np, cudaMemcpyDeviceToHost, st));
+    CU(cudaStreamSynchronize(st));
+    d->rs_info.resize(np);
+    for (uint32_t k = 0; k < np; k++) {
+        const RsFrame &r = fr[pub[k]];
+        const long long d0 = rs_data0(r.start, sps);
+        d->rs_info[k] = lora_b200_rx_info{(uint64_t)r.start, (uint64_t)d0, r.stream, r.cfo_bins * bin_hz, r.snr_db, 0u};
+        end_pub[r.stream] = std::max(end_pub[r.stream], (size_t)(d0 + (8ll + r.n_payload) * sps));
+    }
+    return finish();
+}
+
+static_assert(sizeof(lora_b200_rx_info) == 32 && sizeof(lora_b200_rx_params) == 32, "lora_b200_rx_* layout");
+
+size_t lora_b200_rx_info_last(lora_b200_decoder *d, const lora_b200_rx_info **info, uint32_t *hdr_drops) {
+    if (!d || !info) { fail(LORA_B200_EINVAL, "null argument"); return 0; }
+    *info = d->rs_info.data();
+    if (hdr_drops) *hdr_drops = d->rs_hdr_drops;
+    return d->rs_info.size();
 }
 
 int lora_b200_work_batch_sc8(lora_b200_decoder *d, const void *iq_sc8, float scale, size_t n_items, size_t stride_items,

@@ -102,7 +102,7 @@ struct RxParams {
 enum RxSymbolResult { RX_SYMBOL_NEXT = 0, RX_FRAME_DONE = 1, RX_HEADER_DONE = 2 };
 
 // decoder_impl's members as the constructor leaves them (:55-66, :72-73)
-inline void rx_state_init(RxStreamState *s, uint8_t phdr1) {
+LB_HD void rx_state_init(RxStreamState *s, uint8_t phdr1) {
     memset(s, 0, sizeof *s);
     s->state = LORA_B200_DETECT;                                  // :55
     s->snr = 1.0f;                                                // the reference leaves d_snr uninitialised (oracle D4)

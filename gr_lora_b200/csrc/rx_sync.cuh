@@ -1,0 +1,412 @@
+// rx_sync.cuh -- the dechirp-synchronised receive path (lora_b200_receive): frames below the noise floor.
+//
+// The stream state machine (rx_stream.cuh, rx_warp.cuh) gates on per-sample statistics -- an autocorrelation and a Pearson
+// correlation of instantaneous frequency -- which gain nothing from the spreading factor.  This path gates on dechirped
+// windows instead, whose peak carries the full sps-fold processing gain:
+//   screen      K1 (dechirp + FFT + argmax) on every window of every stream, at hops of sps in two phases sps/2 apart
+//   detect      runs of >= min_preamble windows of one phase whose bins agree within +-1: one candidate per preamble
+//   synchronise one CTA per candidate: SFD bin (up-chirp dechirp) -> integer CFO and timing, fractional CFO from the phase
+//               advance of the preamble peak, timing to the sample by the summed energy of the frame's known symbols,
+//               sync-word check
+//   assemble    each frame's data windows, de-rotated by its CFO, contiguous -> K1 batch kernels -> bins
+//   decode      rx_symbol_commit / rx_frame_record of rx_stream.cuh over the bins, header checksum, then K8
+// A window at p dechirped with the down-chirp sees an up-chirp that started tau samples before p at bin tau / decim + F, and
+// dechirped with the up-chirp sees a down-chirp at bin -tau / decim + F (F = CFO in bins, modulo N): the preamble bin A and
+// the SFD bin B give 2F = A + B and 2 tau / decim = A - B, the N/2 ambiguity resolved by |F| <= N/4.
+// Everything a kernel decides is in the __host__ __device__ functions below, which host_emul.cu runs on the CPU.
+#pragma once
+#include "int_chain.cuh"
+#include "k1_fft.cuh"
+#include "rx_stream.cuh"
+#include "tx_encode.cuh"
+
+namespace lb {
+
+struct RsParams {
+    uint32_t sps, n_bins, decim, sf;
+    uint32_t min_preamble;             // windows of one phase
+    uint32_t sw[2];                    // sync-word bins, ((sw >> 4) & 15) * 8 and (sw & 15) * 8 (tx.modulate_frame)
+    float max_cfo_bins;                // |CFO| accepted, in bins (<= N / 4)
+    float fs;                          // samples per second
+};
+
+struct RsCand {                        // one preamble run of the screen
+    long long p_last;                  // first sample of the run's last window
+    uint32_t bin;                      // its bin
+    uint32_t run;                      // windows in the run
+    float mag;                         // mean peak magnitude of the run
+    uint32_t pad;
+};
+
+enum RsStatus { RS_OK = 0, RS_INCOMPLETE = 1, RS_REJECT = 2 };
+
+struct RsFrame {                       // a synchronised frame
+    long long start;                   // first preamble sample (in the row)
+    uint32_t stream;
+    float cfo_bins;                    // CFO in bins (BW / N Hz)
+    float snr_db;                      // estimated SNR in the LoRa bandwidth
+    int32_t status;                    // RsStatus
+    int32_t n_payload;                 // after the header round: payload symbols, -1 = header checksum failed
+    uint32_t pad;
+};
+
+// samples of a frame before its first data symbol: 8 preamble up-chirps, 2 sync symbols, 2.25 down-chirps
+LB_HD long long rs_data0(long long start, uint32_t sps) { return start + 12ll * sps + sps / 4u; }
+
+LB_HD int rs_smod(int v, int n) {      // v mod n in [-n/2, n/2)
+    v %= n;
+    if (v < 0) v += n;
+    return v >= n / 2 ? v - n : v;
+}
+
+// ---- detect: one stream's screen -> candidates --------------------------------------------------------------------------
+// bins/mags[ph] hold the windows of phase ph, window j at j * sps + ph * sps / 2, n[ph] of them.  Windows are visited in
+// order of position; a run of one phase grows while consecutive bins agree within +-1.  Runs of both phases that end within
+// two symbols of each other describe the same preamble: the one with the larger mean peak (the better aligned) is kept.
+// Writes at most cap candidates, returns how many there were (more than cap: the caller holds back from the first extra).
+LB_HD uint32_t rs_detect_stream(const uint32_t *const bins[2], const float *const mags[2], const uint32_t n[2], const RsParams &p,
+                                RsCand *out, uint32_t cap, long long *first_dropped) {
+    const int N = (int)p.n_bins;
+    uint32_t run[2] = {0, 0}, last[2] = {0, 0};
+    float msum[2] = {0.f, 0.f};
+    RsCand pend = {0, 0, 0, 0.f, 0};
+    bool have = false;
+    uint32_t cnt = 0;
+    *first_dropped = -1;
+    auto emit = [&](const RsCand &c) {
+        if (cnt < cap) out[cnt] = c;
+        else if (cnt == cap) *first_dropped = c.p_last - (long long)c.run * p.sps;
+        cnt++;
+    };
+    auto close = [&](int ph, uint32_t j_end) {     // run of phase ph whose last window is j_end - 1
+        if (run[ph] >= p.min_preamble) {
+            RsCand c;
+            c.p_last = (long long)(j_end - 1) * p.sps + ph * (p.sps / 2);
+            c.bin = last[ph]; c.run = run[ph]; c.mag = msum[ph] / (float)run[ph]; c.pad = 0;
+            if (have && c.p_last - pend.p_last < 2ll * p.sps && pend.p_last - c.p_last < 2ll * p.sps) {
+                if (c.mag > pend.mag) pend = c;
+            } else {
+                if (have) emit(pend);
+                pend = c;
+                have = true;
+            }
+        }
+        run[ph] = 0; msum[ph] = 0.f;
+    };
+    const uint32_t jmax = n[0] > n[1] ? n[0] : n[1];
+    for (uint32_t j = 0; j < jmax; j++) {
+        for (int ph = 0; ph < 2; ph++) {
+            if (j >= n[ph]) continue;
+            const uint32_t b = bins[ph][j];
+            if (run[ph] && (rs_smod((int)b - (int)last[ph], N) < -1 || rs_smod((int)b - (int)last[ph], N) > 1)) close(ph, j);
+            run[ph]++;
+            msum[ph] += mags[ph][j];
+            last[ph] = b;
+        }
+    }
+    close(0, n[0]);
+    close(1, n[1]);
+    if (have) emit(pend);
+    return cnt;
+}
+
+// ---- synchronise ---------------------------------------------------------------------------------------------------------
+// Ops gives the procedure its windows (block-collective on the device, plain loops on the host):
+//   bool in_range(long long pos)                       window [pos, pos + sps) inside the row
+//   unsigned long long argmax(long long pos, bool up)  K1 argmax key of the raw window, dechirped with the down (up) chirp
+//   float2 binval(long long pos, float F, bool up, int bin)   bin `bin` (signed, -N/2..N/2) of the window de-rotated by F bins
+//   float energy(long long pos)                        sum |x|^2 over the window
+// The dechirp tables are (1 + 1j) e^{+-j phase}: |table|^2 = 2.
+LB_HD float rs_phase_rev(float2 z) { return atan2f(z.y, z.x) * 0.15915494309189535f; }   // arg / 2 pi
+
+// score of a hypothesis (start t, CFO F bins): energy at the expected bins of the preamble, the sync word and the SFD
+#ifdef __CUDACC__
+#pragma nv_exec_check_disable
+#endif
+template <class Ops>
+LB_HD float rs_score(Ops &ops, const RsParams &p, long long t, float F) {
+    const int N = (int)p.n_bins;
+    float s = 0.f;
+    for (int i = 0; i < 12; i++) {
+        const long long pos = t + i * (long long)p.sps;
+        if (pos < 0 || !ops.in_range(pos)) continue;
+        const int bin = i == 8 ? rs_smod((int)p.sw[0], N) : i == 9 ? rs_smod((int)p.sw[1], N) : 0;
+        s += cnorm2(ops.binval(pos, F, i >= 10, bin));
+    }
+    return s;
+}
+
+#ifdef __CUDACC__
+#pragma nv_exec_check_disable
+#endif
+template <class Ops>
+LB_HD RsFrame rs_synchronise(Ops &ops, const RsCand &c, const RsParams &p, uint32_t stream) {
+    const long long sps = p.sps;
+    const int N = (int)p.n_bins;
+    const float decim = (float)p.decim;
+    RsFrame r;
+    r.start = c.p_last - (long long)c.run * sps; r.stream = stream; r.cfo_bins = 0.f; r.snr_db = 0.f;
+    r.status = RS_REJECT; r.n_payload = 0; r.pad = 0;
+    // SFD: the window 2..6 symbols after the run's last one with the strongest up-chirp dechirp
+    unsigned long long best = 0ull;
+    int kbest = -1;
+    for (int k = 2; k <= 6; k++) {
+        const long long pos = c.p_last + k * sps;
+        if (!ops.in_range(pos)) { r.status = RS_INCOMPLETE; return r; }
+        const unsigned long long key = ops.argmax(pos, true);
+        if (key > best) { best = key; kbest = k; }
+    }
+    const int A = (int)c.bin, B = (int)key_idx(best);
+    const float Fc = 0.5f * (float)rs_smod(A + B, N);
+    if (fabsf(Fc) > p.max_cfo_bins + 1.0f) return r;
+    const long long pd = c.p_last + kbest * sps;
+    float tau = fmodf((float)A - Fc, (float)N);
+    if (tau < 0.f) tau += (float)N;
+    const long long t0 = pd - (long long)lrintf(tau * decim) - 10 * sps;     // frame start if pd lies in the first down-chirp
+    // fractional CFO: phase advance of the preamble peak from symbol to symbol (its residual modulo one bin)
+    float2 z = make_float2(0.f, 0.f), prev = make_float2(0.f, 0.f);
+    for (int i = 1; i <= 6; i++) {
+        const long long pos = t0 + i * sps;
+        if (pos < 0 || !ops.in_range(pos)) continue;
+        const float2 x = ops.binval(pos, Fc, false, 0);
+        if (i > 1) z = cadd(z, cmul(x, cconj(prev)));
+        prev = x;
+    }
+    const float eps = rs_phase_rev(z);
+    float best_s = -1.f, Fb = 0.f;
+    long long tb = 0;
+    for (int j = -1; j <= 1; j++) {
+        const float F = Fc + eps + (float)j;
+        if (fabsf(F) > p.max_cfo_bins + 0.5f) continue;
+        const long long tj = t0 + (long long)lrintf((F - Fc) * decim);   // timing follows the CFO: tau = (A - F) decim
+        for (int m = -1; m <= 1; m++) {
+            const long long t = tj + m * sps;
+            const float s = rs_score(ops, p, t, F);
+            if (s > best_s) { best_s = s; Fb = F; tb = t; }
+        }
+    }
+    if (best_s < 0.f) return r;
+    // timing to the sample: +-decim/2 around the best hypothesis
+    long long tf = tb;
+    for (int d = -(int)p.decim / 2; d <= (int)p.decim / 2; d++) {
+        if (d == 0) continue;
+        const float s = rs_score(ops, p, tb + d, Fb);
+        if (s > best_s) { best_s = s; tf = tb + d; }
+    }
+    // the residual CFO at the final timing
+    z = make_float2(0.f, 0.f);
+    float pk = 0.f, en = 0.f;
+    int npk = 0;
+    for (int i = 0; i < 8; i++) {
+        const long long pos = tf + i * sps;
+        if (pos < 0 || !ops.in_range(pos)) continue;
+        const float2 x = ops.binval(pos, Fb, false, 0);
+        if (npk) z = cadd(z, cmul(x, cconj(prev)));
+        prev = x;
+        if (i >= 1 && i <= 6) { pk += cnorm2(x); en += ops.energy(pos); }
+        npk++;
+    }
+    const float F = Fb + rs_phase_rev(z);
+    // sync word: the argmax of both sync symbols (raw windows, so shifted by the CFO) within one bin of the expected one
+    const int Fi = (int)lrintf(F);
+    for (int i = 0; i < 2; i++) {
+        const long long pos = tf + (8 + i) * sps;
+        if (pos < 0 || !ops.in_range(pos)) return r;
+        const int b = (int)key_idx(ops.argmax(pos, false));
+        const int dv = rs_smod(b - Fi - (int)p.sw[i], N);
+        if (dv < -1 || dv > 1) return r;
+    }
+    if (fabsf(F) > p.max_cfo_bins) return r;
+    // SNR: |X|^2 / (2 sps) = sps S + s2, window energy = sps (S + s2)  (S: signal power, s2: noise power per sample)
+    const float px = pk / 12.0f / (float)sps, e = en / 6.0f;       // 6 windows, |table|^2 = 2
+    const float s2 = fmaxf((e - px) / (float)(sps - 1), 1e-30f);
+    const float S = fmaxf((px - s2) / (float)sps, 1e-30f);
+    r.start = tf; r.cfo_bins = F; r.snr_db = 10.0f * log10f(S / s2 * decim);
+    r.status = RS_OK;
+    return r;
+}
+
+// ---- the integer chain of one frame -------------------------------------------------------------------------------------
+// FFT demodulator's bin -> rx_symbol_commit (rx_stream.cuh) for the 8 header-block symbols.  Returns the payload symbols
+// to read, or -1 when the explicit header's checksum (or coding rate) is wrong.  implicit_len: payload bytes of an
+// implicit-header frame.
+LB_HD int32_t rs_header(RxStreamState *st, const RxParams &p, uint8_t phdr1, const uint32_t *bins, uint32_t implicit_len) {
+    rx_state_init(st, phdr1);
+    for (int k = 0; k < 8; k++) {
+        const int bin = ((int)bins[k] + (int)p.n_bins - 1) % (int)p.n_bins;
+        if (rx_symbol_commit(st, p, true, true, bin) == RX_HEADER_DONE) break;
+    }
+    if (p.implicit) {                                 // as many payload blocks as the code words of implicit_len bytes need
+        const TxCode c{p.sf, (uint32_t)(phdr1 >> 5), 0u, (phdr1 >> 4) & 1u, p.reduced_rate ? 1u : 0u};
+        st->payload_length = implicit_len;
+        st->payload_symbols = (int32_t)(tx_payload_blocks(c, implicit_len) * (c.cr + 4u));
+        return st->payload_symbols;
+    }
+    const uint32_t len = st->hdr_print[0], cr = st->hdr_print[1] >> 5, crc = (st->hdr_print[1] >> 4) & 1u;
+    const uint32_t chk = ((st->hdr_print[1] & 1u) << 4) | (st->hdr_print[2] >> 4);
+    if (cr < 1u || cr > 4u || header_checksum(len, cr, crc) != chk) return -1;
+    return st->payload_symbols;
+}
+
+// ... and the payload symbols after it; fills the frame record K8 decodes
+LB_HD void rs_frame(RxStreamState *st, const RxParams &p, const uint32_t *bins, int32_t n_payload, RxFrameRec *fr,
+                    uint32_t stream, uint32_t seq, float snr_lin) {
+    RxParams q = p;
+    q.implicit = 0;                                   // count the payload down for an implicit header too
+    for (int32_t k = 0; k < n_payload; k++) {
+        const int bin = ((int)bins[k] + (int)p.n_bins - 1) % (int)p.n_bins;
+        if (rx_symbol_commit(st, q, false, true, bin) == RX_FRAME_DONE) break;
+    }
+    st->frame_seq = seq;
+    st->snr = snr_lin;
+    rx_frame_record(fr, st, stream, p.implicit);
+    for (uint32_t k = 0; k < st->n_demod; k++) fr->cw[k] = st->demodulated[k];
+}
+
+#ifdef __CUDACC__
+// ---- kernels ---------------------------------------------------------------------------------------------------------------
+// detect: one thread per stream.  The screen's windows of row s are the K1 results starting at s * stride / sps (stride a
+// multiple of sps) in each phase array.
+__global__ void rs_detect_kernel(const uint32_t *__restrict__ bins0, const float *__restrict__ mags0, const uint32_t *__restrict__ bins1,
+                                 const float *__restrict__ mags1, size_t stride, size_t n_items, uint32_t n_streams, RsParams p,
+                                 RsCand *__restrict__ cands, uint32_t cap, uint32_t *__restrict__ n_cands,
+                                 long long *__restrict__ dropped) {
+    const uint32_t s = blockIdx.x * blockDim.x + threadIdx.x;
+    if (s >= n_streams) return;
+    const size_t base = s * (stride / p.sps);
+    const uint32_t *b[2] = {bins0 + base, bins1 + base};
+    const float *m[2] = {mags0 + base, mags1 + base};
+    const uint32_t n[2] = {(uint32_t)(n_items / p.sps), (uint32_t)(n_items >= p.sps + p.sps / 2 ? (n_items - p.sps / 2) / p.sps : 0)};
+    n_cands[s] = rs_detect_stream(b, m, n, p, cands + (size_t)s * cap, cap, dropped + s);
+}
+
+// the windows of one candidate, block-collective (all threads call every member with the same arguments)
+template <int SF>
+struct RsDevOps {
+    const float2 *x;                   // the row
+    long long n_items;
+    const float2 *down, *up, *tw;
+    uint32_t sps;
+    float2 *smem;
+    RxShared *sh;
+    LB_D bool in_range(long long pos) const { return pos >= 0 && pos + (long long)sps <= n_items; }
+    LB_D unsigned long long argmax(long long pos, bool use_up) {
+        using C = K1Cfg<SF>;
+        const int tid = threadIdx.x;
+        K1Args a{x + pos, use_up ? up : down, tw, 1};
+        unsigned long long best = 0ull;
+        float2 wtab[C::NP / C::TPS];
+        k1_combine_twiddles<SF>(a, tid, wtab);
+        for (int s = 0; s < C::S; s++) {
+            k1_pass0<SF, false>(a, 0, s, tid, smem);
+            __syncthreads();
+            k1_pass<SF, C::R1, C::SIG1>(a, tid, smem);
+            __syncthreads();
+            if (C::R2 > 1) { k1_pass<SF, (C::R2 > 1 ? C::R2 : 2), 1>(a, tid, smem); __syncthreads(); }
+            const unsigned long long k = tid < C::TPS ? k1_combine<SF>(a, s, tid, smem, wtab) : 0ull;
+            best = k > best ? k : best;
+            __syncthreads();
+        }
+        return block_max_key(best, *sh);
+    }
+    LB_D float2 binval(long long pos, float F, bool use_up, int bin) {
+        const float2 *ch = use_up ? up : down;
+        double base = (double)F * (double)pos / (double)sps;     // de-rotation phase (revolutions) at the window's first sample
+        base -= floor(base);
+        const float fb = (float)base, fr = F / (float)sps;
+        const uint32_t kb = (uint32_t)((bin % (int)sps) + (int)sps) % sps;
+        float v[2] = {0.f, 0.f};
+        for (uint32_t n = threadIdx.x; n < sps; n += RX_THREADS) {
+            float t = fmaf(fr, (float)n, fb);
+            t -= floorf(t);
+            float sn, cs;
+            sincospif(-2.0f * t, &sn, &cs);
+            float2 m = cmul(cmul(x[pos + n], __ldg(ch + n)), make_float2(cs, sn));
+            if (kb) m = cmul(m, __ldg(tw + (size_t)((unsigned long long)kb * n % sps)));
+            v[0] += m.x; v[1] += m.y;
+        }
+        block_sum<2>(v, *sh);
+        return make_float2(v[0], v[1]);
+    }
+    LB_D float energy(long long pos) {
+        float v[1] = {0.f};
+        for (uint32_t n = threadIdx.x; n < sps; n += RX_THREADS) { const float2 a = x[pos + n]; v[0] += a.x * a.x + a.y * a.y; }
+        block_sum<1>(v, *sh);
+        return v[0];
+    }
+};
+
+// synchronise: one CTA per candidate slot (stream = slot / cap); synchronised frames are appended to `frames`
+template <int SF>
+__global__ void __launch_bounds__(RX_THREADS)
+rs_sync_kernel(const float2 *__restrict__ iq, size_t stride, size_t n_items, const float2 *down, const float2 *up, const float2 *tw,
+               RsParams p, const RsCand *__restrict__ cands, const uint32_t *__restrict__ n_cands, uint32_t cap,
+               RsFrame *__restrict__ frames, uint32_t *__restrict__ n_frames, uint32_t frame_cap,
+               unsigned long long *__restrict__ hold) {
+    extern __shared__ float2 rs_dyn_smem[];
+    __shared__ RxShared sh;
+    const uint32_t s = blockIdx.x / cap, i = blockIdx.x % cap;
+    const uint32_t nc = n_cands[s];
+    if (i >= (nc < cap ? nc : cap)) return;
+    RsDevOps<SF> ops{iq + (size_t)s * stride, (long long)n_items, down, up, tw, p.sps, rs_dyn_smem, &sh};
+    const RsFrame r = rs_synchronise(ops, cands[(size_t)s * cap + i], p, s);
+    if (threadIdx.x == 0) {
+        if (r.status == RS_INCOMPLETE) atomicMin(hold + s, (unsigned long long)(r.start > 0 ? r.start : 0));
+        if (r.status == RS_OK) {
+            const uint32_t slot = atomicAdd(n_frames, 1u);
+            if (slot < frame_cap) frames[slot] = r;
+        }
+    }
+}
+
+// assemble: frame f's windows k = 0 .. cnt-1 (first data symbol `first` + k) de-rotated by its CFO into
+// out[(off_f + k) * sps ..]; off_f = f * 8 and cnt = 8 without tables (the header round).  One CTA per frame.
+// With idx, frame f is frames[idx[f]] and its windows go to (offs[f] - off_base) * sps.  Samples past n_items read 0.
+__global__ void rs_assemble_kernel(const float2 *__restrict__ iq, size_t stride, long long n_items, const RsFrame *__restrict__ frames, uint32_t n_frames,
+                                   const uint32_t *__restrict__ idx, uint32_t first, const uint32_t *__restrict__ offs, uint32_t off_base,
+                                   const uint32_t *__restrict__ cnts, uint32_t sps, float2 *__restrict__ out) {
+    for (uint32_t f = blockIdx.x; f < n_frames; f += gridDim.x) {
+        const RsFrame fr = frames[idx ? idx[f] : f];
+        const uint32_t off = offs ? offs[f] - off_base : f * 8u, cnt = cnts ? cnts[f] : 8u;
+        const float2 *x = iq + (size_t)fr.stream * stride;
+        const long long d0 = rs_data0(fr.start, sps) + (long long)first * sps;
+        const double rev = (double)fr.cfo_bins / (double)sps;     // revolutions per sample (cfo / fs)
+        for (size_t o = threadIdx.x; o < (size_t)cnt * sps; o += blockDim.x) {
+            const long long n = d0 + (long long)o;
+            double t = rev * (double)n;                            // phase reduced in double, as tx_channel.cuh
+            t -= floor(t);
+            float sn, cs;
+            sincospif(-2.0f * (float)t, &sn, &cs);
+            out[(size_t)off * sps + o] = n < n_items ? cmul(x[n], make_float2(cs, sn)) : make_float2(0.f, 0.f);
+        }
+    }
+}
+
+// header round: one thread per frame
+__global__ void rs_header_kernel(RsFrame *__restrict__ frames, const uint32_t *__restrict__ n_frames, uint32_t cap, RxParams p,
+                                 uint8_t phdr1, const uint32_t *__restrict__ bins, uint32_t implicit_len) {
+    uint32_t n = *n_frames;
+    if (n > cap) n = cap;
+    const uint32_t f = blockIdx.x * blockDim.x + threadIdx.x;
+    if (f >= n) return;
+    RxStreamState st;
+    frames[f].n_payload = rs_header(&st, p, phdr1, bins + (size_t)f * 8, implicit_len);
+}
+
+// payload round: one thread per published frame (index list `pub`), the header replayed from its bins
+__global__ void rs_frame_kernel(const RsFrame *__restrict__ frames, const uint32_t *__restrict__ pub, const uint32_t *__restrict__ seq,
+                                uint32_t n_pub, RxParams p, uint8_t phdr1, const uint32_t *__restrict__ hdr_bins,
+                                const uint32_t *__restrict__ bins, const uint32_t *__restrict__ offs, uint32_t implicit_len,
+                                RxFrameRec *__restrict__ recs) {
+    const uint32_t k = blockIdx.x * blockDim.x + threadIdx.x;
+    if (k >= n_pub) return;
+    const uint32_t f = pub[k];
+    const RsFrame fr = frames[f];
+    RxStreamState st;
+    rs_header(&st, p, phdr1, hdr_bins + (size_t)f * 8, implicit_len);
+    const float snr = exp10f(fr.snr_db / 10.0f);          // loratap's SNR byte: the estimate in dB
+    rs_frame(&st, p, bins + offs[k], fr.n_payload, recs + k, fr.stream, seq[k], snr > 1e-30f ? snr : 1e-30f);
+}
+#endif  // __CUDACC__
+
+}  // namespace lb

@@ -107,7 +107,9 @@ class decoder:
         self._handlers.append(handler)
 
     def _on_frame(self, _user, stream, data, length):
-        blob = bytes(C.string_at(data, length))
+        self._publish(int(stream), bytes(C.string_at(data, length)))
+
+    def _publish(self, stream, blob):
         self.frames.append((int(stream), blob))
         if not self.implicit and len(blob) >= 18:     # side channel only: the published bytes are never touched
             self.header_checks["ok" if parse_frame(blob).header_ok else "bad"] += 1
@@ -174,6 +176,39 @@ class decoder:
             for s in range(self.n_streams):
                 self._emit_stdout(s)
         return consumed.astype(np.int64)
+
+    RX_INFO_DTYPE = np.dtype([("start", "<u8"), ("data_start", "<u8"), ("stream", "<u4"), ("cfo_hz", "<f4"), ("snr_db", "<f4"),
+                              ("reserved", "<u4")])      # struct lora_b200_rx_info
+
+    def receive(self, iq, n_items=None, stride_items=None, host=None, sync_word=0x12, implicit_len=0, min_preamble=0,
+                max_cfo_hz=0.0):
+        """The dechirp-synchronised receiver (lora_b200_receive): decodes frames below the noise floor.  ``iq`` as for
+        work_batch (host ndarray [n_streams, n_items] or a device tensor / pointer).  Returns (consumed, frames, info):
+        consumed[s] = where stream s must be re-presented from, frames = FRAME_DTYPE records, info = RX_INFO_DTYPE records
+        (first preamble sample, first data sample, stream, CFO in Hz, SNR in dB in the LoRa bandwidth), one per frame.
+        ``self.header_drops`` counts the explicit headers of the call whose checksum failed."""
+        if isinstance(iq, np.ndarray):
+            x = np.ascontiguousarray(iq, dtype=np.complex64)
+            assert x.ndim == 2 and x.shape[0] == self.n_streams
+            ptr, n_items, stride_items, host = x.ctypes.data, x.shape[1], x.shape[1], 1
+        else:
+            ptr = _dev_ptr(iq)
+            if n_items is None and hasattr(iq, "shape"):
+                n_items = int(iq.shape[-1])
+            host = 0 if host is None else int(host)
+            if stride_items is None:
+                stride_items = n_items
+        p = N.RxParams(sync_word=int(sync_word) & 0xFF, implicit_len=int(implicit_len), min_preamble=int(min_preamble),
+                       max_cfo_hz=float(max_cfo_hz))
+        consumed = np.zeros(self.n_streams, dtype=np.uint64)
+        N.check(self._L.lora_b200_receive(self._h, ptr, int(n_items), int(stride_items), host, C.byref(p),
+                                          consumed.ctypes.data_as(C.POINTER(C.c_size_t))), "lora_b200_receive")
+        iptr, drops = C.c_void_p(0), C.c_uint32(0)
+        n = int(self._L.lora_b200_rx_info_last(self._h, C.byref(iptr), C.byref(drops)))
+        info = (np.frombuffer(C.string_at(iptr.value, n * self.RX_INFO_DTYPE.itemsize), dtype=self.RX_INFO_DTYPE) if n
+                else np.zeros(0, self.RX_INFO_DTYPE))
+        self.header_drops = int(drops.value)
+        return consumed.astype(np.int64), self.frames_last(), info
 
     def _emit_stdout(self, stream):
         if self.quiet:

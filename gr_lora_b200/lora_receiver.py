@@ -12,10 +12,15 @@ from .decoder import decoder
 class lora_receiver:
     def __init__(self, samp_rate, center_freq, channel_list, bandwidth, sf, implicit, cr, crc, reduced_rate=False,
                  conj=False, decimation=1, disable_channelization=False, disable_drift_correction=False, cfo_feedback=False,
-                 **decoder_kw):
+                 sync="reference", sync_word=0x12, implicit_len=0, **decoder_kw):
         self.samp_rate, self.center_freq, self.channel_list = samp_rate, center_freq, list(channel_list)
         self.bandwidth, self.sf, self.implicit, self.cr, self.crc = bandwidth, sf, implicit, cr, crc
         self.decimation, self.conj = decimation, conj
+        # sync="dechirp": run() goes through the dechirp-synchronised receiver (decoder.receive), which decodes below the
+        # noise floor; the default "reference" is the reference's work() state machine
+        if sync not in ("reference", "dechirp"):
+            raise ValueError(f"sync must be 'reference' or 'dechirp', got {sync!r}")
+        self.sync, self.sync_word, self.implicit_len = sync, sync_word, implicit_len
         self.disable_channelization = disable_channelization
         self.disable_drift_correction = disable_drift_correction
         self.channelizer = None
@@ -60,6 +65,9 @@ class lora_receiver:
         stays in device memory: the decoder consumes the channelizer's output buffer directly.  Only
         channel_list[0] reaches the decoder, as in the reference (lib/channelizer_impl.cc:47,56-57)."""
         if self.channelizer is None:
+            if self.sync == "dechirp":
+                x = np.ascontiguousarray(self._front(samples), np.complex64)
+                return self._run_dechirp(x, x.size, int(self.decoder.cfg.max_items_per_call or (1 << 20)))
             return self.decoder.run(self._front(samples), stream)
         x = np.asarray(samples, dtype=np.complex64)
         x = x[: (x.size // self.decimation) * self.decimation]
@@ -69,6 +77,8 @@ class lora_receiver:
         # buffer and the decoder walks over it call by call
         n_out = self.channelizer.work(x)
         ptr, stride = self.channelizer.output_ptr(0)
+        if self.sync == "dechirp":
+            return self._run_dechirp(ptr, n_out, limit) * self.decimation
         while n_out - pos_out >= need:
             n = min(limit, n_out - pos_out)
             c = int(self.decoder.work_batch(ptr + 8 * pos_out, n_items=n, stride_items=n, host=0)[0])
@@ -82,6 +92,31 @@ class lora_receiver:
                 self.channelizer.apply_cfo(cfo)      # channelizer_impl::apply_cfo, lib/channelizer_impl.cc:68-71
         return pos_out * self.decimation
 
+    def _run_dechirp(self, src, n_out, limit):
+        """decoder.receive over the channelizer's device output (src: its address) or a host capture (src: ndarray), call by
+        call under the consumed rule; every frame is published on the 'frames' port.  Returns the samples consumed.
+        A call that consumes nothing while samples remain holds a frame longer than its chunk: the next call presents a
+        chunk twice as long (receive() has no per-call size limit), so no frame is lost to the chunk size."""
+        pos, n = 0, limit
+        while pos < n_out:
+            n = min(n, n_out - pos)
+            part = src[None, pos: pos + n] if isinstance(src, np.ndarray) else src + 8 * pos
+            c, frames, _ = self.decoder.receive(part, n_items=n, stride_items=n, host=0, sync_word=self.sync_word,
+                                                implicit_len=self.implicit_len)
+            for f in frames:
+                self.decoder._publish(int(f["stream"]), bytes(f["bytes"][: int(f["len"])]))
+            c = int(c[0])
+            at_end = pos + n >= n_out
+            if c == 0:
+                if at_end:
+                    break
+                n *= 2
+                continue
+            pos += c
+            n = limit
+            if at_end:
+                break
+        return pos
     def get_sf(self):
         return self.sf
 

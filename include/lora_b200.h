@@ -233,6 +233,45 @@ typedef struct lora_b200_frame {
     uint8_t  bytes[LORA_B200_MAX_FRAME_BYTES];
 } lora_b200_frame;
 size_t lora_b200_frames_last(lora_b200_decoder *d, const lora_b200_frame **frames);
+/* ---- dechirp-synchronised receiver: frames below the noise floor (an opt-in path beside the reference state machine) ----
+ * iq = [n_streams][n_items] cf32 (row stride stride_items; host_ptr != 0: host memory, copied inside; 0: device memory).
+ * Every stream is screened by K1 (dechirp + FFT + argmax) on windows at hops of sps/2; runs of >= min_preamble windows whose
+ * bins agree within one bin are preamble candidates, each synchronised by one CTA: integer CFO and timing from the preamble and
+ * SFD bins, fractional CFO from the preamble peak's phase advance, timing to the sample, then the two sync-word symbols are
+ * checked.  Data windows are de-rotated by the frame's CFO and demodulated by the K1 batch kernels; the FFT demodulator's
+ * (bin - 1) mod N mapping and the stream path's integer chain follow.  Explicit headers whose 5-bit checksum fails are dropped
+ * (and counted); the payload CRC is not checked.  Implicit headers carry implicit_len payload bytes (0 with an implicit-header
+ * decoder: LORA_B200_EINVAL).  Needs the FFT kernels (samp_rate / bandwidth == 8, SF7..SF12), else LORA_B200_EUNSUPPORTED.
+ * Limits: |CFO| <= max_cfo_hz <= BW / 4, timing fixed per frame (no clock-drift tracking: ppm x frame length <~ 1/4 chip),
+ * one frame at a time per stream, the decoder's SF only.  The stream state machine's per-stream state is not touched.
+ * Streaming: a frame is published only when its last sample lies inside the call; consumed[s] is where the caller must
+ * re-present stream s from: the earliest preamble whose frame was incomplete, else n_items minus a guard of
+ * (min_preamble + 4) symbols, never before the end of a published frame.  consumed[s] == 0 with more samples pending means
+ * stream s holds a frame longer than this call's n_items: present a longer chunk (there is no per-call size limit; buffers
+ * grow as needed).  At most max_frames_per_call frames per stream;
+ * further preambles are held back the same way.  Frames come back through lora_b200_frames_last (delivery order: by stream,
+ * then by start), their synchronisation through lora_b200_rx_info_last. */
+typedef struct lora_b200_rx_params {
+    uint8_t  sync_word;          /* 0 = 0x12                                                    */
+    uint8_t  reserved0[3];
+    uint32_t implicit_len;       /* payload bytes of implicit-header frames (incl. CRC bytes)  */
+    uint32_t min_preamble;       /* windows of one phase (0 = 5)                                */
+    float    max_cfo_hz;         /* 0 = BW / 4; larger values are clamped to BW / 4             */
+    uint32_t reserved[4];
+} lora_b200_rx_params;
+typedef struct lora_b200_rx_info {
+    uint64_t start;              /* first preamble sample in the row of this call               */
+    uint64_t data_start;         /* first sample of the first data symbol                       */
+    uint32_t stream;
+    float    cfo_hz;
+    float    snr_db;             /* estimated SNR in the LoRa bandwidth                         */
+    uint32_t reserved;
+} lora_b200_rx_info;
+int lora_b200_receive(lora_b200_decoder *d, const void *iq, size_t n_items, size_t stride_items, int host_ptr,
+                      const lora_b200_rx_params *p, size_t *consumed /* [n_streams] */);
+/* per published frame of the last lora_b200_receive call, parallel to lora_b200_frames_last; *hdr_drops (may be NULL) =
+ * synchronised explicit-header frames dropped for a failed header checksum */
+size_t lora_b200_rx_info_last(lora_b200_decoder *d, const lora_b200_rx_info **info, uint32_t *hdr_drops);
 /* current state of a stream (LORA_B200_DETECT ...) */
 int lora_b200_stream_state(lora_b200_decoder *d, uint32_t stream);
 /* N4 (SURVEY.md 8f): the CFO estimate the reference computes in experimental_determine_cfo (lib/decoder_impl.cc:730-738:

@@ -1,0 +1,160 @@
+"""Measure the dechirp-synchronised receiver (lora_b200_receive) on the GPU and print one JSON line:
+  * sensitivity: per SF, the share of frames decoded byte-exact at SNRs around its sensitivity point (CR 4/8, explicit header,
+    random CFO within +-0.9 BW/4, random starts; --runs captures of 96 frames per point, or 32 with --quick), next to the
+    genie-timing symbol error rate of K1 at the same SNR;
+  * stages: device time per stage of a call (torch.profiler; median, min and max over --repeats profiled calls): screen (the
+    K1 launches before detection), detect, sync, assemble + K1 (data windows), integer chain (header, frame records, K8);
+  * realtime: 384 SF7 streams x 2 s (1 MS/s) with frames, wall time per call (median of repeats) and the real-time factor.
+Usage: python tools/bench_rx_sync.py [--quick]"""
+from __future__ import annotations
+
+import argparse
+import json
+import sys
+import time
+from pathlib import Path
+
+import numpy as np
+
+sys.path.insert(0, str(Path(__file__).resolve().parent.parent))
+
+BW, FS = 125000, 1e6
+POINTS = {7: (-5.0, -3.5, -2.0, 0.0), 8: (-8.0, -6.5, -5.0, -3.0), 9: (-10.5, -9.0, -7.5, -5.5), 10: (-13.0, -11.5, -10.0, -8.0),
+          11: (-15.5, -14.0, -12.5, -10.5), 12: (-18.0, -16.5, -15.0, -13.0)}
+
+
+def sigma_for(snr_db):
+    return float(np.sqrt(10 ** (-(snr_db - 10 * np.log10(FS / BW)) / 10) / 2))
+
+
+def dec(sf, rr, **kw):
+    import gr_lora_b200 as G
+    return G.decoder(FS, BW, sf, False, 4, True, rr, quiet=True, demod="fft", **kw)
+
+
+def capture(torch, sf, n_streams, per_stream, snr, seed, n_items=None, plen=10):
+    import gr_lora_b200 as G
+    from gr_lora_b200 import tx
+    rr = sf >= 11
+    rng = np.random.default_rng(seed)
+    sps = 8 << sf
+    flen = (12 + G.tx_frame_symbols(plen, sf, 4, False, True, rr)) * sps + sps // 4
+    if n_items is None:
+        n_items = per_stream * (flen + 5 * sps) + 8 * sps
+    pays = [[bytes(rng.integers(0, 256, plen, dtype=np.uint8)) for _ in range(per_stream)] for _ in range(n_streams)]
+    cfo = [[float(rng.uniform(-0.9, 0.9) * BW / 4) for _ in p] for p in pays]
+    gen = dec(sf, rr)
+    up = torch.from_numpy(tx.base_upchirp(sf).astype(np.complex64)).cuda()
+    out, placed = gen.synth_streams(pays, n_items, lead_symbols=float(rng.uniform(1, 3)), gap_symbols=4.3, cfo_hz=cfo,
+                                    noise_sigma=sigma_for(snr), seed=seed, up_table_dev=up)
+    torch.cuda.synchronize()
+    return out, placed, n_items
+
+
+def decoded(frames, placed):
+    got = {}
+    for r in frames:
+        got.setdefault(int(r["stream"]), []).append(bytes(r["bytes"][18: int(r["len"])]))
+    return sum(1 for s, _, p in placed if p in got.get(s, []))
+
+
+def genie_ser(torch, sf, snr, n=2048, seed=1):
+    """K1 on aligned symbols with known timing and no CFO (the demodulator's own limit)."""
+    from gr_lora_b200 import tx
+    d = dec(sf, False)
+    rng = np.random.default_rng(seed)
+    vals = torch.from_numpy(rng.integers(0, 1 << sf, n).astype(np.int32)).cuda()
+    x = torch.empty(n * (8 << sf), dtype=torch.complex64, device="cuda")
+    up = torch.from_numpy(tx.base_upchirp(sf).astype(np.complex64)).cuda()
+    d.tx_symbols(vals, x, n, noise_sigma=sigma_for(snr), seed=seed, up_table_dev=up)
+    bins = torch.empty(n, dtype=torch.int32, device="cuda")
+    d.demod_fft(x, n, bins)
+    torch.cuda.synchronize()
+    return float((bins != vals).float().mean().item())
+
+
+def stages(torch, rx, out, n_items):
+    from torch.profiler import ProfilerActivity, profile
+    rx.receive(out, n_items=n_items)
+    torch.cuda.synchronize()
+    with profile(activities=[ProfilerActivity.CUDA]) as prof:
+        rx.receive(out, n_items=n_items)
+        torch.cuda.synchronize()
+    ev = sorted([e for e in prof.events() if e.device_type.name == "CUDA"], key=lambda e: e.time_range.start)
+    t = {"screen": 0.0, "detect": 0.0, "sync": 0.0, "assemble_k1": 0.0, "integer_chain": 0.0, "copies": 0.0}
+    seen_detect = False
+    for e in ev:
+        name, us = e.name, e.time_range.elapsed_us()
+        if "rs_detect" in name:
+            t["detect"] += us
+            seen_detect = True
+        elif "rs_sync" in name:
+            t["sync"] += us
+        elif "rs_header" in name or "rs_frame" in name or "k8_frames" in name:
+            t["integer_chain"] += us
+        elif "Memcpy" in name or "Memset" in name or "memcpy" in name or "memset" in name:
+            t["copies"] += us
+        elif not seen_detect:
+            t["screen"] += us
+        else:
+            t["assemble_k1"] += us
+    return {k: round(v / 1e3, 3) for k, v in t.items()}
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--quick", action="store_true", help="fewer frames per point")
+    ap.add_argument("--repeats", type=int, default=5, help="timed calls of the real-time shape, and profiled calls")
+    ap.add_argument("--runs", type=int, default=3, help="independent captures (seeds) per sensitivity point")
+    a = ap.parse_args()
+    import torch
+    if not torch.cuda.is_available():
+        raise SystemExit("bench_rx_sync.py needs a CUDA device")
+    res = {"gpu": torch.cuda.get_device_name(0)}
+    try:
+        import subprocess
+        res["power_limit_w"] = subprocess.run(["nvidia-smi", "--query-gpu=power.limit", "--format=csv,noheader,nounits", "-i", "0"],
+                                              capture_output=True, text=True, timeout=30).stdout.strip()
+    except Exception:
+        res["power_limit_w"] = "unknown"
+    ns = 32 if a.quick else 96
+    curve = {}
+    for sf, pts in POINTS.items():
+        rr = sf >= 11
+        row = []
+        for snr in pts:
+            oks, n = [], 0
+            for r in range(a.runs):
+                out, placed, n_items = capture(torch, sf, ns, 1, snr, seed=sf * 100 + int(snr * 10) % 97 + 7919 * r)
+                rx = dec(sf, rr, n_streams=ns, max_items_per_call=n_items)
+                _, frames, _ = rx.receive(out, n_items=n_items)
+                oks.append(decoded(frames, placed))
+                n = len(placed)
+                rx.close()
+                del out
+            row.append({"snr_db": snr, "frames_per_run": n, "ok_per_run": oks, "frames_ok": sum(oks) / (n * a.runs),
+                        "genie_ser": genie_ser(torch, sf, snr), "genie_symbols": 2048})
+        curve[f"sf{sf}"] = row
+    res["sensitivity"] = curve
+    # config-4 shape: 384 SF7 streams x 2 s, frames 3 dB above the sensitivity point
+    out, placed, n_items = capture(torch, 7, 384, 40, 1.0, seed=4, n_items=2_000_000)
+    rx = dec(7, False, n_streams=384, max_items_per_call=n_items, max_frames_per_call=64)
+    runs = [stages(torch, rx, out, n_items) for _ in range(a.repeats)]
+    res["stages_ms"] = {k: {"median": float(np.median([r[k] for r in runs])), "min": min(r[k] for r in runs),
+                            "max": max(r[k] for r in runs)} for k in runs[0]}
+    times = []
+    for _ in range(a.repeats):
+        torch.cuda.synchronize()
+        t0 = time.perf_counter()
+        _, frames, _ = rx.receive(out, n_items=n_items)
+        times.append(time.perf_counter() - t0)
+    med = float(np.median(times))
+    res["realtime"] = {"streams": 384, "seconds_per_stream": n_items / FS, "frames_placed": len(placed),
+                       "frames_decoded": decoded(frames, placed), "call_s_median": round(med, 4),
+                       "call_s_min": round(min(times), 4), "call_s_max": round(max(times), 4),
+                       "realtime_factor": round(384 * n_items / FS / med, 1)}
+    print(json.dumps(res))
+
+
+if __name__ == "__main__":
+    main()
