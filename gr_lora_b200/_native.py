@@ -32,7 +32,7 @@ class TxFrame(C.Structure):
 class RxParams(C.Structure):
     """struct lora_b200_rx_params (include/lora_b200.h)."""
     _fields_ = [("sync_word", C.c_uint8), ("reserved0", C.c_uint8 * 3), ("implicit_len", C.c_uint32), ("min_preamble", C.c_uint32),
-                ("max_cfo_hz", C.c_float), ("reserved", C.c_uint32 * 4)]
+                ("max_cfo_hz", C.c_float), ("sfo_ppm", C.c_float), ("reserved1", C.c_uint32), ("carrier_hz", C.c_double)]
 
 
 FRAME_CB = C.CFUNCTYPE(None, C.c_void_p, C.c_uint32, C.POINTER(C.c_uint8), C.c_size_t)
@@ -70,6 +70,8 @@ SIGNATURES = {
     "lora_b200_tx_frame_symbols": (_u32, [C.POINTER(Config), _u32]),
     "lora_b200_tx_encode_dev": (_i, [_vp, _vp, _vp, _vp, _sz, _vp, _u32, _vp]),
     "lora_b200_tx_frames_dev": (_i, [_vp, _vp, C.POINTER(TxFrame), _sz, _vp, _u32, C.c_float, C.c_uint64, _sz, _sz, _vp, _vp]),
+    "lora_b200_tx_frames_sfo_dev": (_i, [_vp, _vp, C.POINTER(TxFrame), _sz, _vp, _vp, _u32, C.c_float, C.c_uint64, _sz, _sz, _vp,
+                                         _vp]),
     "lora_b200_decode_codewords_dev": (_i, [_vp, _vp, _vp, _sz, _vp, _vp, _sz, _vp, _sz, _vp, _vp]),
     "lora_b200_deinterleave_dev": (_i, [_vp, _vp, _u32, _u32, _sz, _vp, _vp]),
     "lora_b200_work": (_i, [_vp, _u32, _vp, _sz, C.POINTER(_sz), FRAME_CB, _vp]),

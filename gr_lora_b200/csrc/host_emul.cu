@@ -170,13 +170,17 @@ struct RsHostOps {
     }
 };
 
-// windows start + k * sps (k < cnt) of one row, de-rotated by F bins, through K1
-void rs_host_bins(const RsHostOps &o, long long start, uint32_t cnt, float F, std::vector<uint32_t> &bins) {
+// data windows first .. first + cnt - 1 of frame r (each from its own start, rs_sym), de-rotated by its CFO, through K1
+void rs_host_bins(const RsHostOps &o, const lb::RsFrame &r, uint32_t first, uint32_t cnt, std::vector<uint32_t> &bins) {
     std::vector<float2> w((size_t)cnt * o.sps);
-    for (size_t i = 0; i < w.size(); i++) {
-        const double a = -2.0 * M_PI * (double)F * (double)(start + (long long)i) / o.sps;
-        const float2 v = o.x[start + (long long)i];
-        w[i] = make_float2((float)(v.x * cos(a) - v.y * sin(a)), (float)(v.x * sin(a) + v.y * cos(a)));
+    for (uint32_t k = 0; k < cnt; k++) {
+        const long long s0 = lb::rs_sym(r.start, lb::rs_data_j((long long)first + k), o.sps, r.sfo_ppm);
+        for (uint32_t i = 0; i < o.sps; i++) {
+            const long long n = s0 + i;
+            const double a = -2.0 * M_PI * (double)r.cfo_bins * (double)n / o.sps;
+            const float2 v = o.x[n];
+            w[(size_t)k * o.sps + i] = make_float2((float)(v.x * cos(a) - v.y * sin(a)), (float)(v.x * sin(a) + v.y * cos(a)));
+        }
     }
     bins.resize(cnt);
     std::vector<float> mags(cnt);
@@ -187,17 +191,19 @@ void rs_host_bins(const RsHostOps &o, long long start, uint32_t cnt, float F, st
 
 extern "C" {
 
-// The whole dechirp-synchronised receive path (rx_sync.cuh) of one row on the host: screen, detect, synchronise, header
-// and payload rounds, integer chain.  Per synchronised frame f (at most cap): start[f], cfo_bins[f], snr_db[f],
-// status[f] (0 published, 1 header checksum failed, 2 incomplete) and, when published, its payload in
+// The whole dechirp-synchronised receive path (rx_sync.cuh) of one row on the host (fs = 1 MHz, BW = 125 kHz): screen,
+// detect, synchronise, header and payload rounds, integer chain.  sfo_ppm and carrier_hz as in lora_b200_rx_params.  Per
+// synchronised frame f (at most cap): start[f], cfo_bins[f], snr_db[f], status[f] (0 published, 1 header checksum failed,
+// 2 incomplete), the clock offset its windows were placed with sfo[f] (may be NULL) and, when published, its payload in
 // payload[f * 256 ..] with length len[f].  Returns the number of synchronised frames.
-uint32_t lb_emul_rx_receive(const float2 *x, size_t n_items, const float2 *down, const float2 *up, const float2 *tw, uint32_t sf,
-                            uint32_t cr, int implicit, int crc, int reduced_rate, uint32_t sync_word, uint32_t implicit_len,
-                            uint32_t min_preamble, long long *start, float *cfo_bins, float *snr_db, int32_t *status,
-                            uint8_t *payload, uint32_t *len, uint32_t cap) {
+uint32_t lb_emul_rx_receive_sfo(const float2 *x, size_t n_items, const float2 *down, const float2 *up, const float2 *tw, uint32_t sf,
+                                uint32_t cr, int implicit, int crc, int reduced_rate, uint32_t sync_word, uint32_t implicit_len,
+                                uint32_t min_preamble, float sfo_ppm, double carrier_hz, long long *start, float *cfo_bins,
+                                float *snr_db, int32_t *status, float *sfo, uint8_t *payload, uint32_t *len, uint32_t cap) {
     const uint32_t N = 1u << sf, sps = 8u * N;
-    lb::RsParams p{sps, N, 8u, sf, min_preamble ? min_preamble : 5u, {((sync_word >> 4) & 15u) * 8u % N, (sync_word & 15u) * 8u % N},
-                   (float)N / 4.0f, 1e6f};
+    const double bin_hz = 125e3 / N;
+    lb::RsParams p{sps, N, 8u, sfo_ppm, min_preamble ? min_preamble : 5u, {((sync_word >> 4) & 15u) * 8u % N, (sync_word & 15u) * 8u % N},
+                   (float)N / 4.0f, carrier_hz > 0.0 ? (float)(1e6 * bin_hz / carrier_hz) : 0.0f};
     RsHostOps o{x, (long long)n_items, down, up, tw, sps, sf};
     // screen
     std::vector<uint32_t> bins[2];
@@ -220,18 +226,20 @@ uint32_t lb_emul_rx_receive(const float2 *x, size_t n_items, const float2 *down,
     const uint8_t phdr1 = (uint8_t)(((cr & 7u) << 5) | (crc ? 1u << 4 : 0u));
     uint32_t nf = 0;
     for (uint32_t c = 0; c < nc && nf < cap; c++) {
-        const lb::RsFrame r = lb::rs_synchronise(o, cands[c], p, 0);
+        const lb::RsFrame r = lb::rs_drift(p) ? lb::rs_synchronise<true>(o, cands[c], p, 0) : lb::rs_synchronise<false>(o, cands[c], p, 0);
         if (r.status == lb::RS_REJECT) continue;
         start[nf] = r.start; cfo_bins[nf] = r.cfo_bins; snr_db[nf] = r.snr_db; status[nf] = 2; len[nf] = 0;
-        const long long d0 = lb::rs_data0(r.start, sps);
-        if (r.status == lb::RS_OK && d0 + 8ll * sps <= (long long)n_items) {
+        if (sfo) sfo[nf] = r.sfo_ppm;
+        // end of the window of data symbol n - 1
+        auto data_end = [&](long long n) { return lb::rs_sym(r.start, lb::rs_data_j(n - 1), sps, r.sfo_ppm) + (long long)sps; };
+        if (r.status == lb::RS_OK && data_end(8) <= (long long)n_items) {
             std::vector<uint32_t> hb, pb;
-            rs_host_bins(o, d0, 8, r.cfo_bins, hb);
+            rs_host_bins(o, r, 0, 8, hb);
             lb::RxStreamState st;
             const int32_t np = lb::rs_header(&st, rp, phdr1, hb.data(), implicit_len);
             if (np < 0) status[nf] = 1;
-            else if (d0 + (8ll + np) * sps <= (long long)n_items) {
-                rs_host_bins(o, d0 + 8ll * sps, (uint32_t)np, r.cfo_bins, pb);
+            else if (data_end(8ll + np) <= (long long)n_items) {
+                rs_host_bins(o, r, 8, (uint32_t)np, pb);
                 lb::RxFrameRec fr;
                 lb::rs_frame(&st, rp, pb.data(), np, &fr, 0, nf, 1.0f);
                 const uint32_t nd = lb::decode_len_bytes(lb::decode_len_words(fr.n_cw, 0), fr.cr);
@@ -243,6 +251,15 @@ uint32_t lb_emul_rx_receive(const float2 *x, size_t n_items, const float2 *down,
         nf++;
     }
     return nf;
+}
+
+// lb_emul_rx_receive_sfo without a clock offset
+uint32_t lb_emul_rx_receive(const float2 *x, size_t n_items, const float2 *down, const float2 *up, const float2 *tw, uint32_t sf,
+                            uint32_t cr, int implicit, int crc, int reduced_rate, uint32_t sync_word, uint32_t implicit_len,
+                            uint32_t min_preamble, long long *start, float *cfo_bins, float *snr_db, int32_t *status,
+                            uint8_t *payload, uint32_t *len, uint32_t cap) {
+    return lb_emul_rx_receive_sfo(x, n_items, down, up, tw, sf, cr, implicit, crc, reduced_rate, sync_word, implicit_len, min_preamble,
+                                  0.0f, 0.0, start, cfo_bins, snr_db, status, nullptr, payload, len, cap);
 }
 
 // reserve(bytes[i]) in turn on one DeviceBuffer (cuda_owned.h): the cudaError_t, pointer and capacity after each

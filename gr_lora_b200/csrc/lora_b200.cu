@@ -959,6 +959,13 @@ static_assert(sizeof(lora_b200_tx_frame) == 24 && offsetof(lora_b200_tx_frame, s
 int lora_b200_tx_frames_dev(lora_b200_decoder *d, const void *up_table, const lora_b200_tx_frame *frames, size_t n_frames,
                             const uint32_t *shifts, uint32_t max_symbols, float noise_sigma, uint64_t seed, size_t n_streams,
                             size_t n_items, void *out, void *stream) {
+    return lora_b200_tx_frames_sfo_dev(d, up_table, frames, n_frames, nullptr, shifts, max_symbols, noise_sigma, seed, n_streams,
+                                       n_items, out, stream);
+}
+
+int lora_b200_tx_frames_sfo_dev(lora_b200_decoder *d, const void *up_table, const lora_b200_tx_frame *frames, size_t n_frames,
+                                const float *sfo_ppm, const uint32_t *shifts, uint32_t max_symbols, float noise_sigma, uint64_t seed,
+                                size_t n_streams, size_t n_items, void *out, void *stream) {
     if (!d || (n_frames && (!frames || !shifts)) || (n_streams && n_items && !out)) return fail(LORA_B200_EINVAL, "null argument");
     if (n_items & 1u) return fail(LORA_B200_EINVAL, "n_items must be even");
     if (((uintptr_t)out & 15u) != 0) return fail(LORA_B200_EINVAL, "out must be 16-byte aligned");
@@ -966,11 +973,16 @@ int lora_b200_tx_frames_dev(lora_b200_decoder *d, const void *up_table, const lo
     if (n_frames >= 0xFFFFFFFFu || n_streams >= 0xFFFFFFFFu) return fail(LORA_B200_EINVAL, "too many frames or streams");
     // sort by (row, start), check placement, then one upload: row_ptr[n_streams + 1] | pad | TxFrameDesc[n_frames]
     std::vector<uint32_t> order(n_frames);
+    std::vector<double> rate(n_frames, 1.0);
+    std::vector<unsigned long long> n_rx(n_frames);
     for (size_t f = 0; f < n_frames; f++) {
         const lora_b200_tx_frame &fr = frames[f];
         if (fr.stream >= n_streams) return fail(LORA_B200_EINVAL, "frame %zu: stream %u >= n_streams %zu", f, fr.stream, n_streams);
         if (fr.n_symbols > max_symbols) return fail(LORA_B200_EINVAL, "frame %zu: n_symbols %u > max_symbols %u", f, fr.n_symbols, max_symbols);
-        const unsigned long long len = tx_frame_samples(fr.n_symbols, d->sps);
+        if (sfo_ppm && (!std::isfinite(sfo_ppm[f]) || std::fabs(sfo_ppm[f]) > 500.0f))
+            return fail(LORA_B200_EINVAL, "frame %zu: sfo_ppm %g is not finite within +-500", f, (double)sfo_ppm[f]);
+        if (sfo_ppm) rate[f] = 1.0 + 1e-6 * (double)sfo_ppm[f];
+        const unsigned long long len = n_rx[f] = tx_drifted_samples(tx_frame_samples(fr.n_symbols, d->sps), rate[f]);
         if (len > 0xFFFFFFFFull || fr.start > n_items || len > n_items - fr.start)
             return fail(LORA_B200_EINVAL, "frame %zu: samples [%llu, %llu) run past n_items %zu", f, (unsigned long long)fr.start,
                         (unsigned long long)fr.start + len, n_items);
@@ -987,11 +999,11 @@ int lora_b200_tx_frames_dev(lora_b200_decoder *d, const void *up_table, const lo
         const lora_b200_tx_frame &fr = frames[order[k]];
         if (k && frames[order[k - 1]].stream == fr.stream) {
             const lora_b200_tx_frame &pr = frames[order[k - 1]];
-            if (pr.start + tx_frame_samples(pr.n_symbols, d->sps) > fr.start)
+            if (pr.start + n_rx[order[k - 1]] > fr.start)
                 return fail(LORA_B200_EINVAL, "frames %u and %u overlap in stream %u", order[k - 1], order[k], fr.stream);
         }
         const uint32_t sync = ((((fr.sync_word >> 4) & 15u) * 8u) % d->n_bins) | ((((fr.sync_word & 15u) * 8u) % d->n_bins) << 16);
-        desc[k] = TxFrameDesc{fr.start, fr.n_symbols, fr.cfo_hz, order[k], sync};
+        desc[k] = TxFrameDesc{fr.start, fr.n_symbols, fr.cfo_hz, order[k], sync, rate[order[k]], n_rx[order[k]]};
         row_ptr[fr.stream + 1]++;
     }
     for (size_t s = 0; s < n_streams; s++) row_ptr[s + 1] += row_ptr[s];
@@ -1012,27 +1024,33 @@ int lora_b200_tx_frames_dev(lora_b200_decoder *d, const void *up_table, const lo
 }  // extern "C"
 
 // ---- lora_b200_receive: the dechirp-synchronised receiver (rx_sync.cuh), every launch on rx_stream ----------------------
-template <int SF>
+template <int SF, bool DRIFT>
 static int rs_launch_sync(lora_b200_decoder *d, const float2 *x, size_t stride, size_t n_items, const RsParams &rp, uint32_t cap) {
     static DeviceOnce once;
     const size_t smem = sizeof(float2) * K1Cfg<SF>::SMEM_ELEMS;
-    CU(once(d->device, [&] { return cudaFuncSetAttribute(rs_sync_kernel<SF>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem); }));
-    rs_sync_kernel<SF><<<d->cfg.n_streams * cap, RX_THREADS, smem, d->rx_stream>>>(
+    CU(once(d->device, [&] { return cudaFuncSetAttribute(rs_sync_kernel<SF, DRIFT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem); }));
+    rs_sync_kernel<SF, DRIFT><<<d->cfg.n_streams * cap, RX_THREADS, smem, d->rx_stream>>>(
         x, stride, n_items, tab<float2>(d, d->toff.down), tab<float2>(d, d->toff.up), tab<float2>(d, d->toff.tw), rp, d->d_rs_cands,
         d->d_rs_ncand, cap, d->d_rs_frames, d->d_rs_nframes, d->cfg.n_streams * cap, d->d_rs_hold);
     return launched(d);
 }
 
-static int rs_sync(lora_b200_decoder *d, const float2 *x, size_t stride, size_t n_items, const RsParams &rp, uint32_t cap) {
+template <bool DRIFT>
+static int rs_sync_sf(lora_b200_decoder *d, const float2 *x, size_t stride, size_t n_items, const RsParams &rp, uint32_t cap) {
     switch (d->cfg.sf) {
-    case 7: return rs_launch_sync<7>(d, x, stride, n_items, rp, cap);
-    case 8: return rs_launch_sync<8>(d, x, stride, n_items, rp, cap);
-    case 9: return rs_launch_sync<9>(d, x, stride, n_items, rp, cap);
-    case 10: return rs_launch_sync<10>(d, x, stride, n_items, rp, cap);
-    case 11: return rs_launch_sync<11>(d, x, stride, n_items, rp, cap);
-    case 12: return rs_launch_sync<12>(d, x, stride, n_items, rp, cap);
+    case 7: return rs_launch_sync<7, DRIFT>(d, x, stride, n_items, rp, cap);
+    case 8: return rs_launch_sync<8, DRIFT>(d, x, stride, n_items, rp, cap);
+    case 9: return rs_launch_sync<9, DRIFT>(d, x, stride, n_items, rp, cap);
+    case 10: return rs_launch_sync<10, DRIFT>(d, x, stride, n_items, rp, cap);
+    case 11: return rs_launch_sync<11, DRIFT>(d, x, stride, n_items, rp, cap);
+    case 12: return rs_launch_sync<12, DRIFT>(d, x, stride, n_items, rp, cap);
     }
     return fail(LORA_B200_EUNSUPPORTED, "unsupported SF %u", d->cfg.sf);
+}
+
+// without a clock offset the synchroniser runs its DRIFT = false instantiation, which does no drift arithmetic
+static int rs_sync(lora_b200_decoder *d, const float2 *x, size_t stride, size_t n_items, const RsParams &rp, uint32_t cap) {
+    return rs_drift(rp) ? rs_sync_sf<true>(d, x, stride, n_items, rp, cap) : rs_sync_sf<false>(d, x, stride, n_items, rp, cap);
 }
 
 extern "C" {
@@ -1048,13 +1066,20 @@ int lora_b200_receive(lora_b200_decoder *d, const void *iq, size_t n_items, size
     const uint32_t crc2 = d->cfg.crc ? 2u : 0u;
     if (d->cfg.implicit && (P.implicit_len == 0 || P.implicit_len > 255u + crc2))
         return fail(LORA_B200_EINVAL, "an implicit-header decoder needs implicit_len in 1..%u, got %u", 255u + crc2, P.implicit_len);
+    if (!std::isfinite(P.sfo_ppm) || std::fabs(P.sfo_ppm) > 500.0f)
+        return fail(LORA_B200_EINVAL, "sfo_ppm must be finite and within +-500, got %g", (double)P.sfo_ppm);
+    if (P.carrier_hz != 0.0 && !(std::isfinite(P.carrier_hz) && P.carrier_hz > d->samples_per_second))
+        return fail(LORA_B200_EINVAL, "carrier_hz must be 0 or above the sample rate %g, got %g", d->samples_per_second, P.carrier_hz);
     CU(cudaSetDevice(d->device));
     const uint32_t ns = d->cfg.n_streams, sps = d->sps, N = d->n_bins, cap = d->cfg.max_frames_per_call;
     const uint8_t sw = P.sync_word ? P.sync_word : 0x12;
     const float fs = (float)d->samples_per_second, bin_hz = fs / (float)sps;
     const float max_cfo = P.max_cfo_hz > 0.f && P.max_cfo_hz < d->cfg.bandwidth / 4.0f ? P.max_cfo_hz : d->cfg.bandwidth / 4.0f;
-    RsParams rp{sps, N, d->decim, d->cfg.sf, P.min_preamble ? P.min_preamble : 5u, {((sw >> 4) & 15u) * 8u % N, (sw & 15u) * 8u % N},
-                max_cfo / bin_hz, fs};
+    const float ppm_per_bin = P.carrier_hz > 0.0 ? (float)(1e6 * (double)bin_hz / P.carrier_hz) : 0.0f;
+    RsParams rp{sps, N, d->decim, P.sfo_ppm, P.min_preamble ? P.min_preamble : 5u, {((sw >> 4) & 15u) * 8u % N, (sw & 15u) * 8u % N},
+                max_cfo / bin_hz, ppm_per_bin};
+    // end of the window of data symbol n - 1 of a frame (its first n data symbols inside the row)
+    auto data_end = [&](const RsFrame &r, long long n) { return rs_sym(r.start, rs_data_j(n - 1), sps, r.sfo_ppm) + (long long)sps; };
     d->rs_info.clear();
     d->h_sorted.clear();
     d->rs_hdr_drops = 0;
@@ -1155,8 +1180,7 @@ int lora_b200_receive(lora_b200_decoder *d, const void *iq, size_t n_items, size
     // which frames are whole inside this call
     for (uint32_t f : reps) {
         const RsFrame &r = fr[f];
-        const long long d0 = rs_data0(r.start, sps);
-        if (d0 + 8ll * sps > (long long)n_items || (r.n_payload >= 0 && d0 + (8ll + r.n_payload) * sps > (long long)n_items)) {
+        if (data_end(r, 8) > (long long)n_items || (r.n_payload >= 0 && data_end(r, 8ll + r.n_payload) > (long long)n_items)) {
             hold[r.stream] = std::min(hold[r.stream], (size_t)std::max<long long>(0, r.start - (long long)sps));
             continue;
         }
@@ -1208,14 +1232,15 @@ int lora_b200_receive(lora_b200_decoder *d, const void *iq, size_t n_items, size
     d->rs_info.resize(np);
     for (uint32_t k = 0; k < np; k++) {
         const RsFrame &r = fr[pub[k]];
-        const long long d0 = rs_data0(r.start, sps);
-        d->rs_info[k] = lora_b200_rx_info{(uint64_t)r.start, (uint64_t)d0, r.stream, r.cfo_bins * bin_hz, r.snr_db, 0u};
-        end_pub[r.stream] = std::max(end_pub[r.stream], (size_t)(d0 + (8ll + r.n_payload) * sps));
+        const long long d0 = rs_sym(r.start, rs_data_j(0), sps, r.sfo_ppm);
+        d->rs_info[k] = lora_b200_rx_info{(uint64_t)r.start, (uint64_t)d0, r.stream, r.cfo_bins * bin_hz, r.snr_db, r.sfo_ppm};
+        end_pub[r.stream] = std::max(end_pub[r.stream], (size_t)data_end(r, 8ll + r.n_payload));
     }
     return finish();
 }
 
-static_assert(sizeof(lora_b200_rx_info) == 32 && sizeof(lora_b200_rx_params) == 32, "lora_b200_rx_* layout");
+static_assert(sizeof(lora_b200_rx_info) == 32 && sizeof(lora_b200_rx_params) == 32 && offsetof(lora_b200_rx_params, sfo_ppm) == 16 &&
+              offsetof(lora_b200_rx_params, carrier_hz) == 24 && offsetof(lora_b200_rx_info, sfo_ppm) == 28, "lora_b200_rx_* layout");
 
 size_t lora_b200_rx_info_last(lora_b200_decoder *d, const lora_b200_rx_info **info, uint32_t *hdr_drops) {
     if (!d || !info) { fail(LORA_B200_EINVAL, "null argument"); return 0; }

@@ -23,11 +23,12 @@
 namespace lb {
 
 struct RsParams {
-    uint32_t sps, n_bins, decim, sf;
+    uint32_t sps, n_bins, decim;
+    float sfo_ppm;                     // clock offset of every frame, in ppm (0: none)
     uint32_t min_preamble;             // windows of one phase
     uint32_t sw[2];                    // sync-word bins, ((sw >> 4) & 15) * 8 and (sw & 15) * 8 (tx.modulate_frame)
     float max_cfo_bins;                // |CFO| accepted, in bins (<= N / 4)
-    float fs;                          // samples per second
+    float ppm_per_bin;                 // clock offset per bin of CFO: 1e6 * bin_hz / carrier_hz (0: no carrier given)
 };
 
 struct RsCand {                        // one preamble run of the screen
@@ -47,11 +48,34 @@ struct RsFrame {                       // a synchronised frame
     float snr_db;                      // estimated SNR in the LoRa bandwidth
     int32_t status;                    // RsStatus
     int32_t n_payload;                 // after the header round: payload symbols, -1 = header checksum failed
-    uint32_t pad;
+    float sfo_ppm;                     // the clock offset its windows are placed with
 };
 
-// samples of a frame before its first data symbol: 8 preamble up-chirps, 2 sync symbols, 2.25 down-chirps
-LB_HD long long rs_data0(long long start, uint32_t sps) { return start + 12ll * sps + sps / 4u; }
+// ---- clock offset ----------------------------------------------------------------------------------------------------------
+// delta = ppm * 1e-6.  delta > 0: the transmitter's clock is fast against the receiver's, and receiver sample n holds
+// transmitter time u = (n - start) (1 + delta) samples (tests/conftest.py::make_capture(sfo_ppm=...)); one crystal makes its
+// carrier high by delta * carrier_hz as well, a positive CFO.  A frame's delta is sfo_ppm * 1e-6 + cfo_hz / carrier_hz (the
+// second term 0 without a carrier frequency).  TX symbol position j counts from the frame start: 0..7 preamble, 8, 9 sync
+// word, 10..12.25 SFD, 12.25 + k data symbol k.  It starts at receiver sample start + llround(j sps / (1 + delta)), which is
+// exactly start + j sps at delta = 0.  Every window of a frame is placed by this rule, each at its own rounded start.
+LB_HD long long rs_sym(long long start, double j, uint32_t sps, float ppm) {
+    const double u = j * (double)sps;                 // (exact: j is a multiple of 1/4 and sps of 4)
+    return start + (ppm == 0.f ? (long long)u : llround(u / (1.0 + 1e-6 * (double)ppm)));   // (no division at delta = 0)
+}
+
+// TX symbol position of data symbol k: 8 preamble up-chirps, 2 sync symbols, 2.25 down-chirps come first
+LB_HD double rs_data_j(long long k) { return 12.25 + (double)k; }
+
+// the clock offset (ppm) of a hypothesis with CFO F bins
+LB_HD float rs_ppm(const RsParams &p, float F) { return p.sfo_ppm + F * p.ppm_per_bin; }
+
+// whether a call places windows with a clock offset at all; without one the synchroniser is instantiated with DRIFT = false
+// and does no drift arithmetic (rs_pos = start + j sps, the clock offset 0)
+LB_HD bool rs_drift(const RsParams &p) { return p.sfo_ppm != 0.f || p.ppm_per_bin != 0.f; }
+template <bool DRIFT> LB_HD float rs_ppm_of(const RsParams &p, float F) { return DRIFT ? rs_ppm(p, F) : 0.f; }
+template <bool DRIFT> LB_HD long long rs_pos(long long start, int j, uint32_t sps, float ppm) {
+    return DRIFT ? rs_sym(start, j, sps, ppm) : start + (long long)j * sps;
+}
 
 LB_HD int rs_smod(int v, int n) {      // v mod n in [-n/2, n/2)
     v %= n;
@@ -119,16 +143,19 @@ LB_HD uint32_t rs_detect_stream(const uint32_t *const bins[2], const float *cons
 // The dechirp tables are (1 + 1j) e^{+-j phase}: |table|^2 = 2.
 LB_HD float rs_phase_rev(float2 z) { return atan2f(z.y, z.x) * 0.15915494309189535f; }   // arg / 2 pi
 
-// score of a hypothesis (start t, CFO F bins): energy at the expected bins of the preamble, the sync word and the SFD
+// score of a hypothesis (start rs_sym(t, m), CFO F bins, windows placed with its clock offset): energy at the expected bins
+// of the preamble, the sync word and the SFD.  The windows are placed from t, so that hypotheses a symbol apart (m = -1, 0,
+// 1) score the very same windows, whatever the clock offset.
 #ifdef __CUDACC__
 #pragma nv_exec_check_disable
 #endif
-template <class Ops>
-LB_HD float rs_score(Ops &ops, const RsParams &p, long long t, float F) {
+template <bool DRIFT, class Ops>
+LB_HD float rs_score(Ops &ops, const RsParams &p, long long t, int m, float F) {
     const int N = (int)p.n_bins;
+    const float ppm = rs_ppm_of<DRIFT>(p, F);
     float s = 0.f;
     for (int i = 0; i < 12; i++) {
-        const long long pos = t + i * (long long)p.sps;
+        const long long pos = rs_pos<DRIFT>(t, i + m, p.sps, ppm);
         if (pos < 0 || !ops.in_range(pos)) continue;
         const int bin = i == 8 ? rs_smod((int)p.sw[0], N) : i == 9 ? rs_smod((int)p.sw[1], N) : 0;
         s += cnorm2(ops.binval(pos, F, i >= 10, bin));
@@ -139,14 +166,14 @@ LB_HD float rs_score(Ops &ops, const RsParams &p, long long t, float F) {
 #ifdef __CUDACC__
 #pragma nv_exec_check_disable
 #endif
-template <class Ops>
+template <bool DRIFT, class Ops>
 LB_HD RsFrame rs_synchronise(Ops &ops, const RsCand &c, const RsParams &p, uint32_t stream) {
     const long long sps = p.sps;
     const int N = (int)p.n_bins;
     const float decim = (float)p.decim;
     RsFrame r;
     r.start = c.p_last - (long long)c.run * sps; r.stream = stream; r.cfo_bins = 0.f; r.snr_db = 0.f;
-    r.status = RS_REJECT; r.n_payload = 0; r.pad = 0;
+    r.status = RS_REJECT; r.n_payload = 0; r.sfo_ppm = 0.f;
     // SFD: the window 2..6 symbols after the run's last one with the strongest up-chirp dechirp
     unsigned long long best = 0ull;
     int kbest = -1;
@@ -159,14 +186,17 @@ LB_HD RsFrame rs_synchronise(Ops &ops, const RsCand &c, const RsParams &p, uint3
     const int A = (int)c.bin, B = (int)key_idx(best);
     const float Fc = 0.5f * (float)rs_smod(A + B, N);
     if (fabsf(Fc) > p.max_cfo_bins + 1.0f) return r;
-    const long long pd = c.p_last + kbest * sps;
     float tau = fmodf((float)A - Fc, (float)N);
     if (tau < 0.f) tau += (float)N;
-    const long long t0 = pd - (long long)lrintf(tau * decim) - 10 * sps;     // frame start if pd lies in the first down-chirp
+    // frame start if the SFD window (kbest symbols after the run's last window) lies in the first down-chirp, TX symbol
+    // position 10: the run's last window, whose bin gave tau, then lies in preamble symbol 10 - kbest
+    const float rc = rs_ppm_of<DRIFT>(p, Fc);
+    const long long t0 = DRIFT ? c.p_last - (long long)lrintf(tau * decim) - rs_pos<DRIFT>(0, 10 - kbest, p.sps, rc)
+                               : c.p_last + kbest * sps - (long long)lrintf(tau * decim) - 10 * sps;
     // fractional CFO: phase advance of the preamble peak from symbol to symbol (its residual modulo one bin)
     float2 z = make_float2(0.f, 0.f), prev = make_float2(0.f, 0.f);
     for (int i = 1; i <= 6; i++) {
-        const long long pos = t0 + i * sps;
+        const long long pos = rs_pos<DRIFT>(t0, i, p.sps, rc);
         if (pos < 0 || !ops.in_range(pos)) continue;
         const float2 x = ops.binval(pos, Fc, false, 0);
         if (i > 1) z = cadd(z, cmul(x, cconj(prev)));
@@ -180,9 +210,8 @@ LB_HD RsFrame rs_synchronise(Ops &ops, const RsCand &c, const RsParams &p, uint3
         if (fabsf(F) > p.max_cfo_bins + 0.5f) continue;
         const long long tj = t0 + (long long)lrintf((F - Fc) * decim);   // timing follows the CFO: tau = (A - F) decim
         for (int m = -1; m <= 1; m++) {
-            const long long t = tj + m * sps;
-            const float s = rs_score(ops, p, t, F);
-            if (s > best_s) { best_s = s; Fb = F; tb = t; }
+            const float s = DRIFT ? rs_score<DRIFT>(ops, p, tj, m, F) : rs_score<DRIFT>(ops, p, tj + m * sps, 0, F);
+            if (s > best_s) { best_s = s; Fb = F; tb = rs_pos<DRIFT>(tj, m, p.sps, rs_ppm_of<DRIFT>(p, F)); }
         }
     }
     if (best_s < 0.f) return r;
@@ -190,15 +219,16 @@ LB_HD RsFrame rs_synchronise(Ops &ops, const RsCand &c, const RsParams &p, uint3
     long long tf = tb;
     for (int d = -(int)p.decim / 2; d <= (int)p.decim / 2; d++) {
         if (d == 0) continue;
-        const float s = rs_score(ops, p, tb + d, Fb);
+        const float s = rs_score<DRIFT>(ops, p, tb + d, 0, Fb);
         if (s > best_s) { best_s = s; tf = tb + d; }
     }
     // the residual CFO at the final timing
     z = make_float2(0.f, 0.f);
     float pk = 0.f, en = 0.f;
     int npk = 0;
+    const float rb = rs_ppm_of<DRIFT>(p, Fb);
     for (int i = 0; i < 8; i++) {
-        const long long pos = tf + i * sps;
+        const long long pos = rs_pos<DRIFT>(tf, i, p.sps, rb);
         if (pos < 0 || !ops.in_range(pos)) continue;
         const float2 x = ops.binval(pos, Fb, false, 0);
         if (npk) z = cadd(z, cmul(x, cconj(prev)));
@@ -209,8 +239,9 @@ LB_HD RsFrame rs_synchronise(Ops &ops, const RsCand &c, const RsParams &p, uint3
     const float F = Fb + rs_phase_rev(z);
     // sync word: the argmax of both sync symbols (raw windows, so shifted by the CFO) within one bin of the expected one
     const int Fi = (int)lrintf(F);
+    const float rf = rs_ppm_of<DRIFT>(p, F);
     for (int i = 0; i < 2; i++) {
-        const long long pos = tf + (8 + i) * sps;
+        const long long pos = rs_pos<DRIFT>(tf, 8 + i, p.sps, rf);
         if (pos < 0 || !ops.in_range(pos)) return r;
         const int b = (int)key_idx(ops.argmax(pos, false));
         const int dv = rs_smod(b - Fi - (int)p.sw[i], N);
@@ -221,7 +252,7 @@ LB_HD RsFrame rs_synchronise(Ops &ops, const RsCand &c, const RsParams &p, uint3
     const float px = pk / 12.0f / (float)sps, e = en / 6.0f;       // 6 windows, |table|^2 = 2
     const float s2 = fmaxf((e - px) / (float)(sps - 1), 1e-30f);
     const float S = fmaxf((px - s2) / (float)sps, 1e-30f);
-    r.start = tf; r.cfo_bins = F; r.snr_db = 10.0f * log10f(S / s2 * decim);
+    r.start = tf; r.cfo_bins = F; r.snr_db = 10.0f * log10f(S / s2 * decim); r.sfo_ppm = rs_ppm_of<DRIFT>(p, F);
     r.status = RS_OK;
     return r;
 }
@@ -337,7 +368,7 @@ struct RsDevOps {
 };
 
 // synchronise: one CTA per candidate slot (stream = slot / cap); synchronised frames are appended to `frames`
-template <int SF>
+template <int SF, bool DRIFT>
 __global__ void __launch_bounds__(RX_THREADS)
 rs_sync_kernel(const float2 *__restrict__ iq, size_t stride, size_t n_items, const float2 *down, const float2 *up, const float2 *tw,
                RsParams p, const RsCand *__restrict__ cands, const uint32_t *__restrict__ n_cands, uint32_t cap,
@@ -349,7 +380,7 @@ rs_sync_kernel(const float2 *__restrict__ iq, size_t stride, size_t n_items, con
     const uint32_t nc = n_cands[s];
     if (i >= (nc < cap ? nc : cap)) return;
     RsDevOps<SF> ops{iq + (size_t)s * stride, (long long)n_items, down, up, tw, p.sps, rs_dyn_smem, &sh};
-    const RsFrame r = rs_synchronise(ops, cands[(size_t)s * cap + i], p, s);
+    const RsFrame r = rs_synchronise<DRIFT>(ops, cands[(size_t)s * cap + i], p, s);
     if (threadIdx.x == 0) {
         if (r.status == RS_INCOMPLETE) atomicMin(hold + s, (unsigned long long)(r.start > 0 ? r.start : 0));
         if (r.status == RS_OK) {
@@ -361,7 +392,8 @@ rs_sync_kernel(const float2 *__restrict__ iq, size_t stride, size_t n_items, con
 
 // assemble: frame f's windows k = 0 .. cnt-1 (first data symbol `first` + k) de-rotated by its CFO into
 // out[(off_f + k) * sps ..]; off_f = f * 8 and cnt = 8 without tables (the header round).  One CTA per frame.
-// With idx, frame f is frames[idx[f]] and its windows go to (offs[f] - off_base) * sps.  Samples past n_items read 0.
+// With idx, frame f is frames[idx[f]] and its windows go to (offs[f] - off_base) * sps.  Each window is read from its own
+// start (rs_sym, the frame's clock offset); samples past n_items read 0.
 __global__ void rs_assemble_kernel(const float2 *__restrict__ iq, size_t stride, long long n_items, const RsFrame *__restrict__ frames, uint32_t n_frames,
                                    const uint32_t *__restrict__ idx, uint32_t first, const uint32_t *__restrict__ offs, uint32_t off_base,
                                    const uint32_t *__restrict__ cnts, uint32_t sps, float2 *__restrict__ out) {
@@ -369,15 +401,18 @@ __global__ void rs_assemble_kernel(const float2 *__restrict__ iq, size_t stride,
         const RsFrame fr = frames[idx ? idx[f] : f];
         const uint32_t off = offs ? offs[f] - off_base : f * 8u, cnt = cnts ? cnts[f] : 8u;
         const float2 *x = iq + (size_t)fr.stream * stride;
-        const long long d0 = rs_data0(fr.start, sps) + (long long)first * sps;
         const double rev = (double)fr.cfo_bins / (double)sps;     // revolutions per sample (cfo / fs)
-        for (size_t o = threadIdx.x; o < (size_t)cnt * sps; o += blockDim.x) {
-            const long long n = d0 + (long long)o;
-            double t = rev * (double)n;                            // phase reduced in double, as tx_channel.cuh
-            t -= floor(t);
-            float sn, cs;
-            sincospif(-2.0f * (float)t, &sn, &cs);
-            out[(size_t)off * sps + o] = n < n_items ? cmul(x[n], make_float2(cs, sn)) : make_float2(0.f, 0.f);
+        for (uint32_t k = 0; k < cnt; k++) {
+            const long long w = rs_sym(fr.start, rs_data_j((long long)first + k), sps, fr.sfo_ppm);
+            float2 *o = out + ((size_t)off + k) * sps;
+            for (uint32_t r = threadIdx.x; r < sps; r += blockDim.x) {
+                const long long n = w + (long long)r;
+                double t = rev * (double)n;                        // phase reduced in double, as tx_channel.cuh
+                t -= floor(t);
+                float sn, cs;
+                sincospif(-2.0f * (float)t, &sn, &cs);
+                o[r] = n < n_items ? cmul(x[n], make_float2(cs, sn)) : make_float2(0.f, 0.f);
+            }
         }
     }
 }

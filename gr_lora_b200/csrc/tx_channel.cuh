@@ -103,10 +103,20 @@ struct TxFrameDesc {
     float cfo_hz;
     uint32_t shift_row;
     uint32_t sync;              // bins of the two sync symbols, low and high half
+    double rate;                // 1 + delta: transmitter samples per row sample (1: no clock offset)
+    unsigned long long n_rx;    // row samples the frame covers: those with (n - start) * rate < tx_frame_samples
 };
 
 // samples of a frame: 8 preamble up-chirps, 2 sync symbols, 2.25 down-chirps (conj(up)), then the data symbols
 LB_HD unsigned long long tx_frame_samples(uint32_t n_symbols, uint32_t sps) { return (12ull + n_symbols) * sps + sps / 4u; }
+
+// row samples i >= 0 of a frame of len transmitter samples with i * rate < len, rate = 1 + delta (rx_sync.cuh's convention)
+inline unsigned long long tx_drifted_samples(unsigned long long len, double rate) {
+    unsigned long long n = (unsigned long long)ceil((double)len / rate);
+    while (n && (double)(n - 1) * rate >= (double)len) n--;
+    while ((double)n * rate < (double)len) n++;
+    return n;
+}
 
 // sample o (< tx_frame_samples) of frame fr, before the CFO rotation
 LB_D float2 tx_frame_sample(const float2 *__restrict__ up, uint32_t sps, uint32_t decim, const TxFrameDesc &fr,
@@ -122,6 +132,36 @@ LB_D float2 tx_frame_sample(const float2 *__restrict__ up, uint32_t sps, uint32_
     const uint32_t d = o - sfd_end, k = d / sps, rr = d - k * sps;
     const uint32_t sh = __ldg(shifts + (size_t)fr.shift_row * max_symbols + k) % n_bins;
     return __ldg(up + (rr + sh * decim) % sps);
+}
+
+// the same at fractional transmitter time u (a frame with a clock offset), from the phase law of tx.base_upchirp:
+// up(m) = e^{j 2 pi m (m - sps) / (2 decim sps)} for 0 <= m < sps, in double and reduced to revolutions, times up[0] (the
+// table's value at phase 0, so that its amplitude and rotation carry over); a cyclic shift by sh bins reads up at
+// (m + sh decim) mod sps, the SFD is the conjugate
+LB_D float2 tx_frame_sample_at(const float2 *__restrict__ up, uint32_t sps, uint32_t decim, const TxFrameDesc &fr,
+                               const uint32_t *__restrict__ shifts, uint32_t max_symbols, uint32_t n_bins, double u) {
+    const double S = (double)sps;
+    double q = floor(u / S), m = u - q * S;
+    bool conj = false;
+    if (q >= 8.0 && q < 10.0) {
+        m += (double)(((q == 8.0 ? fr.sync : fr.sync >> 16) & 0xFFFFu) * decim);
+    } else if (q >= 10.0) {
+        const double d = u - 12.25 * S;
+        if (d < 0.0) {
+            conj = true;
+        } else {
+            const double k = floor(d / S);
+            const uint32_t sh = __ldg(shifts + (size_t)fr.shift_row * max_symbols + (uint32_t)k) % n_bins;
+            m = d - k * S + (double)(sh * decim);
+        }
+    }
+    if (m >= S) m -= S;
+    double rev = m * (m - S) / (2.0 * (double)decim * S);
+    rev -= floor(rev);
+    float sn, cs;
+    sincospif(2.0f * (float)rev, &sn, &cs);
+    const float2 v = cmul(__ldg(up), make_float2(cs, sn));
+    return conj ? make_float2(v.x, -v.y) : v;
 }
 
 // whole streams of frames: out[s][n] = frame sample (0 outside every frame) * e^{j 2 pi cfo n / fs} + noise(seed, s, n), the
@@ -148,8 +188,9 @@ __global__ void tx_frames_kernel(const float2 *__restrict__ up, uint32_t sps, ui
             const uint32_t k = (e == 0 && frames[lo - 1].start > n) ? lo - 2 : lo - 1;
             if (k < first || k == 0xFFFFFFFFu) continue;
             const TxFrameDesc fr = frames[k];
-            if (n < fr.start || n - fr.start >= tx_frame_samples(fr.n_symbols, sps)) continue;
-            float2 a = tx_frame_sample(up, sps, decim, fr, shifts, max_symbols, n_bins, (uint32_t)(n - fr.start));
+            if (n < fr.start || n - fr.start >= fr.n_rx) continue;
+            float2 a = fr.rate == 1.0 ? tx_frame_sample(up, sps, decim, fr, shifts, max_symbols, n_bins, (uint32_t)(n - fr.start))
+                                      : tx_frame_sample_at(up, sps, decim, fr, shifts, max_symbols, n_bins, (double)(n - fr.start) * fr.rate);
             if (fr.cfo_hz != 0.0f) {                                 // as tx_symbols_kernel: phase reduced in double
                 double t = (double)fr.cfo_hz * inv_fs * (double)n;
                 t -= floor(t);

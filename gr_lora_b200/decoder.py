@@ -178,14 +178,16 @@ class decoder:
         return consumed.astype(np.int64)
 
     RX_INFO_DTYPE = np.dtype([("start", "<u8"), ("data_start", "<u8"), ("stream", "<u4"), ("cfo_hz", "<f4"), ("snr_db", "<f4"),
-                              ("reserved", "<u4")])      # struct lora_b200_rx_info
+                              ("sfo_ppm", "<f4")])       # struct lora_b200_rx_info
 
     def receive(self, iq, n_items=None, stride_items=None, host=None, sync_word=0x12, implicit_len=0, min_preamble=0,
-                max_cfo_hz=0.0):
+                max_cfo_hz=0.0, sfo_ppm=0.0, carrier_hz=0.0):
         """The dechirp-synchronised receiver (lora_b200_receive): decodes frames below the noise floor.  ``iq`` as for
         work_batch (host ndarray [n_streams, n_items] or a device tensor / pointer).  Returns (consumed, frames, info):
         consumed[s] = where stream s must be re-presented from, frames = FRAME_DTYPE records, info = RX_INFO_DTYPE records
-        (first preamble sample, first data sample, stream, CFO in Hz, SNR in dB in the LoRa bandwidth), one per frame.
+        (first preamble sample, first data sample, stream, CFO in Hz, SNR in dB in the LoRa bandwidth, clock offset in ppm),
+        one per frame.  Clock offset of a frame: sfo_ppm, plus its CFO / carrier_hz when carrier_hz (the channel's RF
+        frequency) is given -- one crystal sets a radio's carrier and its sample clock.
         ``self.header_drops`` counts the explicit headers of the call whose checksum failed."""
         if isinstance(iq, np.ndarray):
             x = np.ascontiguousarray(iq, dtype=np.complex64)
@@ -199,7 +201,7 @@ class decoder:
             if stride_items is None:
                 stride_items = n_items
         p = N.RxParams(sync_word=int(sync_word) & 0xFF, implicit_len=int(implicit_len), min_preamble=int(min_preamble),
-                       max_cfo_hz=float(max_cfo_hz))
+                       max_cfo_hz=float(max_cfo_hz), sfo_ppm=float(sfo_ppm), carrier_hz=float(carrier_hz))
         consumed = np.zeros(self.n_streams, dtype=np.uint64)
         N.check(self._L.lora_b200_receive(self._h, ptr, int(n_items), int(stride_items), host, C.byref(p),
                                           consumed.ctypes.data_as(C.POINTER(C.c_size_t))), "lora_b200_receive")
@@ -316,26 +318,39 @@ class decoder:
                                                _dev_ptr(shifts_dev), int(max_symbols), int(cuda_stream)), "lora_b200_tx_encode_dev")
 
     def tx_frames(self, frames, shifts_dev, max_symbols, n_streams, n_items, out_dev, noise_sigma=0.0, seed=0, up_table_dev=None,
-                  cuda_stream=0):
+                  cuda_stream=0, sfo_ppm=None):
         """Whole streams of frames on the device: out_dev [n_streams, n_items] cf32.  frames: structured array of TX_FRAME_DTYPE
-        (host, any order); frame f's data symbols are shifts_dev[f * max_symbols ..]."""
+        (host, any order); frame f's data symbols are shifts_dev[f * max_symbols ..].  sfo_ppm: None, or one clock offset
+        per frame (lora_b200_tx_frames_sfo_dev)."""
         fr = np.ascontiguousarray(frames, dtype=self.TX_FRAME_DTYPE)
-        N.check(self._L.lora_b200_tx_frames_dev(self._h, _dev_ptr(up_table_dev), C.cast(fr.ctypes.data, C.POINTER(N.TxFrame)), fr.size,
-                                               _dev_ptr(shifts_dev), int(max_symbols), float(noise_sigma), int(seed), int(n_streams),
-                                               int(n_items), _dev_ptr(out_dev), int(cuda_stream)), "lora_b200_tx_frames_dev")
+        if sfo_ppm is None:
+            N.check(self._L.lora_b200_tx_frames_dev(self._h, _dev_ptr(up_table_dev), C.cast(fr.ctypes.data, C.POINTER(N.TxFrame)),
+                                                   fr.size, _dev_ptr(shifts_dev), int(max_symbols), float(noise_sigma), int(seed),
+                                                   int(n_streams), int(n_items), _dev_ptr(out_dev), int(cuda_stream)),
+                    "lora_b200_tx_frames_dev")
+            return
+        ppm = np.ascontiguousarray(sfo_ppm, dtype=np.float32)
+        if ppm.shape != fr.shape:
+            raise ValueError(f"sfo_ppm needs one value per frame: shape {ppm.shape}, frames {fr.shape}")
+        N.check(self._L.lora_b200_tx_frames_sfo_dev(self._h, _dev_ptr(up_table_dev), C.cast(fr.ctypes.data, C.POINTER(N.TxFrame)),
+                                                   fr.size, ppm.ctypes.data, _dev_ptr(shifts_dev), int(max_symbols),
+                                                   float(noise_sigma), int(seed), int(n_streams), int(n_items), _dev_ptr(out_dev),
+                                                   int(cuda_stream)), "lora_b200_tx_frames_sfo_dev")
 
     def synth_streams(self, payloads_per_stream, n_items, *, lead_symbols=3.0, gap_symbols=4.0, sync_word=0x12, cfo_hz=0.0,
-                      noise_sigma=0.0, seed=0, up_table_dev=None):
+                      noise_sigma=0.0, seed=0, up_table_dev=None, sfo_ppm=0.0):
         """Stream s of a [len(payloads_per_stream), n_items] cf32 device tensor carries the frames of payloads_per_stream[s]
         under this decoder's sf / cr / implicit / crc / reduced_rate, laid out as tx.channel does it: int(lead_symbols * sps)
         of silence, then every frame followed by int(gap_symbols * sps) of silence.  A frame is placed while it and the gap
-        after it fit in the row.  cfo_hz: one value for every frame, or a sequence per stream with one value per payload.
-        Encoding (tx_encode) and modulation (tx_frames) run on the device, on torch's current stream.
-        Returns (tensor, [(stream, start, payload) of every placed frame])."""
+        after it fit in the row.  cfo_hz and sfo_ppm (the transmitter's clock offset, tx_frames_sfo): one value for every
+        frame, or a sequence per stream with one value per payload; a frame with a clock offset is as long as
+        tx.drifted_length makes it.  Encoding (tx_encode) and modulation (tx_frames) run on the device, on torch's current
+        stream.  Returns (tensor, [(stream, start, payload) of every placed frame])."""
         import torch
+        from .tx import drifted_length
         sps, lead, gap = self.sps, int(lead_symbols * self.sps), int(gap_symbols * self.sps)
         n_sym = {}
-        placed, rows = [], []
+        placed, rows, ppms = [], [], []
         for s, pays in enumerate(payloads_per_stream):
             pos = lead
             for k, p in enumerate(pays):
@@ -344,10 +359,12 @@ class decoder:
                     n_sym[len(p)] = int(self._L.lora_b200_tx_frame_symbols(C.byref(self.cfg), len(p)))
                     if n_sym[len(p)] == 0:
                         raise ValueError(f"payload length {len(p)} is not encodable under this configuration")
-                flen = (12 + n_sym[len(p)]) * sps + sps // 4
+                ppm = float(sfo_ppm if np.isscalar(sfo_ppm) else sfo_ppm[s][k])
+                flen = drifted_length((12 + n_sym[len(p)]) * sps + sps // 4, ppm)
                 if pos + flen + gap > n_items:
                     break
                 placed.append((s, pos, p))
+                ppms.append(ppm)
                 rows.append((pos, s, n_sym[len(p)], float(cfo_hz if np.isscalar(cfo_hz) else cfo_hz[s][k]), int(sync_word) & 0xFF))
                 pos += flen + gap
         dev = torch.device("cuda", self.cfg.device if self.cfg.device >= 0 else torch.cuda.current_device())
@@ -363,7 +380,8 @@ class decoder:
         for f, (start, s, n, cfo, sw) in enumerate(rows):
             frames[f] = (start, s, n, cfo, sw, (0, 0, 0))
         out = torch.empty((len(payloads_per_stream), n_items), dtype=torch.complex64, device=dev)
-        self.tx_frames(frames, shifts, max_symbols, len(payloads_per_stream), n_items, out, noise_sigma, seed, up_table_dev, stream)
+        self.tx_frames(frames, shifts, max_symbols, len(payloads_per_stream), n_items, out, noise_sigma, seed, up_table_dev, stream,
+                       sfo_ppm=ppms if any(ppms) else None)
         return out, placed
 
     def ifreq(self, iq_dev, n_windows, window, out_dev, cuda_stream=0):

@@ -12,7 +12,7 @@ from .decoder import decoder
 class lora_receiver:
     def __init__(self, samp_rate, center_freq, channel_list, bandwidth, sf, implicit, cr, crc, reduced_rate=False,
                  conj=False, decimation=1, disable_channelization=False, disable_drift_correction=False, cfo_feedback=False,
-                 sync="reference", sync_word=0x12, implicit_len=0, **decoder_kw):
+                 sync="reference", sync_word=0x12, implicit_len=0, clock_from_carrier=False, **decoder_kw):
         self.samp_rate, self.center_freq, self.channel_list = samp_rate, center_freq, list(channel_list)
         self.bandwidth, self.sf, self.implicit, self.cr, self.crc = bandwidth, sf, implicit, cr, crc
         self.decimation, self.conj = decimation, conj
@@ -21,6 +21,12 @@ class lora_receiver:
         if sync not in ("reference", "dechirp"):
             raise ValueError(f"sync must be 'reference' or 'dechirp', got {sync!r}")
         self.sync, self.sync_word, self.implicit_len = sync, sync_word, implicit_len
+        # clock_from_carrier: the dechirp receiver places every frame's windows with the clock offset its CFO implies
+        # (cfo / carrier, one crystal sets a radio's carrier and its sample clock); the carrier is channel_list[0], or
+        # center_freq without the channelizer.  The reference state machine tracks drift itself (fine_sync).
+        if clock_from_carrier and sync != "dechirp":
+            raise ValueError("clock_from_carrier needs sync='dechirp' (the reference state machine has fine_sync)")
+        self.clock_from_carrier = bool(clock_from_carrier)
         self.disable_channelization = disable_channelization
         self.disable_drift_correction = disable_drift_correction
         self.channelizer = None
@@ -98,11 +104,14 @@ class lora_receiver:
         A call that consumes nothing while samples remain holds a frame longer than its chunk: the next call presents a
         chunk twice as long (receive() has no per-call size limit), so no frame is lost to the chunk size."""
         pos, n = 0, limit
+        carrier = 0.0
+        if self.clock_from_carrier:
+            carrier = float(self.center_freq if self.channelizer is None else self.channel_list[0])
         while pos < n_out:
             n = min(n, n_out - pos)
             part = src[None, pos: pos + n] if isinstance(src, np.ndarray) else src + 8 * pos
             c, frames, _ = self.decoder.receive(part, n_items=n, stride_items=n, host=0, sync_word=self.sync_word,
-                                                implicit_len=self.implicit_len)
+                                                implicit_len=self.implicit_len, carrier_hz=carrier)
             for f in frames:
                 self.decoder._publish(int(f["stream"]), bytes(f["bytes"][: int(f["len"])]))
             c = int(c[0])

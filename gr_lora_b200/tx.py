@@ -218,17 +218,58 @@ def modulate_shifts(shifts, sf: int, bw: float = 125e3, fs: float = 1e6) -> np.n
     return up[idx].reshape(-1)
 
 
+def drifted_length(n_samples: int, sfo_ppm: float) -> int:
+    """Receiver samples of a frame of n_samples transmitter samples sent with a clock off by sfo_ppm: those n >= 0 with
+    n (1 + delta) < n_samples, delta = float32(sfo_ppm) * 1e-6 (the arithmetic of lora_b200_tx_frames_sfo_dev)."""
+    rate = 1.0 + 1e-6 * float(np.float32(sfo_ppm))
+    n = int(math.ceil(n_samples / rate))
+    while n and (n - 1) * rate >= n_samples:
+        n -= 1
+    while n * rate < n_samples:
+        n += 1
+    return n
+
+
 def modulate_frame(fs_syms: FrameSymbols, sf: int, *, bw: float = 125e3, fs: float = 1e6,
-                   n_preamble: int = 8, sync_word: int = 0x12) -> np.ndarray:
-    """preamble | 2 sync symbols | 2.25 downchirps | data symbols (complex128, unit power)."""
+                   n_preamble: int = 8, sync_word: int = 0x12, sfo_ppm: float = 0.0) -> np.ndarray:
+    """preamble | 2 sync symbols | 2.25 downchirps | data symbols (complex128, unit power).
+
+    sfo_ppm: the transmitter's clock is off by delta = sfo_ppm * 1e-6 (> 0: fast against the receiver), so receiver sample n
+    holds transmitter time u = n (1 + delta) samples; the frame is the base_upchirp phase law evaluated at those fractional
+    times (cyclic shifts at fractional positions, the conjugate for the SFD), drifted_length() samples long.  0: exactly the
+    undrifted frame."""
     up = base_upchirp(sf, bw, fs)
     sps = up.size
     down = np.conj(up)
     n_bins = 1 << sf
     sync = [((sync_word >> 4) & 0xF) * 8 % n_bins, (sync_word & 0xF) * 8 % n_bins]
-    parts = [np.tile(up, n_preamble), modulate_shifts(sync, sf, bw, fs), down, down, down[: sps // 4],
-             modulate_shifts(fs_syms.shifts, sf, bw, fs)]
-    return np.concatenate(parts)
+    if sfo_ppm == 0:
+        parts = [np.tile(up, n_preamble), modulate_shifts(sync, sf, bw, fs), down, down, down[: sps // 4],
+                 modulate_shifts(fs_syms.shifts, sf, bw, fs)]
+        return np.concatenate(parts)
+    decim = sps // n_bins
+    n_sfd = n_preamble + 2                               # first SFD symbol
+    data0 = (n_sfd + 2) * sps + sps // 4
+    length = data0 + len(fs_syms.shifts) * sps
+    rate = 1.0 + 1e-6 * float(np.float32(sfo_ppm))
+    u = np.arange(drifted_length(length, sfo_ppm), dtype=np.float64) * rate
+    q = np.floor(u / sps)
+    m = u - q * sps                                      # position in the chirp, before any cyclic shift
+    shift = np.zeros(u.size, np.int64)
+    for i, b in enumerate(sync):
+        shift[q == n_preamble + i] = b
+    d = u - data0
+    data = d >= 0
+    k = np.floor(d[data] / sps).astype(np.int64)
+    m[data] = d[data] - k * sps
+    shift[data] = np.asarray(fs_syms.shifts, np.int64)[k] % n_bins
+    m = np.mod(m + shift * decim, sps)
+    t = m / fs
+    phase = -2.0 * np.pi * t * (bw / 2.0 + (-0.5 * bw * (bw / n_bins)) * t)
+    x = np.exp(1j * phase)
+    sfd = (q >= n_sfd) & ~data
+    x[sfd] = np.conj(x[sfd])
+    return x
 
 
 def awgn(n: int, snr_db: float, rng: np.random.Generator) -> np.ndarray:

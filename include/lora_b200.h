@@ -187,6 +187,17 @@ int lora_b200_tx_encode_dev(lora_b200_decoder *d, const uint8_t *payloads, const
 int lora_b200_tx_frames_dev(lora_b200_decoder *d, const void *up_table, const lora_b200_tx_frame *frames, size_t n_frames,
                             const uint32_t *shifts, uint32_t max_symbols, float noise_sigma, uint64_t seed, size_t n_streams,
                             size_t n_items, void *out, void *cuda_stream);
+/* tx_frames_sfo: tx_frames with frames from transmitters whose clock is off.  sfo_ppm = host float[n_frames], parallel to
+ *   frames, or NULL (= tx_frames).  Frame f's clock is off by delta = sfo_ppm[f] * 1e-6 (> 0: fast), so row sample n holds
+ *   transmitter time u = (n - start) (1 + delta) samples; the frame covers the row samples with 0 <= u < frame length, and
+ *   those are what the overlap and n_items checks see.  A frame with delta != 0 is evaluated at the fractional u from the
+ *   phase law of tx.base_upchirp, e^{j 2 pi m (m - sps) / (2 decim sps)} at chirp position m (cyclic shifts at fractional
+ *   positions, the conjugate for the SFD), in double and reduced to revolutions, times up_table[0]; tx.modulate_frame(...,
+ *   sfo_ppm) is its specification.  The CFO rotation and the noise are tx_frames'; a frame with delta = 0 is tx_frames' own.
+ *   LORA_B200_EINVAL, before any launch, for an sfo_ppm that is not finite or beyond +-500. */
+int lora_b200_tx_frames_sfo_dev(lora_b200_decoder *d, const void *up_table, const lora_b200_tx_frame *frames, size_t n_frames,
+                                const float *sfo_ppm, const uint32_t *shifts, uint32_t max_symbols, float noise_sigma, uint64_t seed,
+                                size_t n_streams, size_t n_items, void *out, void *cuda_stream);
 
 /* ---- K8: integer decode of whole code-word vectors (decode(), :567-586, B2-B4) ----
  * For each of n_vec vectors: codewords[i*stride .. +lengths[i]) -> deshuffle, dewhiten,
@@ -242,8 +253,16 @@ size_t lora_b200_frames_last(lora_b200_decoder *d, const lora_b200_frame **frame
  * (bin - 1) mod N mapping and the stream path's integer chain follow.  Explicit headers whose 5-bit checksum fails are dropped
  * (and counted); the payload CRC is not checked.  Implicit headers carry implicit_len payload bytes (0 with an implicit-header
  * decoder: LORA_B200_EINVAL).  Needs the FFT kernels (samp_rate / bandwidth == 8, SF7..SF12), else LORA_B200_EUNSUPPORTED.
- * Limits: |CFO| <= max_cfo_hz <= BW / 4, timing fixed per frame (no clock-drift tracking: ppm x frame length <~ 1/4 chip),
- * one frame at a time per stream, the decoder's SF only.  The stream state machine's per-stream state is not touched.
+ * Clock offset: a transmitter whose clock is off by delta = ppm * 1e-6 (delta > 0: fast against the receiver) sends TX symbol
+ * position j (0..7 preamble, 8, 9 sync word, 10..12.25 SFD, 12.25 + k data symbol k) at receiver sample
+ * start + llround(j * sps / (1 + delta)); every window of a frame is placed by this rule.  A frame's delta is
+ * p->sfo_ppm * 1e-6 + cfo_hz / p->carrier_hz: one crystal sets a radio's carrier and its sample clock, so with carrier_hz
+ * (the RF frequency of the channel, 0 = none) each frame's clock offset follows from its own measured CFO.  Both 0: timing
+ * fixed per frame, which holds while ppm x frame length stays below about a quarter chip.  sfo_ppm must be finite within
+ * +-500 and carrier_hz 0 or finite and above the sample rate, else LORA_B200_EINVAL.
+ * Limits: |CFO| <= max_cfo_hz <= BW / 4, no blind drift estimation (the clock offset is given or follows the CFO), data
+ * windows placed to the nearest sample, one frame at a time per stream, the decoder's SF only.  The stream state machine's
+ * per-stream state is not touched.
  * Streaming: a frame is published only when its last sample lies inside the call; consumed[s] is where the caller must
  * re-present stream s from: the earliest preamble whose frame was incomplete, else n_items minus a guard of
  * (min_preamble + 4) symbols, never before the end of a published frame.  consumed[s] == 0 with more samples pending means
@@ -257,7 +276,10 @@ typedef struct lora_b200_rx_params {
     uint32_t implicit_len;       /* payload bytes of implicit-header frames (incl. CRC bytes)  */
     uint32_t min_preamble;       /* windows of one phase (0 = 5)                                */
     float    max_cfo_hz;         /* 0 = BW / 4; larger values are clamped to BW / 4             */
-    uint32_t reserved[4];
+    float    sfo_ppm;            /* clock offset of every frame in ppm (> 0: transmitter fast)  */
+    uint32_t reserved1;
+    double   carrier_hz;         /* RF carrier of the channel: each frame's clock offset also
+                                    follows its CFO, cfo_hz / carrier_hz (0 = not given)        */
 } lora_b200_rx_params;
 typedef struct lora_b200_rx_info {
     uint64_t start;              /* first preamble sample in the row of this call               */
@@ -265,7 +287,7 @@ typedef struct lora_b200_rx_info {
     uint32_t stream;
     float    cfo_hz;
     float    snr_db;             /* estimated SNR in the LoRa bandwidth                         */
-    uint32_t reserved;
+    float    sfo_ppm;            /* clock offset its windows were placed with (0: none asked)   */
 } lora_b200_rx_info;
 int lora_b200_receive(lora_b200_decoder *d, const void *iq, size_t n_items, size_t stride_items, int host_ptr,
                       const lora_b200_rx_params *p, size_t *consumed /* [n_streams] */);

@@ -5,7 +5,11 @@
   * stages: device time per stage of a call (torch.profiler; median, min and max over --repeats profiled calls): screen (the
     K1 launches before detection), detect, sync, assemble + K1 (data windows), integer chain (header, frame records, K8);
   * realtime: 384 SF7 streams x 2 s (1 MS/s) with frames, wall time per call (median of repeats) and the real-time factor.
-Usage: python tools/bench_rx_sync.py [--quick]"""
+With --ppm P every frame comes from a crystal off by a per-frame offset uniform in +-P ppm at 868.1 MHz, which sets both its
+CFO (ppm * 868.1 Hz, in place of the random CFO) and its clock (tx_frames_sfo); every sensitivity point and the real-time
+shape are then measured both with carrier_hz = 868.1e6 (the clock offset follows each frame's CFO) and without.  P above
+about 36 puts the CFO beyond BW/4.
+Usage: python tools/bench_rx_sync.py [--quick] [--ppm P]"""
 from __future__ import annotations
 
 import argparse
@@ -19,6 +23,7 @@ import numpy as np
 sys.path.insert(0, str(Path(__file__).resolve().parent.parent))
 
 BW, FS = 125000, 1e6
+CARRIER = 868.1e6
 POINTS = {7: (-5.0, -3.5, -2.0, 0.0), 8: (-8.0, -6.5, -5.0, -3.0), 9: (-10.5, -9.0, -7.5, -5.5), 10: (-13.0, -11.5, -10.0, -8.0),
           11: (-15.5, -14.0, -12.5, -10.5), 12: (-18.0, -16.5, -15.0, -13.0)}
 
@@ -32,7 +37,7 @@ def dec(sf, rr, **kw):
     return G.decoder(FS, BW, sf, False, 4, True, rr, quiet=True, demod="fft", **kw)
 
 
-def capture(torch, sf, n_streams, per_stream, snr, seed, n_items=None, plen=10):
+def capture(torch, sf, n_streams, per_stream, snr, seed, n_items=None, plen=10, ppm=0.0):
     import gr_lora_b200 as G
     from gr_lora_b200 import tx
     rr = sf >= 11
@@ -43,10 +48,15 @@ def capture(torch, sf, n_streams, per_stream, snr, seed, n_items=None, plen=10):
         n_items = per_stream * (flen + 5 * sps) + 8 * sps
     pays = [[bytes(rng.integers(0, 256, plen, dtype=np.uint8)) for _ in range(per_stream)] for _ in range(n_streams)]
     cfo = [[float(rng.uniform(-0.9, 0.9) * BW / 4) for _ in p] for p in pays]
+    kw = {}
+    if ppm:                                          # a crystal off by e ppm: CFO e * 868.1 Hz, clock off by e ppm
+        sfo = [[float(rng.uniform(-ppm, ppm)) for _ in p] for p in pays]
+        cfo = [[e * CARRIER * 1e-6 for e in es] for es in sfo]
+        kw["sfo_ppm"] = sfo
     gen = dec(sf, rr)
     up = torch.from_numpy(tx.base_upchirp(sf).astype(np.complex64)).cuda()
     out, placed = gen.synth_streams(pays, n_items, lead_symbols=float(rng.uniform(1, 3)), gap_symbols=4.3, cfo_hz=cfo,
-                                    noise_sigma=sigma_for(snr), seed=seed, up_table_dev=up)
+                                    noise_sigma=sigma_for(snr), seed=seed, up_table_dev=up, **kw)
     torch.cuda.synchronize()
     return out, placed, n_items
 
@@ -73,12 +83,12 @@ def genie_ser(torch, sf, snr, n=2048, seed=1):
     return float((bins != vals).float().mean().item())
 
 
-def stages(torch, rx, out, n_items):
+def stages(torch, rx, out, n_items, carrier_hz=0.0):
     from torch.profiler import ProfilerActivity, profile
-    rx.receive(out, n_items=n_items)
+    rx.receive(out, n_items=n_items, carrier_hz=carrier_hz)
     torch.cuda.synchronize()
     with profile(activities=[ProfilerActivity.CUDA]) as prof:
-        rx.receive(out, n_items=n_items)
+        rx.receive(out, n_items=n_items, carrier_hz=carrier_hz)
         torch.cuda.synchronize()
     ev = sorted([e for e in prof.events() if e.device_type.name == "CUDA"], key=lambda e: e.time_range.start)
     t = {"screen": 0.0, "detect": 0.0, "sync": 0.0, "assemble_k1": 0.0, "integer_chain": 0.0, "copies": 0.0}
@@ -106,7 +116,10 @@ def main():
     ap.add_argument("--quick", action="store_true", help="fewer frames per point")
     ap.add_argument("--repeats", type=int, default=5, help="timed calls of the real-time shape, and profiled calls")
     ap.add_argument("--runs", type=int, default=3, help="independent captures (seeds) per sensitivity point")
+    ap.add_argument("--ppm", type=float, default=0.0, help="per-frame crystal offset uniform in +-PPM at 868.1 MHz (0: none)")
     a = ap.parse_args()
+    if abs(a.ppm) * CARRIER * 1e-6 > BW / 4:
+        raise SystemExit(f"--ppm {a.ppm}: a CFO of {a.ppm * CARRIER * 1e-6:.0f} Hz is beyond BW/4")
     import torch
     if not torch.cuda.is_available():
         raise SystemExit("bench_rx_sync.py needs a CUDA device")
@@ -118,41 +131,51 @@ def main():
     except Exception:
         res["power_limit_w"] = "unknown"
     ns = 32 if a.quick else 96
+    res["ppm"] = a.ppm
+    # with --ppm, every measurement with the clock offset following the CFO ("tracked") and without ("fixed")
+    modes = {"tracked": CARRIER, "fixed": 0.0} if a.ppm else {"": 0.0}
     curve = {}
     for sf, pts in POINTS.items():
         rr = sf >= 11
         row = []
         for snr in pts:
-            oks, n = [], 0
+            oks, n = {m: [] for m in modes}, 0
             for r in range(a.runs):
-                out, placed, n_items = capture(torch, sf, ns, 1, snr, seed=sf * 100 + int(snr * 10) % 97 + 7919 * r)
+                out, placed, n_items = capture(torch, sf, ns, 1, snr, seed=sf * 100 + int(snr * 10) % 97 + 7919 * r, ppm=a.ppm)
                 rx = dec(sf, rr, n_streams=ns, max_items_per_call=n_items)
-                _, frames, _ = rx.receive(out, n_items=n_items)
-                oks.append(decoded(frames, placed))
+                for m, carrier in modes.items():
+                    _, frames, _ = rx.receive(out, n_items=n_items, carrier_hz=carrier)
+                    oks[m].append(decoded(frames, placed))
                 n = len(placed)
                 rx.close()
                 del out
-            row.append({"snr_db": snr, "frames_per_run": n, "ok_per_run": oks, "frames_ok": sum(oks) / (n * a.runs),
-                        "genie_ser": genie_ser(torch, sf, snr), "genie_symbols": 2048})
+            pt = {"snr_db": snr, "frames_per_run": n}
+            for m in modes:
+                pt["ok_per_run" + (m and "_" + m)] = oks[m]
+                pt["frames_ok" + (m and "_" + m)] = sum(oks[m]) / (n * a.runs)
+            pt.update({"genie_ser": genie_ser(torch, sf, snr), "genie_symbols": 2048})
+            row.append(pt)
         curve[f"sf{sf}"] = row
     res["sensitivity"] = curve
     # config-4 shape: 384 SF7 streams x 2 s, frames 3 dB above the sensitivity point
-    out, placed, n_items = capture(torch, 7, 384, 40, 1.0, seed=4, n_items=2_000_000)
+    out, placed, n_items = capture(torch, 7, 384, 40, 1.0, seed=4, n_items=2_000_000, ppm=a.ppm)
     rx = dec(7, False, n_streams=384, max_items_per_call=n_items, max_frames_per_call=64)
-    runs = [stages(torch, rx, out, n_items) for _ in range(a.repeats)]
-    res["stages_ms"] = {k: {"median": float(np.median([r[k] for r in runs])), "min": min(r[k] for r in runs),
-                            "max": max(r[k] for r in runs)} for k in runs[0]}
-    times = []
-    for _ in range(a.repeats):
-        torch.cuda.synchronize()
-        t0 = time.perf_counter()
-        _, frames, _ = rx.receive(out, n_items=n_items)
-        times.append(time.perf_counter() - t0)
-    med = float(np.median(times))
-    res["realtime"] = {"streams": 384, "seconds_per_stream": n_items / FS, "frames_placed": len(placed),
-                       "frames_decoded": decoded(frames, placed), "call_s_median": round(med, 4),
-                       "call_s_min": round(min(times), 4), "call_s_max": round(max(times), 4),
-                       "realtime_factor": round(384 * n_items / FS / med, 1)}
+    for m, carrier in modes.items():
+        runs = [stages(torch, rx, out, n_items, carrier) for _ in range(a.repeats)]
+        res["stages_ms" + (m and "_" + m)] = {k: {"median": float(np.median([r[k] for r in runs])), "min": min(r[k] for r in runs),
+                                                  "max": max(r[k] for r in runs)} for k in runs[0]}
+    times = {m: [] for m in modes}
+    for _ in range(a.repeats):                       # the modes alternate, so that both see the same conditions
+        for m, carrier in modes.items():
+            torch.cuda.synchronize()
+            t0 = time.perf_counter()
+            _, frames, _ = rx.receive(out, n_items=n_items, carrier_hz=carrier)
+            times[m].append(time.perf_counter() - t0)
+            med = float(np.median(times[m]))
+            res["realtime" + (m and "_" + m)] = {
+                "streams": 384, "seconds_per_stream": n_items / FS, "frames_placed": len(placed),
+                "frames_decoded": decoded(frames, placed), "call_s_median": round(med, 4), "call_s_min": round(min(times[m]), 4),
+                "call_s_max": round(max(times[m]), 4), "realtime_factor": round(384 * n_items / FS / med, 1)}
     print(json.dumps(res))
 
 

@@ -3,7 +3,8 @@
   encode      lora_b200_tx_encode_dev: distinct 12-byte payloads -> chirp shifts, frames/s (SF7 and SF12, CR4/8)
   frames      lora_b200_tx_frames_dev against lora_b200_tx_expand_dev writing the same shape, GB/s written and the share of
               the 3 350 GB/s data-sheet HBM3 figure of the H100 SXM: [4096, 256 * sps] at SF7 (bench.py's e2e shape) and the
-              config-4 shape (64 streams x 2 000 000 samples for each of SF7..SF12), with and without noise
+              config-4 shape (64 streams x 2 000 000 samples for each of SF7..SF12), with and without noise, and
+              lora_b200_tx_frames_sfo_dev with every frame's clock off by +-20 ppm (tx_frames_sfo20)
   host        the path the tests and bench.py use today for the same kind of frames: tx.encode_frame + modulate_frame +
               channel on the host + the copy to the device, frames/s
 
@@ -104,17 +105,23 @@ def bench_shape(torch, G, sf, n_streams, n_items, args, payload_len=12):
     base = torch.empty((k, n_items), dtype=torch.complex64, device="cuda")
     dec.tx_frames(fr[fr["stream"] < k], shifts, n_sym, k, n_items, base, up_table_dev=up, cuda_stream=st)
     nbytes = n_streams * n_items * 8
+    ppm = np.where(np.arange(len(fr)) % 2 == 0, 20.0, -20.0).astype(np.float32)
     res = {"sf": sf, "streams": n_streams, "items": n_items, "frames": len(fr), "bytes_written": nbytes}
     for sigma in (0.0, float(np.sqrt(10 ** -3.5 / 2))):
         tag = "noise" if sigma else "clean"
         run_f = lambda: dec.tx_frames(fr, shifts, n_sym, n_streams, n_items, out, noise_sigma=sigma, seed=1, up_table_dev=up, cuda_stream=st)
         run_e = lambda: dec.tx_expand(base, k, n_items, n_streams, out, noise_sigma=sigma, seed=1, cuda_stream=st)
-        tf, te = [], []
-        for _ in range(2):                                 # alternate the two kernels
+        # every frame from a transmitter whose clock is off by +-20 ppm (tx_frames_sfo: the phase law at fractional times)
+        run_d = lambda: dec.tx_frames(fr, shifts, n_sym, n_streams, n_items, out, noise_sigma=sigma, seed=1, up_table_dev=up,
+                                      cuda_stream=st, sfo_ppm=ppm)
+        tf, te, td = [], [], []
+        for _ in range(2):                                 # alternate the kernels
             tf.append(timed(torch, run_f, args.iters, args.warmup))
             te.append(timed(torch, run_e, args.iters, args.warmup))
-        tf, te = min(tf), min(te)
+            td.append(timed(torch, run_d, args.iters, args.warmup))
+        tf, te, td = min(tf), min(te), min(td)
         res[tag] = {"tx_frames_s": tf, "tx_frames_gbs": nbytes / tf / 1e9, "tx_frames_share_of_hbm": nbytes / tf / 1e9 / HBM_GBS,
+                    "tx_frames_sfo20_s": td, "tx_frames_sfo20_gbs": nbytes / td / 1e9,
                     "tx_expand_s": te, "tx_expand_gbs": nbytes / te / 1e9, "tx_expand_share_of_hbm": nbytes / te / 1e9 / HBM_GBS}
     t_enc = timed(torch, lambda: dec.tx_encode(pay, off, ln, shifts, n_sym, st), args.iters, args.warmup)
     res["encode_plus_frames_frames_per_s"] = len(fr) / (t_enc + res["noise"]["tx_frames_s"])
