@@ -31,7 +31,8 @@ class TxFrame(C.Structure):
 
 class RxParams(C.Structure):
     """struct lora_b200_rx_params (include/lora_b200.h)."""
-    _fields_ = [("sync_word", C.c_uint8), ("reserved0", C.c_uint8 * 3), ("implicit_len", C.c_uint32), ("min_preamble", C.c_uint32),
+    _fields_ = [("sync_word", C.c_uint8), ("soft", C.c_uint8), ("reserved0", C.c_uint8 * 2), ("implicit_len", C.c_uint32),
+                ("min_preamble", C.c_uint32),
                 ("max_cfo_hz", C.c_float), ("sfo_ppm", C.c_float), ("reserved1", C.c_uint32), ("carrier_hz", C.c_double)]
 
 
@@ -62,6 +63,7 @@ SIGNATURES = {
     "lora_b200_tables_commit": (_i, [_vp]),
     "lora_b200_demod_fft_dev": (_i, [_vp, _vp, _sz, _vp, _vp, _vp]),
     "lora_b200_demod_fft_host": (_i, [_vp, _vp, _sz, _vp, _vp]),
+    "lora_b200_demod_llr_dev": (_i, [_vp, _vp, _sz, _i, _vp, _vp, _vp]),
     "lora_b200_demod_fft_host_sc16": (_i, [_vp, _vp, C.c_float, _sz, _vp, _vp]),
     "lora_b200_demod_gradient_dev": (_i, [_vp, _vp, _sz, _vp, _vp]),
     "lora_b200_ifreq_dev": (_i, [_vp, _vp, _sz, _u32, _vp, _vp]),

@@ -4,6 +4,7 @@
 // cuda_owned.h.  Not part of liblora_b200.so.
 #include "cuda_owned.h"
 #include "k1_fft.cuh"
+#include "k1_llr.cuh"
 #include "k1_warp.cuh"
 #include "k1_group.cuh"
 #include "k1_sf10.cuh"
@@ -30,6 +31,22 @@ int lb_k1_emulate(int sf, const float2 *x, size_t n_symbols, const float2 *chirp
     case 10: lb::k1_emulate<10>(a, bins, mags); break;
     case 11: lb::k1_emulate<11>(a, bins, mags); break;
     case 12: lb::k1_emulate<12>(a, bins, mags); break;
+    default: return -1;
+    }
+    return 0;
+}
+
+// the LLR demodulator k1_llr_kernel (k1_llr.cuh) on the host: llrs[i * ppm ..], bins may be NULL
+int lb_k1_llr_emulate(int sf, const float2 *x, size_t n_symbols, const float2 *chirp, const float2 *tw, int reduced, float *llrs,
+                      uint32_t *bins) {
+    lb::K1Args a{x, chirp, tw, n_symbols};
+    switch (sf) {
+    case 7: lb::k1_llr_emulate<7>(a, reduced != 0, llrs, bins); break;
+    case 8: lb::k1_llr_emulate<8>(a, reduced != 0, llrs, bins); break;
+    case 9: lb::k1_llr_emulate<9>(a, reduced != 0, llrs, bins); break;
+    case 10: lb::k1_llr_emulate<10>(a, reduced != 0, llrs, bins); break;
+    case 11: lb::k1_llr_emulate<11>(a, reduced != 0, llrs, bins); break;
+    case 12: lb::k1_llr_emulate<12>(a, reduced != 0, llrs, bins); break;
     default: return -1;
     }
     return 0;
@@ -97,6 +114,19 @@ uint32_t lb_emul_tx_encode(const uint8_t *payload, uint32_t len, uint32_t sf, ui
     if (n > cap) return 0;
     for (uint32_t i = 0; i < n; i++) shifts[i] = lb::tx_symbol_shift(c, payload, len, i);
     return n;
+}
+// the soft block decoder of the dechirp receiver (rx_sync.cuh) on given LLRs.  Header block: llr[8][sf - 2] -> 8 corrected
+// bins and sf - 2 nibbles (nib may be NULL); returns the frame's coding rate (from the header when explicit).  Payload block
+// b of a frame with coding rate cr: llr[4 + cr][ppm] -> 4 + cr corrected bins and ppm nibbles.
+uint32_t lb_emul_soft_header(uint32_t sf, uint32_t cr, int implicit, int crc, int reduced_rate, const float *llr, uint32_t *bins,
+                             uint32_t *nib) {
+    const lb::TxCode c{sf, cr, implicit ? 0u : 1u, crc ? 1u : 0u, reduced_rate ? 1u : 0u};
+    return lb::rs_soft_header(c, llr, bins, nib).cr;
+}
+void lb_emul_soft_block(uint32_t sf, uint32_t cr, int implicit, int crc, int reduced_rate, uint32_t b, const float *llr, uint32_t *bins,
+                        uint32_t *nib) {
+    const lb::TxCode c{sf, cr, implicit ? 0u : 1u, crc ? 1u : 0u, reduced_rate ? 1u : 0u};
+    lb::rs_soft_block(c, b, llr, bins, nib);
 }
 uint32_t lb_emul_header_checksum(uint32_t length, uint32_t cr, uint32_t crc) { return lb::header_checksum(length, cr, crc); }
 
@@ -170,8 +200,8 @@ struct RsHostOps {
     }
 };
 
-// data windows first .. first + cnt - 1 of frame r (each from its own start, rs_sym), de-rotated by its CFO, through K1
-void rs_host_bins(const RsHostOps &o, const lb::RsFrame &r, uint32_t first, uint32_t cnt, std::vector<uint32_t> &bins) {
+// data windows first .. first + cnt - 1 of frame r (each from its own start, rs_sym), de-rotated by its CFO
+std::vector<float2> rs_host_windows(const RsHostOps &o, const lb::RsFrame &r, uint32_t first, uint32_t cnt) {
     std::vector<float2> w((size_t)cnt * o.sps);
     for (uint32_t k = 0; k < cnt; k++) {
         const long long s0 = lb::rs_sym(r.start, lb::rs_data_j((long long)first + k), o.sps, r.sfo_ppm);
@@ -182,9 +212,22 @@ void rs_host_bins(const RsHostOps &o, const lb::RsFrame &r, uint32_t first, uint
             w[(size_t)k * o.sps + i] = make_float2((float)(v.x * cos(a) - v.y * sin(a)), (float)(v.x * sin(a) + v.y * cos(a)));
         }
     }
+    return w;
+}
+
+// ... through K1
+void rs_host_bins(const RsHostOps &o, const lb::RsFrame &r, uint32_t first, uint32_t cnt, std::vector<uint32_t> &bins) {
+    const std::vector<float2> w = rs_host_windows(o, r, first, cnt);
     bins.resize(cnt);
     std::vector<float> mags(cnt);
     lb_k1_emulate((int)o.sf, w.data(), cnt, o.down, o.tw, bins.data(), mags.data());
+}
+
+// ... through the LLR demodulator
+void rs_host_llrs(const RsHostOps &o, const lb::RsFrame &r, uint32_t first, uint32_t cnt, bool reduced, std::vector<float> &llr) {
+    const std::vector<float2> w = rs_host_windows(o, r, first, cnt);
+    llr.resize((size_t)cnt * (reduced ? o.sf - 2 : o.sf));
+    lb_k1_llr_emulate((int)o.sf, w.data(), cnt, o.down, o.tw, reduced, llr.data(), nullptr);
 }
 
 }  // namespace
@@ -196,10 +239,11 @@ extern "C" {
 // synchronised frame f (at most cap): start[f], cfo_bins[f], snr_db[f], status[f] (0 published, 1 header checksum failed,
 // 2 incomplete), the clock offset its windows were placed with sfo[f] (may be NULL) and, when published, its payload in
 // payload[f * 256 ..] with length len[f].  Returns the number of synchronised frames.
-uint32_t lb_emul_rx_receive_sfo(const float2 *x, size_t n_items, const float2 *down, const float2 *up, const float2 *tw, uint32_t sf,
-                                uint32_t cr, int implicit, int crc, int reduced_rate, uint32_t sync_word, uint32_t implicit_len,
-                                uint32_t min_preamble, float sfo_ppm, double carrier_hz, long long *start, float *cfo_bins,
-                                float *snr_db, int32_t *status, float *sfo, uint8_t *payload, uint32_t *len, uint32_t cap) {
+// soft != 0: soft decisions, as lora_b200_rx_params.soft (the LLR demodulator's emulation and the soft block decoder).
+uint32_t lb_emul_rx_receive_soft(const float2 *x, size_t n_items, const float2 *down, const float2 *up, const float2 *tw, uint32_t sf,
+                                 uint32_t cr, int implicit, int crc, int reduced_rate, uint32_t sync_word, uint32_t implicit_len,
+                                 uint32_t min_preamble, float sfo_ppm, double carrier_hz, int soft, long long *start, float *cfo_bins,
+                                 float *snr_db, int32_t *status, float *sfo, uint8_t *payload, uint32_t *len, uint32_t cap) {
     const uint32_t N = 1u << sf, sps = 8u * N;
     const double bin_hz = 125e3 / N;
     lb::RsParams p{sps, N, 8u, sfo_ppm, min_preamble ? min_preamble : 5u, {((sync_word >> 4) & 15u) * 8u % N, (sync_word & 15u) * 8u % N},
@@ -234,12 +278,25 @@ uint32_t lb_emul_rx_receive_sfo(const float2 *x, size_t n_items, const float2 *d
         auto data_end = [&](long long n) { return lb::rs_sym(r.start, lb::rs_data_j(n - 1), sps, r.sfo_ppm) + (long long)sps; };
         if (r.status == lb::RS_OK && data_end(8) <= (long long)n_items) {
             std::vector<uint32_t> hb, pb;
-            rs_host_bins(o, r, 0, 8, hb);
+            std::vector<float> llr;
+            if (soft) {
+                hb.resize(8);
+                rs_host_llrs(o, r, 0, 8, true, llr);
+                lb::rs_soft_header(lb::rs_code(rp, phdr1), llr.data(), hb.data(), nullptr);
+            } else {
+                rs_host_bins(o, r, 0, 8, hb);
+            }
             lb::RxStreamState st;
             const int32_t np = lb::rs_header(&st, rp, phdr1, hb.data(), implicit_len);
             if (np < 0) status[nf] = 1;
             else if (data_end(8ll + np) <= (long long)n_items) {
-                rs_host_bins(o, r, 8, (uint32_t)np, pb);
+                if (soft) {
+                    pb.resize((size_t)np);
+                    rs_host_llrs(o, r, 8, (uint32_t)np, reduced_rate != 0, llr);
+                    lb::rs_soft_payload(rp, phdr1, hb.data(), np, implicit_len, llr.data(), pb.data());
+                } else {
+                    rs_host_bins(o, r, 8, (uint32_t)np, pb);
+                }
                 lb::RxFrameRec fr;
                 lb::rs_frame(&st, rp, pb.data(), np, &fr, 0, nf, 1.0f);
                 const uint32_t nd = lb::decode_len_bytes(lb::decode_len_words(fr.n_cw, 0), fr.cr);
@@ -251,6 +308,47 @@ uint32_t lb_emul_rx_receive_sfo(const float2 *x, size_t n_items, const float2 *d
         nf++;
     }
     return nf;
+}
+
+// the header and payload rounds of one frame whose n_windows data windows are given (no synchronisation): as bins
+// (llr NULL), or as LLRs -- the header block's llr[8][sf - 2] (reduced) first, then the payload windows' llr[][ppm].
+// Writes the payload to payload[0 .. 256) and returns its length; -1: the explicit header's checksum failed, -2: the frame
+// needs more than n_windows windows.
+int32_t lb_emul_rx_decode(uint32_t sf, uint32_t cr, int implicit, int crc, int reduced_rate, uint32_t implicit_len, const uint32_t *bins,
+                          const float *llr, uint32_t n_windows, uint8_t *payload) {
+    lb::RxParams rp;
+    memset(&rp, 0, sizeof rp);
+    rp.sf = sf; rp.n_bins = 1u << sf; rp.n_bins_hdr = rp.n_bins / 4; rp.sps = 8u << sf; rp.decim = 8; rp.implicit = implicit;
+    rp.reduced_rate = reduced_rate;
+    const uint8_t phdr1 = (uint8_t)(((cr & 7u) << 5) | (crc ? 1u << 4 : 0u));
+    if (n_windows < 8u) return -2;
+    std::vector<uint32_t> hb(8), pb;
+    if (llr) lb::rs_soft_header(lb::rs_code(rp, phdr1), llr, hb.data(), nullptr);
+    else std::copy(bins, bins + 8, hb.begin());
+    lb::RxStreamState st;
+    const int32_t np = lb::rs_header(&st, rp, phdr1, hb.data(), implicit_len);
+    if (np < 0) return -1;
+    if (8u + (uint32_t)np > n_windows) return -2;
+    if (llr) {
+        pb.resize((size_t)np);
+        lb::rs_soft_payload(rp, phdr1, hb.data(), np, implicit_len, llr + 8 * (sf - 2), pb.data());
+    } else {
+        pb.assign(bins + 8, bins + 8 + np);
+    }
+    lb::RxFrameRec fr;
+    lb::rs_frame(&st, rp, pb.data(), np, &fr, 0, 0, 1.0f);
+    const uint32_t nd = lb::decode_len_bytes(lb::decode_len_words(fr.n_cw, 0), fr.cr), len = std::min<uint32_t>(fr.payload_length, 256u);
+    for (uint32_t i = 0; i < len; i++) payload[i] = i < nd ? lb::decode_byte(fr.cw, fr.n_cw, 0, fr.cr, i) : 0;
+    return (int32_t)len;
+}
+
+// lb_emul_rx_receive_soft with hard decisions
+uint32_t lb_emul_rx_receive_sfo(const float2 *x, size_t n_items, const float2 *down, const float2 *up, const float2 *tw, uint32_t sf,
+                                uint32_t cr, int implicit, int crc, int reduced_rate, uint32_t sync_word, uint32_t implicit_len,
+                                uint32_t min_preamble, float sfo_ppm, double carrier_hz, long long *start, float *cfo_bins,
+                                float *snr_db, int32_t *status, float *sfo, uint8_t *payload, uint32_t *len, uint32_t cap) {
+    return lb_emul_rx_receive_soft(x, n_items, down, up, tw, sf, cr, implicit, crc, reduced_rate, sync_word, implicit_len, min_preamble,
+                                   sfo_ppm, carrier_hz, 0, start, cfo_bins, snr_db, status, sfo, payload, len, cap);
 }
 
 // lb_emul_rx_receive_sfo without a clock offset

@@ -129,7 +129,7 @@ struct lora_b200_decoder : A1Params {
     // lora_b200_receive (rx_sync.cuh), all on rx_stream
     DeviceBuffer<float2> d_rs_stage, d_rs_win;
     DeviceBuffer<uint32_t> d_rs_bins[2], d_rs_hbins, d_rs_pbins, d_rs_ncand, d_rs_nframes, d_rs_tab;
-    DeviceBuffer<float> d_rs_mags[2];
+    DeviceBuffer<float> d_rs_mags[2], d_rs_llr;
     DeviceBuffer<RsCand> d_rs_cands;
     DeviceBuffer<long long> d_rs_dropped;
     DeviceBuffer<unsigned long long> d_rs_hold;
@@ -312,6 +312,34 @@ int dispatch_k1(lora_b200_decoder *d, K1Scratch &ks, const float2 *iq, size_t n,
     CU(cudaEventRecord(ks.done, st));
     ks.last = st;
     return LORA_B200_OK;
+}
+
+// ---- the LLR demodulator (k1_llr.cuh) ----------------------------------------------------------
+template <int SF>
+int llr_launch(lora_b200_decoder *d, const float2 *iq, size_t n, bool reduced, float *llrs, uint32_t *bins, cudaStream_t st) {
+    using C = K1Cfg<SF>;
+    static DeviceOnce once;
+    const size_t smem = sizeof(float2) * C::SMEM_ELEMS;
+    CU(once(d->device, [&] { return cudaFuncSetAttribute(k1_llr_kernel<SF>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem); }));
+    const size_t n_batches = (n + C::G - 1) / C::G;
+    const int grid = (int)std::min<size_t>(n_batches, (size_t)d->n_sms * 2);
+    k1_llr_kernel<SF><<<grid, K1_THREADS, smem, st>>>(K1Args{iq, tab<float2>(d, d->toff.down), tab<float2>(d, d->toff.tw), n},
+                                                      reduced ? 1 : 0, llrs, bins);
+    return launched(d);
+}
+
+int dispatch_llr(lora_b200_decoder *d, const float2 *iq, size_t n, bool reduced, float *llrs, uint32_t *bins, cudaStream_t st) {
+    if (!d->k1_ok) return fail(LORA_B200_EUNSUPPORTED, "the LLR demodulator needs samp_rate/bandwidth == 8 and SF7..SF12");
+    if (n == 0) return LORA_B200_OK;
+    switch (d->cfg.sf) {
+    case 7: return llr_launch<7>(d, iq, n, reduced, llrs, bins, st);
+    case 8: return llr_launch<8>(d, iq, n, reduced, llrs, bins, st);
+    case 9: return llr_launch<9>(d, iq, n, reduced, llrs, bins, st);
+    case 10: return llr_launch<10>(d, iq, n, reduced, llrs, bins, st);
+    case 11: return llr_launch<11>(d, iq, n, reduced, llrs, bins, st);
+    case 12: return llr_launch<12>(d, iq, n, reduced, llrs, bins, st);
+    }
+    return fail(LORA_B200_EUNSUPPORTED, "unsupported SF %u", d->cfg.sf);
 }
 
 // ---- stream-path launch -----------------------------------------------------------------------
@@ -660,6 +688,15 @@ int lora_b200_demod_fft_dev(lora_b200_decoder *d, const void *iq, size_t n_symbo
     if (((uintptr_t)iq & 15u) != 0) return fail(LORA_B200_EINVAL, "iq must be 16-byte aligned");
     CU(cudaSetDevice(d->device));
     return dispatch_k1(d, d->k1s[0], (const float2 *)iq, n_symbols, bins, mags, (cudaStream_t)stream);
+}
+
+int lora_b200_demod_llr_dev(lora_b200_decoder *d, const void *iq, size_t n_symbols, int reduced, float *llrs, uint32_t *bins, void *stream) {
+    if (!d || (n_symbols && (!iq || !llrs))) return fail(LORA_B200_EINVAL, "null argument");
+    if (!d->k1_ok) return fail(LORA_B200_EUNSUPPORTED, "the LLR demodulator needs samp_rate/bandwidth == 8 and SF7..SF12");
+    if (((uintptr_t)iq & 15u) != 0) return fail(LORA_B200_EINVAL, "iq must be 16-byte aligned");
+    if (reduced != 0 && reduced != 1) return fail(LORA_B200_EINVAL, "reduced must be 0 or 1, got %d", reduced);
+    CU(cudaSetDevice(d->device));
+    return dispatch_llr(d, (const float2 *)iq, n_symbols, reduced != 0, llrs, bins, (cudaStream_t)stream);
 }
 
 // K1 from host memory: double-buffered 64 MiB chunks, H2D + kernel + D2H overlapped on two streams (each slot owns its
@@ -1070,8 +1107,10 @@ int lora_b200_receive(lora_b200_decoder *d, const void *iq, size_t n_items, size
         return fail(LORA_B200_EINVAL, "sfo_ppm must be finite and within +-500, got %g", (double)P.sfo_ppm);
     if (P.carrier_hz != 0.0 && !(std::isfinite(P.carrier_hz) && P.carrier_hz > d->samples_per_second))
         return fail(LORA_B200_EINVAL, "carrier_hz must be 0 or above the sample rate %g, got %g", d->samples_per_second, P.carrier_hz);
+    if (P.soft > 1u) return fail(LORA_B200_EINVAL, "soft must be 0 or 1, got %u", (unsigned)P.soft);
     CU(cudaSetDevice(d->device));
     const uint32_t ns = d->cfg.n_streams, sps = d->sps, N = d->n_bins, cap = d->cfg.max_frames_per_call;
+    const bool soft = P.soft != 0;
     const uint8_t sw = P.sync_word ? P.sync_word : 0x12;
     const float fs = (float)d->samples_per_second, bin_hz = fs / (float)sps;
     const float max_cfo = P.max_cfo_hz > 0.f && P.max_cfo_hz < d->cfg.bandwidth / 4.0f ? P.max_cfo_hz : d->cfg.bandwidth / 4.0f;
@@ -1142,18 +1181,29 @@ int lora_b200_receive(lora_b200_decoder *d, const void *iq, size_t n_items, size
     const size_t win_cap = std::max<size_t>(1024, ((size_t)256 << 20) / (sizeof(float2) * sps));
     CU(d->d_rs_win.reserve(win_cap * sps));
     CU(d->d_rs_hbins.reserve((size_t)n_sync * 8));
+    // soft decisions: LLRs of ppm values per window (sf - 2 in the header round), corrected into the bins afterwards
+    const uint32_t hppm = d->cfg.sf - 2u, pppm = d->cfg.reduced_rate ? hppm : d->cfg.sf;
+    if (soft) CU(d->d_rs_llr.reserve((size_t)n_sync * 8 * hppm));
     const int agrid = d->n_sms * 8;
     for (uint32_t f0 = 0; f0 < n_sync; f0 += (uint32_t)(win_cap / 8)) {
         const uint32_t nb = (uint32_t)std::min<size_t>(win_cap / 8, n_sync - f0);
         rs_assemble_kernel<<<std::min<int>((int)nb, agrid), 256, 0, st>>>(x, stride, (long long)n_items, d->d_rs_frames + f0, nb, nullptr, 0,
                                                                           nullptr, 0, nullptr, sps, d->d_rs_win);
         if (int rc = launched(d)) return rc;
-        if (int rc = dispatch_k1(d, d->k1s[0], d->d_rs_win, (size_t)nb * 8, d->d_rs_hbins + (size_t)f0 * 8, nullptr, st)) return rc;
+        if (soft) {
+            if (int rc = dispatch_llr(d, d->d_rs_win, (size_t)nb * 8, true, d->d_rs_llr + (size_t)f0 * 8 * hppm, nullptr, st)) return rc;
+        } else if (int rc = dispatch_k1(d, d->k1s[0], d->d_rs_win, (size_t)nb * 8, d->d_rs_hbins + (size_t)f0 * 8, nullptr, st)) {
+            return rc;
+        }
     }
     RxParams rxp;
     memset(&rxp, 0, sizeof rxp);
     rxp.sps = sps; rxp.n_bins = N; rxp.n_bins_hdr = d->n_bins_hdr; rxp.decim = d->decim; rxp.sf = d->cfg.sf;
     rxp.implicit = d->cfg.implicit; rxp.reduced_rate = d->cfg.reduced_rate;
+    if (soft) {
+        rs_soft_header_kernel<<<(n_sync + 127) / 128, 128, 0, st>>>(n_sync, rxp, d->phdr1_init, d->d_rs_llr, d->d_rs_hbins);
+        if (int rc = launched(d)) return rc;
+    }
     rs_header_kernel<<<(n_sync + 127) / 128, 128, 0, st>>>(d->d_rs_frames, d->d_rs_nframes, fcap, rxp, d->phdr1_init, d->d_rs_hbins,
                                                            P.implicit_len);
     if (int rc = launched(d)) return rc;
@@ -1205,6 +1255,7 @@ int lora_b200_receive(lora_b200_decoder *d, const void *iq, size_t n_items, size
     size_t pwin_cap = win_cap;
     for (uint32_t k = 0; k < np; k++) pwin_cap = std::max<size_t>(pwin_cap, tabh[3 * np + k]);
     CU(d->d_rs_win.reserve(pwin_cap * sps));
+    if (soft) CU(d->d_rs_llr.reserve((size_t)std::max<uint32_t>(total, 1u) * pppm));
     const uint32_t *t_pub = d->d_rs_tab, *t_seq = t_pub + np, *t_off = t_pub + 2 * np, *t_cnt = t_pub + 3 * np;
     for (uint32_t g0 = 0; g0 < np;) {
         uint32_t g1 = g0, w = 0;
@@ -1214,9 +1265,19 @@ int lora_b200_receive(lora_b200_decoder *d, const void *iq, size_t n_items, size
                                                                                     t_pub + g0, 8, t_off + g0, tabh[2 * np + g0], t_cnt + g0,
                                                                                     sps, d->d_rs_win);
             if (int rc = launched(d)) return rc;
-            if (int rc = dispatch_k1(d, d->k1s[0], d->d_rs_win, w, d->d_rs_pbins + tabh[2 * np + g0], nullptr, st)) return rc;
+            const size_t o = tabh[2 * np + g0];
+            if (soft) {
+                if (int rc = dispatch_llr(d, d->d_rs_win, w, d->cfg.reduced_rate != 0, d->d_rs_llr + o * pppm, nullptr, st)) return rc;
+            } else if (int rc = dispatch_k1(d, d->k1s[0], d->d_rs_win, w, d->d_rs_pbins + o, nullptr, st)) {
+                return rc;
+            }
         }
         g0 = g1;
+    }
+    if (soft) {
+        rs_soft_payload_kernel<<<(np + 127) / 128, 128, 0, st>>>(d->d_rs_frames, t_pub, np, rxp, d->phdr1_init, d->d_rs_hbins, t_off,
+                                                                  P.implicit_len, d->d_rs_llr, d->d_rs_pbins);
+        if (int rc = launched(d)) return rc;
     }
     CU(d->d_rs_recs.reserve(np));
     CU(d->d_rs_out.reserve(np));
@@ -1224,6 +1285,9 @@ int lora_b200_receive(lora_b200_decoder *d, const void *iq, size_t n_items, size
                                                       t_off, P.implicit_len, d->d_rs_recs);
     if (int rc = launched(d)) return rc;
     CU(cudaMemcpyAsync(d->d_rs_nframes, &np, sizeof np, cudaMemcpyHostToDevice, st));
+    // K8 writes a record's first len bytes only: zero the rest, so that a published record never carries stale device
+    // memory (after soft decisions, LLRs of an earlier call or decoder)
+    CU(cudaMemsetAsync(d->d_rs_out, 0, sizeof(RxFrameOut) * np, st));
     k8_frames_kernel<<<(int)std::min<uint32_t>(np, (uint32_t)d->n_sms * 4u), 128, 0, st>>>(d->d_rs_recs, d->d_rs_nframes, np, d->d_rs_out);
     if (int rc = launched(d)) return rc;
     d->h_sorted.resize(np);
@@ -1239,7 +1303,8 @@ int lora_b200_receive(lora_b200_decoder *d, const void *iq, size_t n_items, size
     return finish();
 }
 
-static_assert(sizeof(lora_b200_rx_info) == 32 && sizeof(lora_b200_rx_params) == 32 && offsetof(lora_b200_rx_params, sfo_ppm) == 16 &&
+static_assert(sizeof(lora_b200_rx_info) == 32 && sizeof(lora_b200_rx_params) == 32 && offsetof(lora_b200_rx_params, soft) == 1 &&
+              offsetof(lora_b200_rx_params, sfo_ppm) == 16 &&
               offsetof(lora_b200_rx_params, carrier_hz) == 24 && offsetof(lora_b200_rx_info, sfo_ppm) == 28, "lora_b200_rx_* layout");
 
 size_t lora_b200_rx_info_last(lora_b200_decoder *d, const lora_b200_rx_info **info, uint32_t *hdr_drops) {

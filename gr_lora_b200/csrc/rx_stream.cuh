@@ -136,6 +136,16 @@ LB_HD int rx_sfd_commit(RxStreamState *st, float c) {
     return st->corr_fails > 4u ? LORA_B200_DETECT : LORA_B200_FIND_SFD;   // :808-813
 }
 
+// FFT demodulator's bin k -> the demodulated bin (k - 1) mod N (the dechirp receiver's mapping, rx_sync.cuh)
+LB_HD int rx_fft_bin(uint32_t k, uint32_t n_bins) { return ((int)k + (int)n_bins - 1) % (int)n_bins; }
+
+// the Gray word of demodulated bin b (:507-512), as rx_symbol_commit makes it: reduced-rate symbols first fold b to
+// n_bins_hdr bins
+LB_HD uint32_t rx_demod_word(uint32_t b, bool reduced, uint32_t n_bins_hdr) {
+    if (reduced) b = reduce_bin(b, n_bins_hdr);
+    return gray_encode(b);
+}
+
 // DECODE_HEADER / DECODE_PAYLOAD after demodulate() (:826-886): `bin` is the demodulated bin, or nothing when the implicit
 // energy gate (:861) skipped the symbol
 LB_HD RxSymbolResult rx_symbol_commit(RxStreamState *st, const RxParams &p, bool is_first, bool demodulated, int bin) {

@@ -10,6 +10,9 @@
 //               sync-word check
 //   assemble    each frame's data windows, de-rotated by its CFO, contiguous -> K1 batch kernels -> bins
 //   decode      rx_symbol_commit / rx_frame_record of rx_stream.cuh over the bins, header checksum, then K8
+// With soft decisions the assemble stage runs the LLR demodulator (k1_llr.cuh) instead of K1, and each interleaver block's
+// code words are decoded to their maximum-likelihood nibbles and re-encoded into corrected bins (rs_soft_* below); decode
+// then runs unchanged on those bins.
 // A window at p dechirped with the down-chirp sees an up-chirp that started tau samples before p at bin tau / decim + F, and
 // dechirped with the up-chirp sees a down-chirp at bin -tau / decim + F (F = CFO in bins, modulo N): the preamble bin A and
 // the SFD bin B give 2F = A + B and 2 tau / decim = A - B, the N/2 ambiguity resolved by |F| <= N/4.
@@ -17,6 +20,7 @@
 #pragma once
 #include "int_chain.cuh"
 #include "k1_fft.cuh"
+#include "k1_llr.cuh"
 #include "rx_stream.cuh"
 #include "tx_encode.cuh"
 
@@ -264,8 +268,7 @@ LB_HD RsFrame rs_synchronise(Ops &ops, const RsCand &c, const RsParams &p, uint3
 LB_HD int32_t rs_header(RxStreamState *st, const RxParams &p, uint8_t phdr1, const uint32_t *bins, uint32_t implicit_len) {
     rx_state_init(st, phdr1);
     for (int k = 0; k < 8; k++) {
-        const int bin = ((int)bins[k] + (int)p.n_bins - 1) % (int)p.n_bins;
-        if (rx_symbol_commit(st, p, true, true, bin) == RX_HEADER_DONE) break;
+        if (rx_symbol_commit(st, p, true, true, rx_fft_bin(bins[k], p.n_bins)) == RX_HEADER_DONE) break;
     }
     if (p.implicit) {                                 // as many payload blocks as the code words of implicit_len bytes need
         const TxCode c{p.sf, (uint32_t)(phdr1 >> 5), 0u, (phdr1 >> 4) & 1u, p.reduced_rate ? 1u : 0u};
@@ -285,13 +288,82 @@ LB_HD void rs_frame(RxStreamState *st, const RxParams &p, const uint32_t *bins, 
     RxParams q = p;
     q.implicit = 0;                                   // count the payload down for an implicit header too
     for (int32_t k = 0; k < n_payload; k++) {
-        const int bin = ((int)bins[k] + (int)p.n_bins - 1) % (int)p.n_bins;
-        if (rx_symbol_commit(st, q, false, true, bin) == RX_FRAME_DONE) break;
+        if (rx_symbol_commit(st, q, false, true, rx_fft_bin(bins[k], p.n_bins)) == RX_FRAME_DONE) break;
     }
     st->frame_seq = seq;
     st->snr = snr_lin;
     rx_frame_record(fr, st, stream, p.implicit);
     for (uint32_t k = 0; k < st->n_demod; k++) fr->cw[k] = st->demodulated[k];
+}
+
+// ---- soft decisions --------------------------------------------------------------------------------------------------------
+// llr[i * ppm + j]: the LLR of bit j of word i of one interleaver block (k1_llr.cuh, > 0: bit 0).  Code word x's bit i is
+// bit (x - i) mod ppm of word i (the inverse of deinterleave_block), so candidate code word c at slot x scores
+// sum_i (1 - 2 bit_i(c)) llr[i][(x - i) mod ppm] over the block's n_words words.  The candidates cw(s), s = 0..15, are the
+// code words the encoder emits at that slot (tx_encode.cuh); the best score wins, the lowest s on ties (hamming84_decode's
+// rule).  Returns the nibble.
+template <class CW>
+LB_HD uint32_t rs_soft_nibble(const CW &cw, const float *llr, uint32_t n_words, uint32_t ppm, uint32_t x) {
+    float best = 0.f;
+    uint32_t bs = 0;
+    for (uint32_t s = 0; s < 16u; s++) {
+        const uint32_t c = cw(s);
+        float m = 0.f;
+        for (uint32_t i = 0; i < n_words; i++) {
+            const float l = llr[i * ppm + (x + 8u * ppm - i) % ppm];     // (i < 8)
+            m += (c >> i) & 1u ? -l : l;
+        }
+        if (s == 0u || m > best) { best = m; bs = s; }
+    }
+    return bs;
+}
+
+// the code a frame is sent with as the receiver is configured: sf, the configured cr and CRC flag (phdr1), the header mode
+LB_HD TxCode rs_code(const RxParams &p, uint8_t phdr1) {
+    return TxCode{p.sf, (uint32_t)(phdr1 >> 5), p.implicit ? 0u : 1u, (phdr1 >> 4) & 1u, p.reduced_rate ? 1u : 0u};
+}
+
+// the header block (8 words, ppm = sf - 2, llr[8][sf - 2]).  An explicit header's 5 slots come first: their header gives the
+// frame's cr, clamped to 4 as rx_symbol_commit clamps it, which whitens the remaining slots (the payload nibbles of the
+// header block).  Writes the block's 8 corrected bins (the encoder's shifts of the chosen code words) and, when nib is
+// given, its sf - 2 nibbles; returns c with the frame's cr.
+LB_HD TxCode rs_soft_header(TxCode c, const float *llr, uint32_t *bins, uint32_t *nib_out) {
+    const uint32_t ppm = c.sf - 2u;
+    uint32_t nib[LLR_MAX_PPM];
+    uint32_t x = 0;
+    if (c.explicit_hdr) {
+        for (; x < 5u; x++) nib[x] = rs_soft_nibble([&](uint32_t s) { return tx_header_cw(c, s, x); }, llr, 8u, ppm, x);
+        c.cr = nib[2] >> 1 > 4u ? 4u : nib[2] >> 1;
+    }
+    for (; x < ppm; x++) nib[x] = rs_soft_nibble([&](uint32_t s) { return tx_header_cw(c, s, x); }, llr, 8u, ppm, x);
+    for (uint32_t i = 0; i < 8u; i++) bins[i] = tx_block_shift([&](uint32_t y) { return tx_header_cw(c, nib[y], y); }, i, ppm, true, 1u << c.sf);
+    if (nib_out)
+        for (uint32_t k = 0; k < ppm; k++) nib_out[k] = nib[k];
+    return c;
+}
+
+// payload block b of a frame sent with code c (c.cr the frame's): llr[4 + cr][tx_ppm(c)] -> its 4 + cr corrected bins and,
+// when nib is given, its tx_ppm(c) nibbles
+LB_HD void rs_soft_block(const TxCode &c, uint32_t b, const float *llr, uint32_t *bins, uint32_t *nib_out) {
+    const uint32_t spb = c.cr + 4u, ppm = tx_ppm(c), p0 = tx_spare(c) + b * ppm;
+    uint32_t nib[LLR_MAX_PPM];
+    for (uint32_t x = 0; x < ppm; x++) nib[x] = rs_soft_nibble([&](uint32_t s) { return tx_payload_cw(c, s, p0 + x, spb); }, llr, spb, ppm, x);
+    for (uint32_t j = 0; j < spb; j++)
+        bins[j] = tx_block_shift([&](uint32_t y) { return tx_payload_cw(c, nib[y], p0 + y, spb); }, j, ppm, c.reduced_rate != 0u, 1u << c.sf);
+    if (nib_out)
+        for (uint32_t k = 0; k < ppm; k++) nib_out[k] = nib[k];
+}
+
+// the payload of one frame: its cr from its (corrected) header bins, replayed through rs_header as rs_frame_kernel does,
+// then n_payload / (4 + cr) blocks of llr -> bins
+LB_HD void rs_soft_payload(const RxParams &p, uint8_t phdr1, const uint32_t *hdr_bins, int32_t n_payload, uint32_t implicit_len,
+                           const float *llr, uint32_t *bins) {
+    RxStreamState st;
+    rs_header(&st, p, phdr1, hdr_bins, implicit_len);
+    TxCode c = rs_code(p, phdr1);
+    c.cr = st.phdr[1] >> 5;
+    const uint32_t spb = c.cr + 4u, ppm = tx_ppm(c);
+    for (uint32_t b = 0; b < (uint32_t)n_payload / spb; b++) rs_soft_block(c, b, llr + (size_t)b * spb * ppm, bins + (size_t)b * spb, nullptr);
 }
 
 #ifdef __CUDACC__
@@ -441,6 +513,25 @@ __global__ void rs_frame_kernel(const RsFrame *__restrict__ frames, const uint32
     rs_header(&st, p, phdr1, hdr_bins + (size_t)f * 8, implicit_len);
     const float snr = exp10f(fr.snr_db / 10.0f);          // loratap's SNR byte: the estimate in dB
     rs_frame(&st, p, bins + offs[k], fr.n_payload, recs + k, fr.stream, seq[k], snr > 1e-30f ? snr : 1e-30f);
+}
+
+// soft decisions of the header round: one thread per frame, llr[f][8][sf - 2] -> corrected bins[f][8]
+__global__ void rs_soft_header_kernel(uint32_t n, RxParams p, uint8_t phdr1, const float *__restrict__ llr, uint32_t *__restrict__ bins) {
+    const uint32_t f = blockIdx.x * blockDim.x + threadIdx.x;
+    if (f >= n) return;
+    rs_soft_header(rs_code(p, phdr1), llr + (size_t)f * 8 * (p.sf - 2u), bins + (size_t)f * 8, nullptr);
+}
+
+// soft decisions of the payload round: one thread per published frame (index list `pub`), its windows at offs[k] of
+// llr (tx_ppm values each) and bins
+__global__ void rs_soft_payload_kernel(const RsFrame *__restrict__ frames, const uint32_t *__restrict__ pub, uint32_t n_pub, RxParams p,
+                                       uint8_t phdr1, const uint32_t *__restrict__ hdr_bins, const uint32_t *__restrict__ offs,
+                                       uint32_t implicit_len, const float *__restrict__ llr, uint32_t *__restrict__ bins) {
+    const uint32_t k = blockIdx.x * blockDim.x + threadIdx.x;
+    if (k >= n_pub) return;
+    const uint32_t f = pub[k];
+    rs_soft_payload(p, phdr1, hdr_bins + (size_t)f * 8, frames[f].n_payload, implicit_len,
+                    llr + (size_t)offs[k] * tx_ppm(rs_code(p, phdr1)), bins + offs[k]);
 }
 #endif  // __CUDACC__
 

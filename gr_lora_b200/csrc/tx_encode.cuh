@@ -72,40 +72,64 @@ LB_HD uint32_t tx_payload_blocks(const TxCode &c, uint32_t len) {
 // data symbols of one frame: the 8-symbol header block and the payload blocks
 LB_HD uint32_t tx_data_symbols(const TxCode &c, uint32_t len) { return 8u + tx_payload_blocks(c, len) * (c.cr + 4u); }
 
-// whitened, shuffled and masked payload code word p (p counts from the first payload nibble; past the payload: nibble 0)
-LB_HD uint32_t tx_payload_codeword(const TxCode &c, const uint8_t *payload, uint32_t len, uint32_t p, uint32_t nbits) {
-    const uint32_t nib = p < 2u * len ? (payload[p >> 1] >> ((p & 1u) * 4u)) & 15u : 0u;
-    const uint8_t w = (uint8_t)(hamming84_encode((uint8_t)nib) ^ whitening_byte(0, c.cr, p));
+// the nibble the payload puts in payload code word p (p counts from the first payload nibble; past the payload: nibble 0)
+LB_HD uint32_t tx_payload_nibble(const uint8_t *payload, uint32_t len, uint32_t p) {
+    return p < 2u * len ? (payload[p >> 1] >> ((p & 1u) * 4u)) & 15u : 0u;
+}
+
+// the whitened, shuffled code word of nibble s at payload slot p, masked to nbits bits
+LB_HD uint32_t tx_payload_cw(const TxCode &c, uint32_t s, uint32_t p, uint32_t nbits) {
+    const uint8_t w = (uint8_t)(hamming84_encode((uint8_t)s) ^ whitening_byte(0, c.cr, p));
     return shuffle_byte(w) & ((1u << nbits) - 1u);
 }
 
-// code word x of the header block (x < sf - 2): the 5 header code words of an explicit header, then payload code words
-LB_HD uint32_t tx_header_codeword(const TxCode &c, const uint8_t *payload, uint32_t len, uint32_t x) {
+// payload code word p of the frame carrying payload[0 .. len)
+LB_HD uint32_t tx_payload_codeword(const TxCode &c, const uint8_t *payload, uint32_t len, uint32_t p, uint32_t nbits) {
+    return tx_payload_cw(c, tx_payload_nibble(payload, len, p), p, nbits);
+}
+
+// the nibble of header-block slot x (x < sf - 2): the 5 header nibbles of an explicit header, then payload nibbles
+LB_HD uint32_t tx_header_nibble(const TxCode &c, const uint8_t *payload, uint32_t len, uint32_t x) {
     if (c.explicit_hdr && x < 5u) {
         const uint32_t length = (len - 2u * c.crc) & 0xFFu, chk = header_checksum(length, c.cr, c.crc);
         const uint32_t h1 = ((c.cr & 7u) << 5) | ((c.crc & 1u) << 4) | (chk >> 4), h2 = (chk & 15u) << 4;
         const uint32_t nib[5] = {length >> 4, length & 15u, h1 >> 4, h1 & 15u, h2 >> 4};
-        return shuffle_byte((uint8_t)(hamming84_encode((uint8_t)nib[x]) ^ whitening_byte(1, c.cr, x)));
+        return nib[x];
     }
-    return tx_payload_codeword(c, payload, len, x - (c.explicit_hdr ? 5u : 0u), 8u);
+    return tx_payload_nibble(payload, len, x - (c.explicit_hdr ? 5u : 0u));
+}
+
+// the code word of nibble s at header-block slot x (8 bits; payload slots are whitened with c.cr's table)
+LB_HD uint32_t tx_header_cw(const TxCode &c, uint32_t s, uint32_t x) {
+    if (c.explicit_hdr && x < 5u) return shuffle_byte((uint8_t)(hamming84_encode((uint8_t)s) ^ whitening_byte(1, c.cr, x)));
+    return tx_payload_cw(c, s, x - (c.explicit_hdr ? 5u : 0u), 8u);
+}
+
+// code word x of the header block of the frame carrying payload[0 .. len)
+LB_HD uint32_t tx_header_codeword(const TxCode &c, const uint8_t *payload, uint32_t len, uint32_t x) {
+    return tx_header_cw(c, tx_header_nibble(c, payload, len, x), x);
+}
+
+// chirp shift of symbol i of an interleaver block whose ppm code words are cw(0 .. ppm): the word whose bit x is bit i of
+// code word x, rotated right by i, inverse Gray, x4 for reduced-rate symbols, +1 bin
+template <class CW>
+LB_HD uint32_t tx_block_shift(const CW &cw, uint32_t i, uint32_t ppm, bool reduced, uint32_t n_bins) {
+    uint32_t v = 0;
+    for (uint32_t x = 0; x < ppm; x++) v |= ((cw(x) >> i) & 1u) << x;
+    uint32_t g = gray_decode(rotr_bits(v, i, ppm));
+    if (reduced) g = (4u * g) % n_bins;
+    return (g + 1u) % n_bins;
 }
 
 // chirp shift of data symbol i (< tx_data_symbols) of the frame carrying payload[0 .. len)
 LB_HD uint32_t tx_symbol_shift(const TxCode &c, const uint8_t *payload, uint32_t len, uint32_t i) {
     const uint32_t n_bins = 1u << c.sf;
-    uint32_t v = 0, g;
-    if (i < 8u) {                                          // header block: ppm = sf - 2, 8 words, always reduced rate
-        const uint32_t ppm = c.sf - 2u;
-        for (uint32_t x = 0; x < ppm; x++) v |= ((tx_header_codeword(c, payload, len, x) >> i) & 1u) << x;
-        g = (4u * gray_decode(rotr_bits(v, i, ppm))) % n_bins;
-    } else {
-        const uint32_t spb = c.cr + 4u, ppm = tx_ppm(c), b = (i - 8u) / spb, j = (i - 8u) - b * spb;
-        const uint32_t p0 = tx_spare(c) + b * ppm;
-        for (uint32_t x = 0; x < ppm; x++) v |= ((tx_payload_codeword(c, payload, len, p0 + x, spb) >> j) & 1u) << x;
-        g = gray_decode(rotr_bits(v, j, ppm));
-        if (c.reduced_rate) g = (4u * g) % n_bins;
-    }
-    return (g + 1u) % n_bins;
+    if (i < 8u)                                            // header block: ppm = sf - 2, 8 words, always reduced rate
+        return tx_block_shift([&](uint32_t x) { return tx_header_codeword(c, payload, len, x); }, i, c.sf - 2u, true, n_bins);
+    const uint32_t spb = c.cr + 4u, ppm = tx_ppm(c), b = (i - 8u) / spb, j = (i - 8u) - b * spb;
+    const uint32_t p0 = tx_spare(c) + b * ppm;
+    return tx_block_shift([&](uint32_t x) { return tx_payload_codeword(c, payload, len, p0 + x, spb); }, j, ppm, c.reduced_rate != 0u,
+                          n_bins);
 }
 
 #ifdef __CUDACC__

@@ -181,13 +181,14 @@ class decoder:
                               ("sfo_ppm", "<f4")])       # struct lora_b200_rx_info
 
     def receive(self, iq, n_items=None, stride_items=None, host=None, sync_word=0x12, implicit_len=0, min_preamble=0,
-                max_cfo_hz=0.0, sfo_ppm=0.0, carrier_hz=0.0):
+                max_cfo_hz=0.0, sfo_ppm=0.0, carrier_hz=0.0, soft=False):
         """The dechirp-synchronised receiver (lora_b200_receive): decodes frames below the noise floor.  ``iq`` as for
         work_batch (host ndarray [n_streams, n_items] or a device tensor / pointer).  Returns (consumed, frames, info):
         consumed[s] = where stream s must be re-presented from, frames = FRAME_DTYPE records, info = RX_INFO_DTYPE records
         (first preamble sample, first data sample, stream, CFO in Hz, SNR in dB in the LoRa bandwidth, clock offset in ppm),
         one per frame.  Clock offset of a frame: sfo_ppm, plus its CFO / carrier_hz when carrier_hz (the channel's RF
-        frequency) is given -- one crystal sets a radio's carrier and its sample clock.
+        frequency) is given -- one crystal sets a radio's carrier and its sample clock.  soft: decode every code word from
+        its bits' LLRs (the spectrum of each data window, demod_llr) to the most likely nibble, instead of from the argmax.
         ``self.header_drops`` counts the explicit headers of the call whose checksum failed."""
         if isinstance(iq, np.ndarray):
             x = np.ascontiguousarray(iq, dtype=np.complex64)
@@ -201,7 +202,7 @@ class decoder:
             if stride_items is None:
                 stride_items = n_items
         p = N.RxParams(sync_word=int(sync_word) & 0xFF, implicit_len=int(implicit_len), min_preamble=int(min_preamble),
-                       max_cfo_hz=float(max_cfo_hz), sfo_ppm=float(sfo_ppm), carrier_hz=float(carrier_hz))
+                       max_cfo_hz=float(max_cfo_hz), sfo_ppm=float(sfo_ppm), carrier_hz=float(carrier_hz), soft=int(soft))
         consumed = np.zeros(self.n_streams, dtype=np.uint64)
         N.check(self._L.lora_b200_receive(self._h, ptr, int(n_items), int(stride_items), host, C.byref(p),
                                           consumed.ctypes.data_as(C.POINTER(C.c_size_t))), "lora_b200_receive")
@@ -266,6 +267,13 @@ class decoder:
         """K1 on device memory: dechirp + FFT + argmax of n_symbols aligned windows."""
         N.check(self._L.lora_b200_demod_fft_dev(self._h, _dev_ptr(iq_dev), int(n_symbols), _dev_ptr(bins_dev),
                                                _dev_ptr(mags_dev), int(cuda_stream)), "lora_b200_demod_fft_dev")
+
+    def demod_llr(self, iq_dev, n_symbols, llrs_dev, bins_dev=None, reduced=False, cuda_stream=0):
+        """Soft output of n_symbols aligned windows (lora_b200_demod_llr_dev): llrs_dev[i * ppm + j] = the max-log LLR of bit
+        j of symbol i's demodulated word in magnitude units (> 0: bit 0), ppm = sf - 2 with reduced, else sf; bins_dev
+        (optional) = the argmax bins of demod_fft."""
+        N.check(self._L.lora_b200_demod_llr_dev(self._h, _dev_ptr(iq_dev), int(n_symbols), int(bool(reduced)), _dev_ptr(llrs_dev),
+                                               _dev_ptr(bins_dev), int(cuda_stream)), "lora_b200_demod_llr_dev")
 
     def demod_fft_host(self, iq_host, bins_out=None, mags_out=None):
         """K1 end to end from host memory (copies inside). iq_host: complex64 ndarray or (ptr, n_symbols)."""

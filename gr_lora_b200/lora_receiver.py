@@ -12,7 +12,7 @@ from .decoder import decoder
 class lora_receiver:
     def __init__(self, samp_rate, center_freq, channel_list, bandwidth, sf, implicit, cr, crc, reduced_rate=False,
                  conj=False, decimation=1, disable_channelization=False, disable_drift_correction=False, cfo_feedback=False,
-                 sync="reference", sync_word=0x12, implicit_len=0, clock_from_carrier=False, **decoder_kw):
+                 sync="reference", sync_word=0x12, implicit_len=0, clock_from_carrier=False, soft=False, **decoder_kw):
         self.samp_rate, self.center_freq, self.channel_list = samp_rate, center_freq, list(channel_list)
         self.bandwidth, self.sf, self.implicit, self.cr, self.crc = bandwidth, sf, implicit, cr, crc
         self.decimation, self.conj = decimation, conj
@@ -27,6 +27,10 @@ class lora_receiver:
         if clock_from_carrier and sync != "dechirp":
             raise ValueError("clock_from_carrier needs sync='dechirp' (the reference state machine has fine_sync)")
         self.clock_from_carrier = bool(clock_from_carrier)
+        # soft: the dechirp receiver decodes every code word from its bits' LLRs (soft decisions) instead of from the argmax
+        if soft and sync != "dechirp":
+            raise ValueError("soft needs sync='dechirp' (the reference state machine makes hard decisions)")
+        self.soft = bool(soft)
         self.disable_channelization = disable_channelization
         self.disable_drift_correction = disable_drift_correction
         self.channelizer = None
@@ -111,7 +115,7 @@ class lora_receiver:
             n = min(n, n_out - pos)
             part = src[None, pos: pos + n] if isinstance(src, np.ndarray) else src + 8 * pos
             c, frames, _ = self.decoder.receive(part, n_items=n, stride_items=n, host=0, sync_word=self.sync_word,
-                                                implicit_len=self.implicit_len, carrier_hz=carrier)
+                                                implicit_len=self.implicit_len, carrier_hz=carrier, soft=self.soft)
             for f in frames:
                 self.decoder._publish(int(f["stream"]), bytes(f["bytes"][: int(f["len"])]))
             c = int(c[0])

@@ -124,6 +124,14 @@ int lora_b200_demod_fft_dev(lora_b200_decoder *d, const void *iq, size_t n_symbo
                             uint32_t *bins, float *mags, void *cuda_stream);
 int lora_b200_demod_fft_host(lora_b200_decoder *d, const void *iq, size_t n_symbols,
                              uint32_t *bins, float *mags);
+/* Soft output of the same windows, for soft-decision decoding here (lora_b200_rx_params.soft) or in the caller's own FEC:
+ * llrs[i * ppm + j] = max |tmp[k]| over the kept bins k whose demodulated word has bit j = 0, minus the same over bit j = 1
+ * (> 0: bit 0), j < ppm.  The demodulated word of bin k is the receiver's: gray((k - 1) mod N), with (k - 1) mod N first
+ * folded to N / 4 bins as reduced-rate symbols are (reduced = 1, ppm = SF - 2; reduced = 0: ppm = SF).  bins (may be NULL)
+ * = lora_b200_demod_fft_dev's argmax of the same computation.  iq 16-byte aligned; device pointers, async on cuda_stream.
+ * LORA_B200_EUNSUPPORTED unless samp_rate / bandwidth == 8 and SF7..SF12. */
+int lora_b200_demod_llr_dev(lora_b200_decoder *d, const void *iq, size_t n_symbols, int reduced, float *llrs, uint32_t *bins,
+                            void *cuda_stream);
 /* SDR-native ingest: iq_sc16 = interleaved little-endian int16 I/Q (what a USRP / file source delivers before the
  * host-side conversion to gr_complex); the device converts x * scale right after the copy, so PCIe moves 4 instead of
  * 8 bytes per sample.  Results equal lora_b200_demod_fft_host on the host-converted buffer bit for bit. */
@@ -269,10 +277,14 @@ size_t lora_b200_frames_last(lora_b200_decoder *d, const lora_b200_frame **frame
  * stream s holds a frame longer than this call's n_items: present a longer chunk (there is no per-call size limit; buffers
  * grow as needed).  At most max_frames_per_call frames per stream;
  * further preambles are held back the same way.  Frames come back through lora_b200_frames_last (delivery order: by stream,
- * then by start), their synchronisation through lora_b200_rx_info_last. */
+ * then by start), their synchronisation through lora_b200_rx_info_last.
+ * Soft decisions (p->soft = 1; other values than 0 and 1: LORA_B200_EINVAL): the data windows go through the LLR
+ * demodulator (lora_b200_demod_llr_dev) instead of K1, each code word is decoded to the nibble whose encoder code word best
+ * matches its bits' LLRs, and the bins of the re-encoded code words replace the argmax bins before the integer chain. */
 typedef struct lora_b200_rx_params {
     uint8_t  sync_word;          /* 0 = 0x12                                                    */
-    uint8_t  reserved0[3];
+    uint8_t  soft;               /* 1: soft-decision decoding (per-bit LLRs, ML code words)      */
+    uint8_t  reserved0[2];
     uint32_t implicit_len;       /* payload bytes of implicit-header frames (incl. CRC bytes)  */
     uint32_t min_preamble;       /* windows of one phase (0 = 5)                                */
     float    max_cfo_hz;         /* 0 = BW / 4; larger values are clamped to BW / 4             */

@@ -9,7 +9,10 @@ With --ppm P every frame comes from a crystal off by a per-frame offset uniform 
 CFO (ppm * 868.1 Hz, in place of the random CFO) and its clock (tx_frames_sfo); every sensitivity point and the real-time
 shape are then measured both with carrier_hz = 868.1e6 (the clock offset follows each frame's CFO) and without.  P above
 about 36 puts the CFO beyond BW/4.
-Usage: python tools/bench_rx_sync.py [--quick] [--ppm P]"""
+With --soft every capture is decoded with hard and with soft decisions (lora_b200_rx_params.soft), alternating; each SF's
+points gain two SNRs 1.5 and 3 dB below its lowest, and the stages gain the soft-decision kernels (LLR demodulator time is
+part of assemble + K1).
+Usage: python tools/bench_rx_sync.py [--quick] [--ppm P | --soft]"""
 from __future__ import annotations
 
 import argparse
@@ -83,15 +86,15 @@ def genie_ser(torch, sf, snr, n=2048, seed=1):
     return float((bins != vals).float().mean().item())
 
 
-def stages(torch, rx, out, n_items, carrier_hz=0.0):
+def stages(torch, rx, out, n_items, **kw):
     from torch.profiler import ProfilerActivity, profile
-    rx.receive(out, n_items=n_items, carrier_hz=carrier_hz)
+    rx.receive(out, n_items=n_items, **kw)
     torch.cuda.synchronize()
     with profile(activities=[ProfilerActivity.CUDA]) as prof:
-        rx.receive(out, n_items=n_items, carrier_hz=carrier_hz)
+        rx.receive(out, n_items=n_items, **kw)
         torch.cuda.synchronize()
     ev = sorted([e for e in prof.events() if e.device_type.name == "CUDA"], key=lambda e: e.time_range.start)
-    t = {"screen": 0.0, "detect": 0.0, "sync": 0.0, "assemble_k1": 0.0, "integer_chain": 0.0, "copies": 0.0}
+    t = {"screen": 0.0, "detect": 0.0, "sync": 0.0, "assemble_k1": 0.0, "soft_decisions": 0.0, "integer_chain": 0.0, "copies": 0.0}
     seen_detect = False
     for e in ev:
         name, us = e.name, e.time_range.elapsed_us()
@@ -100,6 +103,8 @@ def stages(torch, rx, out, n_items, carrier_hz=0.0):
             seen_detect = True
         elif "rs_sync" in name:
             t["sync"] += us
+        elif "rs_soft" in name:
+            t["soft_decisions"] += us
         elif "rs_header" in name or "rs_frame" in name or "k8_frames" in name:
             t["integer_chain"] += us
         elif "Memcpy" in name or "Memset" in name or "memcpy" in name or "memset" in name:
@@ -117,7 +122,11 @@ def main():
     ap.add_argument("--repeats", type=int, default=5, help="timed calls of the real-time shape, and profiled calls")
     ap.add_argument("--runs", type=int, default=3, help="independent captures (seeds) per sensitivity point")
     ap.add_argument("--ppm", type=float, default=0.0, help="per-frame crystal offset uniform in +-PPM at 868.1 MHz (0: none)")
+    ap.add_argument("--soft", action="store_true", help="decode every capture with hard and with soft decisions, alternating, "
+                    "at two more SNRs 1.5 and 3 dB below each SF's lowest point")
     a = ap.parse_args()
+    if a.soft and a.ppm:
+        raise SystemExit("--soft and --ppm each compare two modes: give one of them")
     if abs(a.ppm) * CARRIER * 1e-6 > BW / 4:
         raise SystemExit(f"--ppm {a.ppm}: a CFO of {a.ppm * CARRIER * 1e-6:.0f} Hz is beyond BW/4")
     import torch
@@ -133,18 +142,23 @@ def main():
     ns = 32 if a.quick else 96
     res["ppm"] = a.ppm
     # with --ppm, every measurement with the clock offset following the CFO ("tracked") and without ("fixed")
-    modes = {"tracked": CARRIER, "fixed": 0.0} if a.ppm else {"": 0.0}
+    # with --soft, every measurement with hard and with soft decisions
+    modes = ({"tracked": dict(carrier_hz=CARRIER), "fixed": dict(carrier_hz=0.0)} if a.ppm else
+             {"hard": dict(soft=False), "soft": dict(soft=True)} if a.soft else {"": {}})
+    res["soft"] = a.soft
     curve = {}
     for sf, pts in POINTS.items():
         rr = sf >= 11
         row = []
+        if a.soft:
+            pts = list(pts) + [min(pts) - 1.5, min(pts) - 3.0]
         for snr in pts:
             oks, n = {m: [] for m in modes}, 0
             for r in range(a.runs):
                 out, placed, n_items = capture(torch, sf, ns, 1, snr, seed=sf * 100 + int(snr * 10) % 97 + 7919 * r, ppm=a.ppm)
                 rx = dec(sf, rr, n_streams=ns, max_items_per_call=n_items)
-                for m, carrier in modes.items():
-                    _, frames, _ = rx.receive(out, n_items=n_items, carrier_hz=carrier)
+                for m, kw in modes.items():
+                    _, frames, _ = rx.receive(out, n_items=n_items, **kw)
                     oks[m].append(decoded(frames, placed))
                 n = len(placed)
                 rx.close()
@@ -160,16 +174,16 @@ def main():
     # config-4 shape: 384 SF7 streams x 2 s, frames 3 dB above the sensitivity point
     out, placed, n_items = capture(torch, 7, 384, 40, 1.0, seed=4, n_items=2_000_000, ppm=a.ppm)
     rx = dec(7, False, n_streams=384, max_items_per_call=n_items, max_frames_per_call=64)
-    for m, carrier in modes.items():
-        runs = [stages(torch, rx, out, n_items, carrier) for _ in range(a.repeats)]
+    for m, kw in modes.items():
+        runs = [stages(torch, rx, out, n_items, **kw) for _ in range(a.repeats)]
         res["stages_ms" + (m and "_" + m)] = {k: {"median": float(np.median([r[k] for r in runs])), "min": min(r[k] for r in runs),
                                                   "max": max(r[k] for r in runs)} for k in runs[0]}
     times = {m: [] for m in modes}
     for _ in range(a.repeats):                       # the modes alternate, so that both see the same conditions
-        for m, carrier in modes.items():
+        for m, kw in modes.items():
             torch.cuda.synchronize()
             t0 = time.perf_counter()
-            _, frames, _ = rx.receive(out, n_items=n_items, carrier_hz=carrier)
+            _, frames, _ = rx.receive(out, n_items=n_items, **kw)
             times[m].append(time.perf_counter() - t0)
             med = float(np.median(times[m]))
             res["realtime" + (m and "_" + m)] = {
