@@ -1307,6 +1307,55 @@ static_assert(sizeof(lora_b200_rx_info) == 32 && sizeof(lora_b200_rx_params) == 
               offsetof(lora_b200_rx_params, sfo_ppm) == 16 &&
               offsetof(lora_b200_rx_params, carrier_hz) == 24 && offsetof(lora_b200_rx_info, sfo_ppm) == 28, "lora_b200_rx_* layout");
 
+}  // extern "C"
+
+template <int SF>
+static int rs_window_launch(lora_b200_decoder *d, const float2 *x, size_t n_items, const RsWindowQuery *q, size_t n, float2 *out,
+                            float *energy) {
+    rs_window_kernel<SF><<<(unsigned)n, RX_THREADS, 0, d->rx_stream>>>(x, (long long)n_items, tab<float2>(d, d->toff.down),
+                                                                       tab<float2>(d, d->toff.up), tab<float2>(d, d->toff.tw), d->sps, q,
+                                                                       out, energy);
+    return launched(d);
+}
+
+extern "C" {
+
+int lora_b200_rs_window_dev(lora_b200_decoder *d, const void *iq, size_t n_items, size_t n, const int64_t *pos, const float *cfo_bins,
+                            const int32_t *up, const int32_t *bin, void *out, float *energy) {
+    if (!d || (n && (!iq || !pos || !cfo_bins || !up || !bin || !out))) return fail(LORA_B200_EINVAL, "null argument");
+    if (!d->k1_ok) return fail(LORA_B200_EUNSUPPORTED, "the dechirp receiver needs samp_rate/bandwidth == 8 and SF7..SF12");
+    if (n > 0x7FFFFFFFu) return fail(LORA_B200_EINVAL, "too many windows: %zu", n);
+    const long long sps = d->sps, N = d->n_bins;
+    std::vector<RsWindowQuery> q(n);
+    for (size_t i = 0; i < n; i++) {
+        if (pos[i] < 0 || pos[i] + sps > (long long)n_items)
+            return fail(LORA_B200_EINVAL, "window %zu: [%lld, %lld) is not inside the row of %zu samples", i, (long long)pos[i],
+                        (long long)pos[i] + sps, n_items);
+        if (up[i] != 0 && up[i] != 1) return fail(LORA_B200_EINVAL, "window %zu: up must be 0 or 1, got %d", i, up[i]);
+        if (bin[i] < -N / 2 || bin[i] >= N / 2) return fail(LORA_B200_EINVAL, "window %zu: bin %d outside -N/2..N/2-1", i, bin[i]);
+        if (!std::isfinite(cfo_bins[i]) || std::fabs(cfo_bins[i]) > (float)N)
+            return fail(LORA_B200_EINVAL, "window %zu: cfo_bins %g is not finite within +-N", i, (double)cfo_bins[i]);
+        q[i] = RsWindowQuery{(long long)pos[i], cfo_bins[i], up[i], bin[i], 0};
+    }
+    CU(cudaSetDevice(d->device));
+    if (n == 0) return LORA_B200_OK;
+    DeviceBuffer<RsWindowQuery> dq;
+    CU(dq.reserve(n));
+    CU(cudaMemcpyAsync(dq, q.data(), sizeof(RsWindowQuery) * n, cudaMemcpyHostToDevice, d->rx_stream));
+    const float2 *x = (const float2 *)iq;
+    int rc = LORA_B200_EUNSUPPORTED;
+    switch (d->cfg.sf) {
+    case 7: rc = rs_window_launch<7>(d, x, n_items, dq, n, (float2 *)out, energy); break;
+    case 8: rc = rs_window_launch<8>(d, x, n_items, dq, n, (float2 *)out, energy); break;
+    case 9: rc = rs_window_launch<9>(d, x, n_items, dq, n, (float2 *)out, energy); break;
+    case 10: rc = rs_window_launch<10>(d, x, n_items, dq, n, (float2 *)out, energy); break;
+    case 11: rc = rs_window_launch<11>(d, x, n_items, dq, n, (float2 *)out, energy); break;
+    case 12: rc = rs_window_launch<12>(d, x, n_items, dq, n, (float2 *)out, energy); break;
+    }
+    CU(cudaStreamSynchronize(d->rx_stream));     // (before dq is freed)
+    return rc;
+}
+
 size_t lora_b200_rx_info_last(lora_b200_decoder *d, const lora_b200_rx_info **info, uint32_t *hdr_drops) {
     if (!d || !info) { fail(LORA_B200_EINVAL, "null argument"); return 0; }
     *info = d->rs_info.data();

@@ -462,6 +462,29 @@ rs_sync_kernel(const float2 *__restrict__ iq, size_t stride, size_t n_items, con
     }
 }
 
+// the synchroniser's window sums on their own (lora_b200_rs_window_dev), so that they can be held to a float64 reference:
+// one CTA per query, RsDevOps::binval and ::energy of the window at pos
+struct RsWindowQuery {
+    long long pos;
+    float cfo_bins;
+    int32_t up, bin, pad;
+};
+
+template <int SF>
+__global__ void __launch_bounds__(RX_THREADS)
+rs_window_kernel(const float2 *__restrict__ x, long long n_items, const float2 *down, const float2 *up, const float2 *tw, uint32_t sps,
+                 const RsWindowQuery *__restrict__ q, float2 *__restrict__ out, float *__restrict__ energy) {
+    __shared__ RxShared sh;
+    RsDevOps<SF> ops{x, n_items, down, up, tw, sps, nullptr, &sh};   // (binval and energy use no dynamic shared memory)
+    const RsWindowQuery w = q[blockIdx.x];
+    const float2 v = ops.binval(w.pos, w.cfo_bins, w.up != 0, w.bin);
+    const float e = ops.energy(w.pos);
+    if (threadIdx.x == 0) {
+        out[blockIdx.x] = v;
+        if (energy) energy[blockIdx.x] = e;
+    }
+}
+
 // assemble: frame f's windows k = 0 .. cnt-1 (first data symbol `first` + k) de-rotated by its CFO into
 // out[(off_f + k) * sps ..]; off_f = f * 8 and cnt = 8 without tables (the header round).  One CTA per frame.
 // With idx, frame f is frames[idx[f]] and its windows go to (offs[f] - off_base) * sps.  Each window is read from its own

@@ -275,6 +275,19 @@ class decoder:
         N.check(self._L.lora_b200_demod_llr_dev(self._h, _dev_ptr(iq_dev), int(n_symbols), int(bool(reduced)), _dev_ptr(llrs_dev),
                                                _dev_ptr(bins_dev), int(cuda_stream)), "lora_b200_demod_llr_dev")
 
+    def rs_window(self, iq_dev, n_items, pos, cfo_bins, up, bins, out_dev, energy_dev=None):
+        """The dechirp receiver's window sums (lora_b200_rs_window_dev): out_dev[i] (complex64) = bin bins[i] of the window at
+        pos[i] of the row iq_dev, dechirped with the up-chirp (up[i]) or the down-chirp and de-rotated by cfo_bins[i] bins;
+        energy_dev[i] = its energy.  pos, cfo_bins, up, bins: host sequences of one length."""
+        p = np.ascontiguousarray(pos, dtype=np.int64)
+        f = np.ascontiguousarray(cfo_bins, dtype=np.float32)
+        u = np.ascontiguousarray(up, dtype=np.int32)
+        b = np.ascontiguousarray(bins, dtype=np.int32)
+        assert p.shape == f.shape == u.shape == b.shape and p.ndim == 1
+        N.check(self._L.lora_b200_rs_window_dev(self._h, _dev_ptr(iq_dev), int(n_items), p.size, p.ctypes.data, f.ctypes.data,
+                                               u.ctypes.data, b.ctypes.data, _dev_ptr(out_dev), _dev_ptr(energy_dev)),
+                "lora_b200_rs_window_dev")
+
     def demod_fft_host(self, iq_host, bins_out=None, mags_out=None):
         """K1 end to end from host memory (copies inside). iq_host: complex64 ndarray or (ptr, n_symbols)."""
         if isinstance(iq_host, tuple):

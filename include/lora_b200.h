@@ -132,6 +132,13 @@ int lora_b200_demod_fft_host(lora_b200_decoder *d, const void *iq, size_t n_symb
  * LORA_B200_EUNSUPPORTED unless samp_rate / bandwidth == 8 and SF7..SF12. */
 int lora_b200_demod_llr_dev(lora_b200_decoder *d, const void *iq, size_t n_symbols, int reduced, float *llrs, uint32_t *bins,
                             void *cuda_stream);
+/* The window sums the dechirp receiver's synchroniser (lora_b200_receive) measures, on their own, to check them against a
+ * reference: for window i, out[i] = sum_n x[pos[i] + n] c[n] exp(-2 pi j (cfo_bins[i] (pos[i] + n) + bin[i] n) / sps),
+ * n < sps, c the down-chirp table (up[i] = 0) or the up-chirp table (up[i] = 1), x the row iq of n_items samples; energy
+ * (may be NULL) = sum |x|^2 over the window.  Every window inside the row, bin in -N/2..N/2-1, |cfo_bins| <= N.  iq, out
+ * (float2[n]) and energy are device pointers, pos, cfo_bins, up and bin host arrays; returns when the results are written. */
+int lora_b200_rs_window_dev(lora_b200_decoder *d, const void *iq, size_t n_items, size_t n, const int64_t *pos, const float *cfo_bins,
+                            const int32_t *up, const int32_t *bin, void *out, float *energy);
 /* SDR-native ingest: iq_sc16 = interleaved little-endian int16 I/Q (what a USRP / file source delivers before the
  * host-side conversion to gr_complex); the device converts x * scale right after the copy, so PCIe moves 4 instead of
  * 8 bytes per sample.  Results equal lora_b200_demod_fft_host on the host-converted buffer bit for bit. */
