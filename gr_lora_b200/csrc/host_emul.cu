@@ -19,37 +19,59 @@
 #include <cstring>
 #include <vector>
 
-extern "C" {
-
-int lb_k1_emulate(int sf, const float2 *x, size_t n_symbols, const float2 *chirp, const float2 *tw,
-                  uint32_t *bins, float *mags) {
-    lb::K1Args a{x, chirp, tw, n_symbols};
+template <int D>
+static int k1_emulate_d(int sf, const lb::K1Args &a, uint32_t *bins, float *mags) {
     switch (sf) {
-    case 7: lb::k1_emulate<7>(a, bins, mags); break;
-    case 8: lb::k1_emulate<8>(a, bins, mags); break;
-    case 9: lb::k1_emulate<9>(a, bins, mags); break;
-    case 10: lb::k1_emulate<10>(a, bins, mags); break;
-    case 11: lb::k1_emulate<11>(a, bins, mags); break;
-    case 12: lb::k1_emulate<12>(a, bins, mags); break;
+    case 7: lb::k1_emulate<7, D>(a, bins, mags); break;
+    case 8: lb::k1_emulate<8, D>(a, bins, mags); break;
+    case 9: lb::k1_emulate<9, D>(a, bins, mags); break;
+    case 10: lb::k1_emulate<10, D>(a, bins, mags); break;
+    case 11: lb::k1_emulate<11, D>(a, bins, mags); break;
+    case 12: lb::k1_emulate<12, D>(a, bins, mags); break;
     default: return -1;
     }
     return 0;
 }
 
-// the LLR demodulator k1_llr_kernel (k1_llr.cuh) on the host: llrs[i * ppm ..], bins may be NULL
-int lb_k1_llr_emulate(int sf, const float2 *x, size_t n_symbols, const float2 *chirp, const float2 *tw, int reduced, float *llrs,
-                      uint32_t *bins) {
-    lb::K1Args a{x, chirp, tw, n_symbols};
+template <int D>
+static int k1_llr_emulate_d(int sf, const lb::K1Args &a, bool reduced, float *llrs, uint32_t *bins) {
     switch (sf) {
-    case 7: lb::k1_llr_emulate<7>(a, reduced != 0, llrs, bins); break;
-    case 8: lb::k1_llr_emulate<8>(a, reduced != 0, llrs, bins); break;
-    case 9: lb::k1_llr_emulate<9>(a, reduced != 0, llrs, bins); break;
-    case 10: lb::k1_llr_emulate<10>(a, reduced != 0, llrs, bins); break;
-    case 11: lb::k1_llr_emulate<11>(a, reduced != 0, llrs, bins); break;
-    case 12: lb::k1_llr_emulate<12>(a, reduced != 0, llrs, bins); break;
+    case 7: lb::k1_llr_emulate<7, D>(a, reduced, llrs, bins); break;
+    case 8: lb::k1_llr_emulate<8, D>(a, reduced, llrs, bins); break;
+    case 9: lb::k1_llr_emulate<9, D>(a, reduced, llrs, bins); break;
+    case 10: lb::k1_llr_emulate<10, D>(a, reduced, llrs, bins); break;
+    case 11: lb::k1_llr_emulate<11, D>(a, reduced, llrs, bins); break;
+    case 12: lb::k1_llr_emulate<12, D>(a, reduced, llrs, bins); break;
     default: return -1;
     }
     return 0;
+}
+
+extern "C" {
+
+// k1_fft_kernel<SF, D> on the host, D = osr = sps / N (8 or 2); -1 for another SF or D
+int lb_k1_emulate_osr(int sf, int osr, const float2 *x, size_t n_symbols, const float2 *chirp, const float2 *tw, uint32_t *bins,
+                      float *mags) {
+    const lb::K1Args a{x, chirp, tw, n_symbols};
+    return osr == 8 ? k1_emulate_d<8>(sf, a, bins, mags) : osr == 2 ? k1_emulate_d<2>(sf, a, bins, mags) : -1;
+}
+
+int lb_k1_emulate(int sf, const float2 *x, size_t n_symbols, const float2 *chirp, const float2 *tw,
+                  uint32_t *bins, float *mags) {
+    return lb_k1_emulate_osr(sf, 8, x, n_symbols, chirp, tw, bins, mags);
+}
+
+// the LLR demodulator k1_llr_kernel<SF, D> (k1_llr.cuh) on the host, D = osr: llrs[i * ppm ..], bins may be NULL
+int lb_k1_llr_emulate_osr(int sf, int osr, const float2 *x, size_t n_symbols, const float2 *chirp, const float2 *tw, int reduced,
+                          float *llrs, uint32_t *bins) {
+    const lb::K1Args a{x, chirp, tw, n_symbols};
+    return osr == 8 ? k1_llr_emulate_d<8>(sf, a, reduced != 0, llrs, bins) : osr == 2 ? k1_llr_emulate_d<2>(sf, a, reduced != 0, llrs, bins) : -1;
+}
+
+// ... at fs/bw = 8
+int lb_k1_llr_emulate(int sf, const float2 *x, size_t n_symbols, const float2 *chirp, const float2 *tw, int reduced, float *llrs,
+                      uint32_t *bins) {
+    return lb_k1_llr_emulate_osr(sf, 8, x, n_symbols, chirp, tw, reduced, llrs, bins);
 }
 
 int lb_k1_emulate_warp_sf7(const float2 *x, size_t n_symbols, const float2 *chirp, const float2 *tw, uint32_t *bins, float *mags) {
@@ -174,12 +196,12 @@ struct RsHostOps {
     const float2 *x;
     long long n_items;
     const float2 *down, *up, *tw;
-    uint32_t sps, sf;
+    uint32_t sps, sf, osr;
     bool in_range(long long pos) const { return pos >= 0 && pos + (long long)sps <= n_items; }
     unsigned long long argmax(long long pos, bool use_up) {
         uint32_t b;
         float m;
-        lb_k1_emulate((int)sf, x + pos, 1, use_up ? up : down, tw, &b, &m);
+        lb_k1_emulate_osr((int)sf, (int)osr, x + pos, 1, use_up ? up : down, tw, &b, &m);
         return lb::pack_key(m * m, b);
     }
     float2 binval(long long pos, float F, bool use_up, int bin) {
@@ -220,35 +242,38 @@ void rs_host_bins(const RsHostOps &o, const lb::RsFrame &r, uint32_t first, uint
     const std::vector<float2> w = rs_host_windows(o, r, first, cnt);
     bins.resize(cnt);
     std::vector<float> mags(cnt);
-    lb_k1_emulate((int)o.sf, w.data(), cnt, o.down, o.tw, bins.data(), mags.data());
+    lb_k1_emulate_osr((int)o.sf, (int)o.osr, w.data(), cnt, o.down, o.tw, bins.data(), mags.data());
 }
 
 // ... through the LLR demodulator
 void rs_host_llrs(const RsHostOps &o, const lb::RsFrame &r, uint32_t first, uint32_t cnt, bool reduced, std::vector<float> &llr) {
     const std::vector<float2> w = rs_host_windows(o, r, first, cnt);
     llr.resize((size_t)cnt * (reduced ? o.sf - 2 : o.sf));
-    lb_k1_llr_emulate((int)o.sf, w.data(), cnt, o.down, o.tw, reduced, llr.data(), nullptr);
+    lb_k1_llr_emulate_osr((int)o.sf, (int)o.osr, w.data(), cnt, o.down, o.tw, reduced, llr.data(), nullptr);
 }
 
 }  // namespace
 
 extern "C" {
 
-// The whole dechirp-synchronised receive path (rx_sync.cuh) of one row on the host (fs = 1 MHz, BW = 125 kHz): screen,
+// The whole dechirp-synchronised receive path (rx_sync.cuh) of one row on the host (BW = 125 kHz, fs = osr x BW with
+// osr = 8 or 2, the decoder's sps / N; other values return 0 frames): screen,
 // detect, synchronise, header and payload rounds, integer chain.  sfo_ppm and carrier_hz as in lora_b200_rx_params.  Per
 // synchronised frame f (at most cap): start[f], cfo_bins[f], snr_db[f], status[f] (0 published, 1 header checksum failed,
 // 2 incomplete), the clock offset its windows were placed with sfo[f] (may be NULL) and, when published, its payload in
 // payload[f * 256 ..] with length len[f].  Returns the number of synchronised frames.
 // soft != 0: soft decisions, as lora_b200_rx_params.soft (the LLR demodulator's emulation and the soft block decoder).
-uint32_t lb_emul_rx_receive_soft(const float2 *x, size_t n_items, const float2 *down, const float2 *up, const float2 *tw, uint32_t sf,
-                                 uint32_t cr, int implicit, int crc, int reduced_rate, uint32_t sync_word, uint32_t implicit_len,
-                                 uint32_t min_preamble, float sfo_ppm, double carrier_hz, int soft, long long *start, float *cfo_bins,
-                                 float *snr_db, int32_t *status, float *sfo, uint8_t *payload, uint32_t *len, uint32_t cap) {
-    const uint32_t N = 1u << sf, sps = 8u * N;
+uint32_t lb_emul_rx_receive_osr(const float2 *x, size_t n_items, const float2 *down, const float2 *up, const float2 *tw, uint32_t sf,
+                                uint32_t osr, uint32_t cr, int implicit, int crc, int reduced_rate, uint32_t sync_word,
+                                uint32_t implicit_len, uint32_t min_preamble, float sfo_ppm, double carrier_hz, int soft,
+                                long long *start, float *cfo_bins, float *snr_db, int32_t *status, float *sfo, uint8_t *payload,
+                                uint32_t *len, uint32_t cap) {
+    if (osr != 8u && osr != 2u) return 0;
+    const uint32_t N = 1u << sf, sps = osr * N;
     const double bin_hz = 125e3 / N;
-    lb::RsParams p{sps, N, 8u, sfo_ppm, min_preamble ? min_preamble : 5u, {((sync_word >> 4) & 15u) * 8u % N, (sync_word & 15u) * 8u % N},
+    lb::RsParams p{sps, N, osr, sfo_ppm, min_preamble ? min_preamble : 5u, {((sync_word >> 4) & 15u) * 8u % N, (sync_word & 15u) * 8u % N},
                    (float)N / 4.0f, carrier_hz > 0.0 ? (float)(1e6 * bin_hz / carrier_hz) : 0.0f};
-    RsHostOps o{x, (long long)n_items, down, up, tw, sps, sf};
+    RsHostOps o{x, (long long)n_items, down, up, tw, sps, sf, osr};
     // screen
     std::vector<uint32_t> bins[2];
     std::vector<float> mags[2];
@@ -257,7 +282,7 @@ uint32_t lb_emul_rx_receive_soft(const float2 *x, size_t n_items, const float2 *
         n[ph] = n_items >= sps + ph * sps / 2 ? (uint32_t)((n_items - ph * sps / 2) / sps) : 0u;
         bins[ph].resize(n[ph] + 1);
         mags[ph].resize(n[ph] + 1);
-        if (n[ph]) lb_k1_emulate((int)sf, x + ph * sps / 2, n[ph], down, tw, bins[ph].data(), mags[ph].data());
+        if (n[ph]) lb_k1_emulate_osr((int)sf, (int)osr, x + ph * sps / 2, n[ph], down, tw, bins[ph].data(), mags[ph].data());
     }
     const uint32_t *bp[2] = {bins[0].data(), bins[1].data()};
     const float *mp[2] = {mags[0].data(), mags[1].data()};
@@ -266,7 +291,7 @@ uint32_t lb_emul_rx_receive_soft(const float2 *x, size_t n_items, const float2 *
     const uint32_t nc = std::min<uint32_t>(lb::rs_detect_stream(bp, mp, n, p, cands.data(), 64, &dropped), 64u);
     lb::RxParams rp;
     memset(&rp, 0, sizeof rp);
-    rp.sf = sf; rp.n_bins = N; rp.n_bins_hdr = N / 4; rp.sps = sps; rp.decim = 8; rp.implicit = implicit; rp.reduced_rate = reduced_rate;
+    rp.sf = sf; rp.n_bins = N; rp.n_bins_hdr = N / 4; rp.sps = sps; rp.decim = osr; rp.implicit = implicit; rp.reduced_rate = reduced_rate;
     const uint8_t phdr1 = (uint8_t)(((cr & 7u) << 5) | (crc ? 1u << 4 : 0u));
     uint32_t nf = 0;
     for (uint32_t c = 0; c < nc && nf < cap; c++) {
@@ -308,6 +333,15 @@ uint32_t lb_emul_rx_receive_soft(const float2 *x, size_t n_items, const float2 *
         nf++;
     }
     return nf;
+}
+
+// lb_emul_rx_receive_osr at fs/bw = 8 (fs = 1 MHz)
+uint32_t lb_emul_rx_receive_soft(const float2 *x, size_t n_items, const float2 *down, const float2 *up, const float2 *tw, uint32_t sf,
+                                 uint32_t cr, int implicit, int crc, int reduced_rate, uint32_t sync_word, uint32_t implicit_len,
+                                 uint32_t min_preamble, float sfo_ppm, double carrier_hz, int soft, long long *start, float *cfo_bins,
+                                 float *snr_db, int32_t *status, float *sfo, uint8_t *payload, uint32_t *len, uint32_t cap) {
+    return lb_emul_rx_receive_osr(x, n_items, down, up, tw, sf, 8u, cr, implicit, crc, reduced_rate, sync_word, implicit_len,
+                                  min_preamble, sfo_ppm, carrier_hz, soft, start, cfo_bins, snr_db, status, sfo, payload, len, cap);
 }
 
 // the header and payload rounds of one frame whose n_windows data windows are given (no synchronisation): as bins

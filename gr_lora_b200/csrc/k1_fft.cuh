@@ -8,7 +8,9 @@
 //     bin    = first argmax |tmp|                                (:452-463)
 // without ever forming the 7N unused bins:  with n = 8*n1 + r (sps = 8N at fs/bw = 8)
 //     F[k'] = sum_r W_sps^{k' r} G_r[k' mod N],   G_r = N-point DFT over n1 of m[8 n1 + r]
-// i.e. 8 N-point FFTs (one per polyphase branch) and one 8-term twiddled sum per kept bin.
+// i.e. 8 N-point FFTs (one per polyphase branch) and one 8-term twiddled sum per kept bin.  The phase functions take the
+// oversampling factor D = sps / N as a template argument (default 8); at fs/bw = 2 the same sum has D = 2 branches
+// (n = 2 n1 + r) and the split below starts at SF12 (sub-problems of up to 2048 bins).
 // For SF11/12 (N > 1024) a radix-S decimation-in-frequency step (S = 2, 4) is folded into
 // the load:  F[S q + s] = DFT_{sps/S}( y_s )[q],  y_s[n] = W_sps^{s n} sum_j W_S^{s j} m[n + j sps/S],
 // giving S independent sub-problems of N' = N/S = 1024 bins whose partial argmaxes are
@@ -28,25 +30,36 @@ namespace lb {
 
 constexpr int K1_THREADS = 256;
 
-template <int SF>
+LB_HD constexpr int k1_log2(int v) { return v > 1 ? 1 + k1_log2(v >> 1) : 0; }
+
+// D = sps / N, the oversampling factor: D polyphase branches (8 at fs/bw = 8, 2 at fs/bw = 2).  Every CTA batch holds
+// G * D * NP = 8192 samples whatever D is, so a symbol's share of the threads and of shared memory scales with D * NP.
+template <int SF, int D = 8>
 struct K1Cfg {
     static constexpr int N = 1 << SF;                 // bins
-    static constexpr int SPS = 8 * N;                 // samples per symbol (fs/bw = 8)
-    static constexpr int S = SF <= 10 ? 1 : (1 << (SF - 10));   // DIF split factor
-    static constexpr int NP = N / S;                  // bins per sub-problem (128..1024)
-    static constexpr int SPS_SUB = 8 * NP;
-    static constexpr int G = 1024 / NP;               // symbols per CTA batch
+    static constexpr int SPS = D * N;                 // samples per symbol
+    static constexpr int NP_MAX = D == 8 ? 1024 : 2048;   // the passes below cover sub-problems of up to 2048 bins
+    static constexpr int S = N <= NP_MAX ? 1 : N / NP_MAX;   // DIF split factor
+    static constexpr int NP = N / S;                  // bins per sub-problem (128..1024 at D = 8, 128..2048 at D = 2)
+    static constexpr int SPS_SUB = D * NP;
+    static constexpr int HB = D / 2;                  // float4 loads (2 adjacent branches each) per row in pass 0
+    static constexpr int G = 8192 / (D * NP);         // symbols per CTA batch
     static constexpr int M0 = NP / 16;                // columns after the radix-16 pass 0
     static constexpr int SB0 = NP + NP / 16;
-    static constexpr int SB = SB0 + ((2 - SB0 % 16) + 16) % 16;   // branch stride, == 2 (mod 16)
-    static constexpr int SYM_STRIDE = 8 * SB;
+    // branch stride, == 2 (mod 16) at D = 8; == 4 (mod 16) at D = 2, where a half-warp can span two symbols (M0 = 8) and
+    // their strides must then fall 8 float2 apart
+    static constexpr int SB = SB0 + (((D == 8 ? 2 : 4) - SB0 % 16) + 16) % 16;
+    static constexpr int SYM_STRIDE = D * SB;
     static constexpr int SMEM_ELEMS = G * SYM_STRIDE; // float2 elements
     static constexpr int TPS = K1_THREADS / G;        // threads per symbol in the combine phase
+    static constexpr int W = TPS < 32 ? TPS : 32;     // lanes of one argmax reduction group (one symbol's, or the warp)
     // passes after pass 0 on blocks of M0 points: (R1, SIG1) then (R2, 1)
     static constexpr int R1 = M0 == 8 ? 8 : M0 == 16 ? 16 : 8;
-    static constexpr int SIG1 = M0 / R1;              // 1, 1, 4, 8
-    static constexpr int R2 = SIG1;                   // 1 (none), 1, 4, 8
+    static constexpr int SIG1 = M0 / R1;              // 1, 1, 4, 8 (16 for NP = 2048)
+    static constexpr int R2 = SIG1;                   // 1 (none), 1, 4, 8 (16)
     static_assert(SF >= 7 && SF <= 12, "K1 supports SF7..SF12");
+    static_assert(D == 8 || D == 2, "K1 runs at fs/bw = 8 or 2");
+    static_assert(G * TPS == K1_THREADS && G * M0 * HB == K1_THREADS, "one thread per pass-0 column pair and combine slot");
 };
 
 LB_HD int k1_pad(int i) { return i + (i >> 4); }
@@ -105,19 +118,21 @@ LB_HD void k1_store(uint32_t *bins, float *mags, size_t i, unsigned long long ke
 }
 
 // ---- pass 0: global -> registers -> radix-16 -> shared ---------------------------------
-template <int SF, bool AL16 = true>
+// Thread (g, m, b) of symbol g holds branches 2b and 2b + 1 of column m: HB = D / 2 threads per column
+template <int SF, bool AL16 = true, int D = 8>
 LB_HD void k1_pass0(const K1Args &a, size_t batch, int s, int tid, float2 *buf) {
-    using C = K1Cfg<SF>;
-    const int g = tid / (4 * C::M0);
-    const int rem = tid % (4 * C::M0);
-    const int m = rem >> 2, b = rem & 3;
+    using C = K1Cfg<SF, D>;
+    constexpr int HB_LOG = k1_log2(C::HB);
+    const int g = tid / (C::HB * C::M0);
+    const int rem = tid % (C::HB * C::M0);
+    const int m = rem >> HB_LOG, b = rem & (C::HB - 1);
     const size_t sym = batch * C::G + g;
     const bool valid = sym < a.n_symbols;
     const float2 *xs = a.x + (valid ? sym : 0) * (size_t)C::SPS;
     float2 v0[16], v1[16];
 #pragma unroll
     for (int c = 0; c < 16; c++) {
-        const int n = 8 * (c * C::M0 + m) + 2 * b;       // index inside the sub-problem
+        const int n = D * (c * C::M0 + m) + 2 * b;       // index inside the sub-problem
         if (C::S == 1) {
             const float4 xv = k1_ld_stream<AL16>(xs + n);
             const float4 dv = k1_ld_table4(a.chirp + n);
@@ -146,7 +161,7 @@ LB_HD void k1_pass0(const K1Args &a, size_t batch, int s, int tid, float2 *buf) 
     // inter-pass twiddle W_{N'}^{m kc} = u^kc with the lane-invariant base u = W_{N'}^m: one table
     // load and a running product instead of 15 scattered loads (they were half of the L1 wavefronts
     // in the first profile).  15 fp32 products in a row: relative error < 2e-6.
-    const float2 u = k1_ld_table(a.tw + m * 8 * C::S);
+    const float2 u = k1_ld_table(a.tw + m * D * C::S);
     float2 t = make_float2(1.0f, 0.0f);
 #pragma unroll
     for (int kc = 0; kc < 16; kc++) {
@@ -164,14 +179,14 @@ LB_HD void k1_pass0(const K1Args &a, size_t batch, int s, int tid, float2 *buf) 
 }
 
 // ---- in-place shared-memory pass of radix R, stride SIG (in n1 units) -------------------
-template <int SF, int R, int SIG>
+template <int SF, int R, int SIG, int D = 8>
 LB_HD void k1_pass(const K1Args &a, int tid, float2 *buf) {
-    using C = K1Cfg<SF>;
+    using C = K1Cfg<SF, D>;
     constexpr int PER_BRANCH = C::NP / R;
-    constexpr int ITEMS = C::G * 8 * PER_BRANCH;
+    constexpr int ITEMS = C::G * D * PER_BRANCH;
     for (int it = tid; it < ITEMS; it += K1_THREADS) {
         const int j = it % PER_BRANCH;
-        const int gr = it / PER_BRANCH;                  // g * 8 + r
+        const int gr = it / PER_BRANCH;                  // g * D + r
         const int lo = j % SIG;
         const int base = (j / SIG) * (R * SIG) + lo;
         float2 *p = buf + gr * C::SB;
@@ -194,9 +209,9 @@ LB_HD void k1_pass(const K1Args &a, int tid, float2 *buf) {
 }
 
 // position p (inside one branch) -> sub-problem bin q held there after all passes
-template <int SF>
+template <int SF, int D = 8>
 LB_HD int k1_pos_to_bin(int p) {
-    using C = K1Cfg<SF>;
+    using C = K1Cfg<SF, D>;
     const int d0 = p / C::M0, dr = p % C::M0;
     int rest;
     if (C::SIG1 == 1) rest = dr;                          // one more pass: digit d1 = dr
@@ -204,38 +219,40 @@ LB_HD int k1_pos_to_bin(int p) {
     return d0 + 16 * rest;
 }
 
-// ---- combine: 8-branch twiddled sum, |.|^2, per-thread argmax over its 4 positions -------
+// ---- combine: D-branch twiddled sum, |.|^2, per-thread argmax over its NP/TPS positions ---
+// (4 positions at D = 8, 16 at D = 2).  At signed bin -N/2 the sum is F[sps - N/2] (tmp[N/2], :447) and plus_quirk adds
+// F[N/2] with the conjugate twiddle (:450): two distinct bins for any D > 1.
 // lane-invariant combine twiddles W_{sps'}^{qs} for the thread's NP/TPS positions (hoisted out of
 // the persistent loop: they were 4 scattered loads per thread and batch)
-template <int SF>
+template <int SF, int D = 8>
 LB_HD void k1_combine_twiddles(const K1Args &a, int tid, float2 *w) {
-    using C = K1Cfg<SF>;
+    using C = K1Cfg<SF, D>;
     const int lt = tid % C::TPS;
     for (int i = 0; i < C::NP / C::TPS; i++) {
-        const int q = k1_pos_to_bin<SF>(lt + C::TPS * i);
+        const int q = k1_pos_to_bin<SF, D>(lt + C::TPS * i);
         const int qs = q < C::NP / 2 ? q : q - C::NP;
         w[i] = k1_ld_table(a.tw + ((qs * C::S) & (C::SPS - 1)));
     }
 }
 
-template <int SF>
+template <int SF, int D = 8>
 LB_HD unsigned long long k1_combine(const K1Args &a, int s, int tid, const float2 *buf, const float2 *wtab) {
-    using C = K1Cfg<SF>;
+    using C = K1Cfg<SF, D>;
     const int g = tid / C::TPS, lt = tid % C::TPS;
     const float2 *bs = buf + g * C::SYM_STRIDE;
     unsigned long long best = 0ull;
 #pragma unroll
     for (int i = 0; i < C::NP / C::TPS; i++) {
         const int p = lt + C::TPS * i;
-        const int q = k1_pos_to_bin<SF>(p);
+        const int q = k1_pos_to_bin<SF, D>(p);
         const int qs = q < C::NP / 2 ? q : q - C::NP;      // signed bin of the sub-problem
         const float2 w = wtab[i];                          // W_{sps'}^{qs}
         const int pp = k1_pad(p);
-        float2 gv[8];
+        float2 gv[D];
 #pragma unroll
-        for (int r = 0; r < 8; r++) gv[r] = bs[r * C::SB + pp];
-        float2 acc = horner<8>(gv, w);
-        if (s == 0 && q == C::NP / 2) acc = plus_quirk<8>(acc, gv, w);
+        for (int r = 0; r < D; r++) gv[r] = bs[r * C::SB + pp];
+        float2 acc = horner<D>(gv, w);
+        if (s == 0 && q == C::NP / 2) acc = plus_quirk<D>(acc, gv, w);
         const int kp = C::S * qs + s;
         const uint32_t idx = (uint32_t)(kp >= 0 ? kp : C::N + kp);
         const unsigned long long key = pack_key(cnorm2(acc), idx);
@@ -246,37 +263,40 @@ LB_HD unsigned long long k1_combine(const K1Args &a, int s, int tid, const float
 
 #ifdef __CUDACC__
 // ---- the kernel: persistent CTAs over (batch, s) work items ------------------------------
-template <int SF>
+// D = 8: fs/bw = 8; D = 2: fs/bw = 2, where one symbol's combine spans fewer than 32 lanes at SF7 and SF8 and each group
+// of W = TPS lanes reduces on its own
+template <int SF, int D = 8>
 __global__ void __launch_bounds__(K1_THREADS, 2)
 k1_fft_kernel(K1Args a, uint32_t *__restrict__ bins, float *__restrict__ mags,
               unsigned long long *__restrict__ packed /* S > 1 only */) {
-    using C = K1Cfg<SF>;
+    using C = K1Cfg<SF, D>;
+    constexpr int W_LOG = k1_log2(C::W);
     extern __shared__ float2 k1_smem[];
-    __shared__ unsigned long long warp_best[K1_THREADS / 32];
+    __shared__ unsigned long long warp_best[K1_THREADS / C::W];
     float2 *buf = k1_smem;
     const int tid = threadIdx.x;
     const size_t n_batches = (a.n_symbols + C::G - 1) / C::G;
     const size_t n_work = n_batches * C::S;
     float2 wtab[C::NP / C::TPS];
-    k1_combine_twiddles<SF>(a, tid, wtab);
+    k1_combine_twiddles<SF, D>(a, tid, wtab);
     for (size_t w = blockIdx.x; w < n_work; w += gridDim.x) {
         const size_t batch = w / C::S;
         const int s = (int)(w % C::S);
-        k1_pass0<SF>(a, batch, s, tid, buf);
+        k1_pass0<SF, true, D>(a, batch, s, tid, buf);
         __syncthreads();
-        k1_pass<SF, C::R1, C::SIG1>(a, tid, buf);
+        k1_pass<SF, C::R1, C::SIG1, D>(a, tid, buf);
         __syncthreads();
         if (C::R2 > 1) {
-            k1_pass<SF, (C::R2 > 1 ? C::R2 : 2), 1>(a, tid, buf);
+            k1_pass<SF, (C::R2 > 1 ? C::R2 : 2), 1, D>(a, tid, buf);
             __syncthreads();
         }
-        unsigned long long best = k1_combine<SF>(a, s, tid, buf, wtab);
-        // warp argmax, then across the warps of one symbol
-        best = warp_max_key(best);
-        if ((tid & 31) == 0) warp_best[tid >> 5] = best;
+        unsigned long long best = k1_combine<SF, D>(a, s, tid, buf, wtab);
+        // group argmax (the warp, or one symbol's lanes), then across the groups of one symbol
+        best = group_max_key<C::W>(best);
+        if ((tid & (C::W - 1)) == 0) warp_best[tid >> W_LOG] = best;
         __syncthreads();
         if (tid < C::G) {
-            constexpr int WPS = C::TPS / 32;              // warps per symbol
+            constexpr int WPS = C::TPS / C::W;            // groups per symbol
             unsigned long long bb = 0ull;
 #pragma unroll
             for (int k = 0; k < WPS; k++) {
@@ -295,23 +315,23 @@ k1_fft_kernel(K1Args a, uint32_t *__restrict__ bins, float *__restrict__ mags,
 #endif  // __CUDACC__
 
 // ---- CPU emulation of the kernel (same phase functions, threads run one after another) ---
-template <int SF>
+template <int SF, int D = 8>
 inline void k1_emulate(const K1Args &a, uint32_t *bins, float *mags) {
-    using C = K1Cfg<SF>;
+    using C = K1Cfg<SF, D>;
     float2 *buf = new float2[C::SMEM_ELEMS];
     const size_t n_batches = (a.n_symbols + C::G - 1) / C::G;
     unsigned long long *packed = new unsigned long long[n_batches * C::G]();
     for (size_t batch = 0; batch < n_batches; batch++) {
         for (int s = 0; s < C::S; s++) {
             for (int i = 0; i < C::SMEM_ELEMS; i++) buf[i] = make_float2(NAN, NAN);   // catch unwritten reads
-            for (int t = 0; t < K1_THREADS; t++) k1_pass0<SF>(a, batch, s, t, buf);
-            for (int t = 0; t < K1_THREADS; t++) k1_pass<SF, C::R1, C::SIG1>(a, t, buf);
+            for (int t = 0; t < K1_THREADS; t++) k1_pass0<SF, true, D>(a, batch, s, t, buf);
+            for (int t = 0; t < K1_THREADS; t++) k1_pass<SF, C::R1, C::SIG1, D>(a, t, buf);
             if (C::R2 > 1)
-                for (int t = 0; t < K1_THREADS; t++) k1_pass<SF, (C::R2 > 1 ? C::R2 : 2), 1>(a, t, buf);
+                for (int t = 0; t < K1_THREADS; t++) k1_pass<SF, (C::R2 > 1 ? C::R2 : 2), 1, D>(a, t, buf);
             for (int t = 0; t < K1_THREADS; t++) {
                 float2 wtab[C::NP / C::TPS];
-                k1_combine_twiddles<SF>(a, t, wtab);
-                const unsigned long long k = k1_combine<SF>(a, s, t, buf, wtab);
+                k1_combine_twiddles<SF, D>(a, t, wtab);
+                const unsigned long long k = k1_combine<SF, D>(a, s, t, buf, wtab);
                 const size_t sym = batch * C::G + t / C::TPS;
                 if (k > packed[sym]) packed[sym] = k;
             }

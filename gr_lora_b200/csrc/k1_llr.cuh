@@ -8,7 +8,8 @@
 // close to linear in |X| at the per-symbol SNRs the dechirp receiver works at, and one frame shares one noise level, so a
 // maximum-likelihood decision over these LLRs needs no SNR scale.
 //
-// The phases are K1's own (k1_pass0, k1_pass, k1_combine_twiddles, the horner<8> / plus_quirk sum per kept bin), so the
+// The phases are K1's own (k1_pass0, k1_pass, k1_combine_twiddles, the horner<D> / plus_quirk sum per kept bin, D = sps / N
+// = 8 or 2), so the
 // argmax key -- and the bin reported beside the LLRs -- is k1_fft_kernel's bit for bit.  The epilogue keeps 2 SF running
 // maxima of |X|^2 per thread and takes square roots only at the end.  At SF11/SF12 a CTA loops over the S sub-problems
 // of its symbol (as RsDevOps::argmax does): each warp's maxima are kept in shared memory between them, and no merge pass
@@ -54,23 +55,23 @@ struct LlrAcc {
 };
 
 // k1_combine's loop with the LLR epilogue: the thread's kept bins of sub-problem s into acc
-template <int SF>
+template <int SF, int D = 8>
 LB_HD void k1_llr_combine(const K1Args &a, int s, int tid, const float2 *buf, const float2 *wtab, bool reduced, LlrAcc<SF> &acc) {
-    using C = K1Cfg<SF>;
+    using C = K1Cfg<SF, D>;
     const int g = tid / C::TPS, lt = tid % C::TPS;
     const float2 *bs = buf + g * C::SYM_STRIDE;
 #pragma unroll
     for (int i = 0; i < C::NP / C::TPS; i++) {
         const int p = lt + C::TPS * i;
-        const int q = k1_pos_to_bin<SF>(p);
+        const int q = k1_pos_to_bin<SF, D>(p);
         const int qs = q < C::NP / 2 ? q : q - C::NP;
         const float2 w = wtab[i];
         const int pp = k1_pad(p);
-        float2 gv[8];
+        float2 gv[D];
 #pragma unroll
-        for (int r = 0; r < 8; r++) gv[r] = bs[r * C::SB + pp];
-        float2 v = horner<8>(gv, w);
-        if (s == 0 && q == C::NP / 2) v = plus_quirk<8>(v, gv, w);
+        for (int r = 0; r < D; r++) gv[r] = bs[r * C::SB + pp];
+        float2 v = horner<D>(gv, w);
+        if (s == 0 && q == C::NP / 2) v = plus_quirk<D>(v, gv, w);
         const int kp = C::S * qs + s;
         const uint32_t idx = (uint32_t)(kp >= 0 ? kp : C::N + kp);
         const float m2 = cnorm2(v);
@@ -82,40 +83,49 @@ LB_HD void k1_llr_combine(const K1Args &a, int s, int tid, const float2 *buf, co
 
 #ifdef __CUDACC__
 LB_D float warp_max_nonneg(float v) { return __uint_as_float(__reduce_max_sync(0xffffffffu, __float_as_uint(v))); }
+// ... of each aligned group of W lanes (W = 32: the warp)
+template <int W>
+LB_D float group_max_nonneg(float v) {
+    if (W == 32) return warp_max_nonneg(v);
+#pragma unroll
+    for (int o = W / 2; o > 0; o >>= 1) v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, o));
+    return v;
+}
 
 // llrs[i * ppm + j] of symbol i, bins[i] its K1 argmax (may be NULL).  Persistent CTAs over batches of G symbols.
-template <int SF>
+// A "warp" below is a reduction group of C::W lanes: the warp at D = 8, one symbol's TPS < 32 lanes at D = 2, SF7 / SF8.
+template <int SF, int D = 8>
 __global__ void __launch_bounds__(K1_THREADS, 2)
 k1_llr_kernel(K1Args a, int reduced, float *__restrict__ llrs, uint32_t *__restrict__ bins) {
-    using C = K1Cfg<SF>;
-    constexpr int NW = K1_THREADS / 32, WPS = C::TPS / 32;   // warps, warps per symbol
+    using C = K1Cfg<SF, D>;
+    constexpr int NW = K1_THREADS / C::W, WPS = C::TPS / C::W, W_LOG = k1_log2(C::W);   // groups, groups per symbol
     extern __shared__ float2 llr_smem[];
     __shared__ float wm[NW][2 * SF];
     __shared__ unsigned long long wkey[NW];
     float2 *buf = llr_smem;
-    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, ppm = reduced ? SF - 2 : SF;
+    const int tid = threadIdx.x, lane = tid & (C::W - 1), warp = tid >> W_LOG, ppm = reduced ? SF - 2 : SF;
     const size_t n_batches = (a.n_symbols + C::G - 1) / C::G;
     float2 wtab[C::NP / C::TPS];
-    k1_combine_twiddles<SF>(a, tid, wtab);
+    k1_combine_twiddles<SF, D>(a, tid, wtab);
     for (size_t batch = blockIdx.x; batch < n_batches; batch += gridDim.x) {
 #pragma unroll 1
         for (int s = 0; s < C::S; s++) {
-            k1_pass0<SF>(a, batch, s, tid, buf);
+            k1_pass0<SF, true, D>(a, batch, s, tid, buf);
             __syncthreads();
-            k1_pass<SF, C::R1, C::SIG1>(a, tid, buf);
+            k1_pass<SF, C::R1, C::SIG1, D>(a, tid, buf);
             __syncthreads();
             if (C::R2 > 1) {
-                k1_pass<SF, (C::R2 > 1 ? C::R2 : 2), 1>(a, tid, buf);
+                k1_pass<SF, (C::R2 > 1 ? C::R2 : 2), 1, D>(a, tid, buf);
                 __syncthreads();
             }
             LlrAcc<SF> acc;
             acc.init();
-            k1_llr_combine<SF>(a, s, tid, buf, wtab, reduced != 0, acc);
-            // the warp's maxima, kept over the sub-problems by its lane 0 (a warp never spans two symbols: TPS >= 32)
-            const unsigned long long key = warp_max_key(acc.key);
+            k1_llr_combine<SF, D>(a, s, tid, buf, wtab, reduced != 0, acc);
+            // the group's maxima, kept over the sub-problems by its lane 0 (a group never spans two symbols)
+            const unsigned long long key = group_max_key<C::W>(acc.key);
 #pragma unroll
             for (int j = 0; j < SF; j++) {
-                const float m0 = warp_max_nonneg(acc.m0[j]), m1 = warp_max_nonneg(acc.m1[j]);
+                const float m0 = group_max_nonneg<C::W>(acc.m0[j]), m1 = group_max_nonneg<C::W>(acc.m1[j]);
                 if (lane == 0) {
                     wm[warp][2 * j] = s ? fmaxf(wm[warp][2 * j], m0) : m0;
                     wm[warp][2 * j + 1] = s ? fmaxf(wm[warp][2 * j + 1], m1) : m1;
@@ -146,9 +156,9 @@ k1_llr_kernel(K1Args a, int reduced, float *__restrict__ llrs, uint32_t *__restr
 #endif  // __CUDACC__
 
 // ---- CPU emulation of the kernel (same phase functions, threads run one after another) ---
-template <int SF>
+template <int SF, int D = 8>
 inline void k1_llr_emulate(const K1Args &a, bool reduced, float *llrs, uint32_t *bins) {
-    using C = K1Cfg<SF>;
+    using C = K1Cfg<SF, D>;
     float2 *buf = new float2[C::SMEM_ELEMS];
     const size_t n_batches = (a.n_symbols + C::G - 1) / C::G;
     const int ppm = reduced ? SF - 2 : SF;
@@ -157,16 +167,16 @@ inline void k1_llr_emulate(const K1Args &a, bool reduced, float *llrs, uint32_t 
         for (int g = 0; g < C::G; g++) acc[g].init();
         for (int s = 0; s < C::S; s++) {
             for (int i = 0; i < C::SMEM_ELEMS; i++) buf[i] = make_float2(NAN, NAN);   // catch unwritten reads
-            for (int t = 0; t < K1_THREADS; t++) k1_pass0<SF>(a, batch, s, t, buf);
-            for (int t = 0; t < K1_THREADS; t++) k1_pass<SF, C::R1, C::SIG1>(a, t, buf);
+            for (int t = 0; t < K1_THREADS; t++) k1_pass0<SF, true, D>(a, batch, s, t, buf);
+            for (int t = 0; t < K1_THREADS; t++) k1_pass<SF, C::R1, C::SIG1, D>(a, t, buf);
             if (C::R2 > 1)
-                for (int t = 0; t < K1_THREADS; t++) k1_pass<SF, (C::R2 > 1 ? C::R2 : 2), 1>(a, t, buf);
+                for (int t = 0; t < K1_THREADS; t++) k1_pass<SF, (C::R2 > 1 ? C::R2 : 2), 1, D>(a, t, buf);
             for (int t = 0; t < K1_THREADS; t++) {
                 float2 wtab[C::NP / C::TPS];
-                k1_combine_twiddles<SF>(a, t, wtab);
+                k1_combine_twiddles<SF, D>(a, t, wtab);
                 LlrAcc<SF> r;
                 r.init();
-                k1_llr_combine<SF>(a, s, t, buf, wtab, reduced, r);
+                k1_llr_combine<SF, D>(a, s, t, buf, wtab, reduced, r);
                 acc[t / C::TPS].merge(r);
             }
         }

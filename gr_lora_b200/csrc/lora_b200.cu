@@ -83,6 +83,7 @@ struct lora_b200_decoder : A1Params {
     uint32_t n_bins_hdr, decim;
     double bits_per_second, bits_per_symbol;
     bool k1_ok;                           // fs/bw == 8 and SF7..12: FFT kernels usable
+    bool k1_osr2;                         // fs/bw == 2 and SF7..12: the generic K1 and LLR kernels at D = 2 usable
     int device, n_sms;
     Tables toff;
     DeviceBuffer<uint8_t> d_tables;
@@ -217,15 +218,15 @@ const T *tab(const lora_b200_decoder *d, size_t off) { return (const T *)(d->d_t
 int launched(lora_b200_decoder *d) { d->launches++; CU(cudaGetLastError()); return LORA_B200_OK; }
 
 // ---- K1 launch -----------------------------------------------------------------------------
-template <int SF>
+template <int SF, int D = 8>
 int k1_launch_generic(const K1Launch &k) {
-    using C = K1Cfg<SF>;
+    using C = K1Cfg<SF, D>;
     static DeviceOnce once;
     const size_t smem = sizeof(float2) * C::SMEM_ELEMS;
-    K1_CU(once(k.device, [&] { return cudaFuncSetAttribute(k1_fft_kernel<SF>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem); }));
+    K1_CU(once(k.device, [&] { return cudaFuncSetAttribute(k1_fft_kernel<SF, D>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem); }));
     const size_t n_work = ((k.a.n_symbols + C::G - 1) / C::G) * C::S;
     const int grid = (int)std::min<size_t>(n_work, (size_t)k.n_sms * 2);
-    k1_fft_kernel<SF><<<grid, K1_THREADS, smem, k.st>>>(k.a, k.bins, k.mags, k.packed);
+    k1_fft_kernel<SF, D><<<grid, K1_THREADS, smem, k.st>>>(k.a, k.bins, k.mags, k.packed);
     K1_CU(cudaGetLastError());
     return 0;
 }
@@ -274,16 +275,31 @@ K1Launcher k1_launcher(int sf, bool generic) {
     return nullptr;
 }
 
+// fs/bw = 2: the generic kernel at D = 2 for every SF (it splits a symbol at SF12 only)
+K1Launcher k1_launcher_osr2(int sf) {
+    static_assert(K1Cfg<11, 2>::S == 1 && K1Cfg<12, 2>::S == 2, "k1_fft_kernel<SF, 2> splits SF12 only");
+    switch (sf) {
+    case 7: return k1_launch_generic<7, 2>;
+    case 8: return k1_launch_generic<8, 2>;
+    case 9: return k1_launch_generic<9, 2>;
+    case 10: return k1_launch_generic<10, 2>;
+    case 11: return k1_launch_generic<11, 2>;
+    case 12: return k1_launch_generic<12, 2>;
+    }
+    return nullptr;
+}
+
 int dispatch_k1_impl(lora_b200_decoder *d, K1Scratch &ks, const float2 *iq, size_t n, uint32_t *bins, float *mags, cudaStream_t st) {
-    if (!d->k1_ok) return fail(LORA_B200_EUNSUPPORTED, "FFT demodulator needs samp_rate/bandwidth == 8 and SF7..SF12");
+    if (!d->k1_ok && !d->k1_osr2) return fail(LORA_B200_EUNSUPPORTED, "FFT demodulator needs samp_rate/bandwidth == 8 or 2 and SF7..SF12");
     if (n == 0) return LORA_B200_OK;
     static const char *rows = getenv("LORA_B200_K1_ROWS");
     const int sf = (int)d->cfg.sf;
     const bool generic = k1_generic() || (sf >= 11 && rows && rows[0] == '0');
-    const K1Launcher launch = k1_launcher(sf, generic);
+    const K1Launcher launch = d->k1_osr2 ? k1_launcher_osr2(sf) : k1_launcher(sf, generic);
     if (!launch) return fail(LORA_B200_EUNSUPPORTED, "unsupported SF %u", d->cfg.sf);
-    // the kernels that split a symbol (every SF12 kernel, the generic one at SF11) merge partial argmax keys in ks.packed
-    const bool split = sf == 12 || (sf == 11 && generic);
+    // the kernels that split a symbol (every SF12 kernel, the generic one at SF11 at fs/bw = 8) merge partial argmax keys in
+    // ks.packed
+    const bool split = sf == 12 || (sf == 11 && generic && !d->k1_osr2);
     if (split) {
         CU(ks.packed.reserve(n));
         CU(cudaMemsetAsync(ks.packed, 0, sizeof(unsigned long long) * n, st));
@@ -315,31 +331,36 @@ int dispatch_k1(lora_b200_decoder *d, K1Scratch &ks, const float2 *iq, size_t n,
 }
 
 // ---- the LLR demodulator (k1_llr.cuh) ----------------------------------------------------------
-template <int SF>
+template <int SF, int D>
 int llr_launch(lora_b200_decoder *d, const float2 *iq, size_t n, bool reduced, float *llrs, uint32_t *bins, cudaStream_t st) {
-    using C = K1Cfg<SF>;
+    using C = K1Cfg<SF, D>;
     static DeviceOnce once;
     const size_t smem = sizeof(float2) * C::SMEM_ELEMS;
-    CU(once(d->device, [&] { return cudaFuncSetAttribute(k1_llr_kernel<SF>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem); }));
+    CU(once(d->device, [&] { return cudaFuncSetAttribute(k1_llr_kernel<SF, D>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem); }));
     const size_t n_batches = (n + C::G - 1) / C::G;
     const int grid = (int)std::min<size_t>(n_batches, (size_t)d->n_sms * 2);
-    k1_llr_kernel<SF><<<grid, K1_THREADS, smem, st>>>(K1Args{iq, tab<float2>(d, d->toff.down), tab<float2>(d, d->toff.tw), n},
-                                                      reduced ? 1 : 0, llrs, bins);
+    k1_llr_kernel<SF, D><<<grid, K1_THREADS, smem, st>>>(K1Args{iq, tab<float2>(d, d->toff.down), tab<float2>(d, d->toff.tw), n},
+                                                         reduced ? 1 : 0, llrs, bins);
     return launched(d);
 }
 
-int dispatch_llr(lora_b200_decoder *d, const float2 *iq, size_t n, bool reduced, float *llrs, uint32_t *bins, cudaStream_t st) {
-    if (!d->k1_ok) return fail(LORA_B200_EUNSUPPORTED, "the LLR demodulator needs samp_rate/bandwidth == 8 and SF7..SF12");
-    if (n == 0) return LORA_B200_OK;
+template <int D>
+int dispatch_llr_d(lora_b200_decoder *d, const float2 *iq, size_t n, bool reduced, float *llrs, uint32_t *bins, cudaStream_t st) {
     switch (d->cfg.sf) {
-    case 7: return llr_launch<7>(d, iq, n, reduced, llrs, bins, st);
-    case 8: return llr_launch<8>(d, iq, n, reduced, llrs, bins, st);
-    case 9: return llr_launch<9>(d, iq, n, reduced, llrs, bins, st);
-    case 10: return llr_launch<10>(d, iq, n, reduced, llrs, bins, st);
-    case 11: return llr_launch<11>(d, iq, n, reduced, llrs, bins, st);
-    case 12: return llr_launch<12>(d, iq, n, reduced, llrs, bins, st);
+    case 7: return llr_launch<7, D>(d, iq, n, reduced, llrs, bins, st);
+    case 8: return llr_launch<8, D>(d, iq, n, reduced, llrs, bins, st);
+    case 9: return llr_launch<9, D>(d, iq, n, reduced, llrs, bins, st);
+    case 10: return llr_launch<10, D>(d, iq, n, reduced, llrs, bins, st);
+    case 11: return llr_launch<11, D>(d, iq, n, reduced, llrs, bins, st);
+    case 12: return llr_launch<12, D>(d, iq, n, reduced, llrs, bins, st);
     }
     return fail(LORA_B200_EUNSUPPORTED, "unsupported SF %u", d->cfg.sf);
+}
+
+int dispatch_llr(lora_b200_decoder *d, const float2 *iq, size_t n, bool reduced, float *llrs, uint32_t *bins, cudaStream_t st) {
+    if (!d->k1_ok && !d->k1_osr2) return fail(LORA_B200_EUNSUPPORTED, "the LLR demodulator needs samp_rate/bandwidth == 8 or 2 and SF7..SF12");
+    if (n == 0) return LORA_B200_OK;
+    return d->k1_osr2 ? dispatch_llr_d<2>(d, iq, n, reduced, llrs, bins, st) : dispatch_llr_d<8>(d, iq, n, reduced, llrs, bins, st);
 }
 
 // ---- stream-path launch -----------------------------------------------------------------------
@@ -579,6 +600,7 @@ lora_b200_decoder *lora_b200_create(const lora_b200_config *cfg) {
         return nullptr;
     }
     d->k1_ok = (d->sps == 8u * d->n_bins) && cfg->sf >= 7 && cfg->sf <= 12;
+    d->k1_osr2 = (d->sps == 2u * d->n_bins) && cfg->sf >= 7 && cfg->sf <= 12;
     if (cfg->demod == LORA_B200_DEMOD_FFT && !d->k1_ok) {
         fail(LORA_B200_EUNSUPPORTED, "FFT demodulator needs samp_rate/bandwidth == 8 and SF7..SF12");
         return nullptr;
@@ -692,7 +714,7 @@ int lora_b200_demod_fft_dev(lora_b200_decoder *d, const void *iq, size_t n_symbo
 
 int lora_b200_demod_llr_dev(lora_b200_decoder *d, const void *iq, size_t n_symbols, int reduced, float *llrs, uint32_t *bins, void *stream) {
     if (!d || (n_symbols && (!iq || !llrs))) return fail(LORA_B200_EINVAL, "null argument");
-    if (!d->k1_ok) return fail(LORA_B200_EUNSUPPORTED, "the LLR demodulator needs samp_rate/bandwidth == 8 and SF7..SF12");
+    if (!d->k1_ok && !d->k1_osr2) return fail(LORA_B200_EUNSUPPORTED, "the LLR demodulator needs samp_rate/bandwidth == 8 or 2 and SF7..SF12");
     if (((uintptr_t)iq & 15u) != 0) return fail(LORA_B200_EINVAL, "iq must be 16-byte aligned");
     if (reduced != 0 && reduced != 1) return fail(LORA_B200_EINVAL, "reduced must be 0 or 1, got %d", reduced);
     CU(cudaSetDevice(d->device));
@@ -703,7 +725,7 @@ int lora_b200_demod_llr_dev(lora_b200_decoder *d, const void *iq, size_t n_symbo
 // own keys / exchange scratch).  elem = 8: gr_complex; elem = 4: int16 I/Q, converted on the device right after the copy.
 static int demod_fft_host_any(lora_b200_decoder *d, const void *iq, size_t elem, float scale, size_t n_symbols, uint32_t *bins, float *mags) {
     if (!d || (!iq && n_symbols) || (!bins && n_symbols)) return fail(LORA_B200_EINVAL, "null argument");
-    if (!d->k1_ok) return fail(LORA_B200_EUNSUPPORTED, "FFT demodulator needs samp_rate/bandwidth == 8 and SF7..SF12");
+    if (!d->k1_ok && !d->k1_osr2) return fail(LORA_B200_EUNSUPPORTED, "FFT demodulator needs samp_rate/bandwidth == 8 or 2 and SF7..SF12");
     CU(cudaSetDevice(d->device));
     const size_t sym_bytes = sizeof(float2) * (size_t)d->sps, sym_in = elem * (size_t)d->sps;
     const bool sc16 = elem == 4;
@@ -1061,33 +1083,38 @@ int lora_b200_tx_frames_sfo_dev(lora_b200_decoder *d, const void *up_table, cons
 }  // extern "C"
 
 // ---- lora_b200_receive: the dechirp-synchronised receiver (rx_sync.cuh), every launch on rx_stream ----------------------
-template <int SF, bool DRIFT>
+template <int SF, int D, bool DRIFT>
 static int rs_launch_sync(lora_b200_decoder *d, const float2 *x, size_t stride, size_t n_items, const RsParams &rp, uint32_t cap) {
     static DeviceOnce once;
-    const size_t smem = sizeof(float2) * K1Cfg<SF>::SMEM_ELEMS;
-    CU(once(d->device, [&] { return cudaFuncSetAttribute(rs_sync_kernel<SF, DRIFT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem); }));
-    rs_sync_kernel<SF, DRIFT><<<d->cfg.n_streams * cap, RX_THREADS, smem, d->rx_stream>>>(
+    const size_t smem = sizeof(float2) * K1Cfg<SF, D>::SMEM_ELEMS;
+    CU(once(d->device, [&] { return cudaFuncSetAttribute(rs_sync_kernel<SF, D, DRIFT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem); }));
+    rs_sync_kernel<SF, D, DRIFT><<<d->cfg.n_streams * cap, RX_THREADS, smem, d->rx_stream>>>(
         x, stride, n_items, tab<float2>(d, d->toff.down), tab<float2>(d, d->toff.up), tab<float2>(d, d->toff.tw), rp, d->d_rs_cands,
         d->d_rs_ncand, cap, d->d_rs_frames, d->d_rs_nframes, d->cfg.n_streams * cap, d->d_rs_hold);
     return launched(d);
 }
 
-template <bool DRIFT>
+template <int D, bool DRIFT>
 static int rs_sync_sf(lora_b200_decoder *d, const float2 *x, size_t stride, size_t n_items, const RsParams &rp, uint32_t cap) {
     switch (d->cfg.sf) {
-    case 7: return rs_launch_sync<7, DRIFT>(d, x, stride, n_items, rp, cap);
-    case 8: return rs_launch_sync<8, DRIFT>(d, x, stride, n_items, rp, cap);
-    case 9: return rs_launch_sync<9, DRIFT>(d, x, stride, n_items, rp, cap);
-    case 10: return rs_launch_sync<10, DRIFT>(d, x, stride, n_items, rp, cap);
-    case 11: return rs_launch_sync<11, DRIFT>(d, x, stride, n_items, rp, cap);
-    case 12: return rs_launch_sync<12, DRIFT>(d, x, stride, n_items, rp, cap);
+    case 7: return rs_launch_sync<7, D, DRIFT>(d, x, stride, n_items, rp, cap);
+    case 8: return rs_launch_sync<8, D, DRIFT>(d, x, stride, n_items, rp, cap);
+    case 9: return rs_launch_sync<9, D, DRIFT>(d, x, stride, n_items, rp, cap);
+    case 10: return rs_launch_sync<10, D, DRIFT>(d, x, stride, n_items, rp, cap);
+    case 11: return rs_launch_sync<11, D, DRIFT>(d, x, stride, n_items, rp, cap);
+    case 12: return rs_launch_sync<12, D, DRIFT>(d, x, stride, n_items, rp, cap);
     }
     return fail(LORA_B200_EUNSUPPORTED, "unsupported SF %u", d->cfg.sf);
 }
 
-// without a clock offset the synchroniser runs its DRIFT = false instantiation, which does no drift arithmetic
+// without a clock offset the synchroniser runs its DRIFT = false instantiation, which does no drift arithmetic; D = sps / N
+// (8 or 2) selects the K1 phase functions of its argmax windows
+template <int D>
+static int rs_sync_d(lora_b200_decoder *d, const float2 *x, size_t stride, size_t n_items, const RsParams &rp, uint32_t cap) {
+    return rs_drift(rp) ? rs_sync_sf<D, true>(d, x, stride, n_items, rp, cap) : rs_sync_sf<D, false>(d, x, stride, n_items, rp, cap);
+}
 static int rs_sync(lora_b200_decoder *d, const float2 *x, size_t stride, size_t n_items, const RsParams &rp, uint32_t cap) {
-    return rs_drift(rp) ? rs_sync_sf<true>(d, x, stride, n_items, rp, cap) : rs_sync_sf<false>(d, x, stride, n_items, rp, cap);
+    return d->k1_osr2 ? rs_sync_d<2>(d, x, stride, n_items, rp, cap) : rs_sync_d<8>(d, x, stride, n_items, rp, cap);
 }
 
 extern "C" {
@@ -1096,7 +1123,7 @@ int lora_b200_receive(lora_b200_decoder *d, const void *iq, size_t n_items, size
                       const lora_b200_rx_params *prm, size_t *consumed) {
     if (!d || !consumed || (!iq && n_items)) return fail(LORA_B200_EINVAL, "null argument");
     if (stride_items < n_items) return fail(LORA_B200_EINVAL, "stride_items %zu < n_items %zu", stride_items, n_items);
-    if (!d->k1_ok) return fail(LORA_B200_EUNSUPPORTED, "the dechirp receiver needs samp_rate/bandwidth == 8 and SF7..SF12");
+    if (!d->k1_ok && !d->k1_osr2) return fail(LORA_B200_EUNSUPPORTED, "the dechirp receiver needs samp_rate/bandwidth == 8 or 2 and SF7..SF12");
     lora_b200_rx_params P;
     memset(&P, 0, sizeof P);
     if (prm) P = *prm;
@@ -1323,7 +1350,7 @@ extern "C" {
 int lora_b200_rs_window_dev(lora_b200_decoder *d, const void *iq, size_t n_items, size_t n, const int64_t *pos, const float *cfo_bins,
                             const int32_t *up, const int32_t *bin, void *out, float *energy) {
     if (!d || (n && (!iq || !pos || !cfo_bins || !up || !bin || !out))) return fail(LORA_B200_EINVAL, "null argument");
-    if (!d->k1_ok) return fail(LORA_B200_EUNSUPPORTED, "the dechirp receiver needs samp_rate/bandwidth == 8 and SF7..SF12");
+    if (!d->k1_ok && !d->k1_osr2) return fail(LORA_B200_EUNSUPPORTED, "the dechirp receiver needs samp_rate/bandwidth == 8 or 2 and SF7..SF12");
     if (n > 0x7FFFFFFFu) return fail(LORA_B200_EINVAL, "too many windows: %zu", n);
     const long long sps = d->sps, N = d->n_bins;
     std::vector<RsWindowQuery> q(n);

@@ -200,6 +200,17 @@ LB_D unsigned long long warp_max_key(unsigned long long k) {
     const uint32_t l = __reduce_max_sync(0xffffffffu, hi == m ? (uint32_t)k : 0u);
     return ((unsigned long long)m << 32) | (unsigned long long)l;
 }
+// Maximum key of each aligned group of W lanes (W a power of two <= 32) in every lane of the group; W = 32 is warp_max_key
+template <int W>
+LB_D unsigned long long group_max_key(unsigned long long k) {
+    if (W == 32) return warp_max_key(k);
+#pragma unroll
+    for (int o = W / 2; o > 0; o >>= 1) {
+        const unsigned long long v = __shfl_xor_sync(0xffffffffu, k, o);
+        k = v > k ? v : k;
+    }
+    return k;
+}
 #endif
 
 }  // namespace lb

@@ -383,8 +383,9 @@ __global__ void rs_detect_kernel(const uint32_t *__restrict__ bins0, const float
     n_cands[s] = rs_detect_stream(b, m, n, p, cands + (size_t)s * cap, cap, dropped + s);
 }
 
-// the windows of one candidate, block-collective (all threads call every member with the same arguments)
-template <int SF>
+// the windows of one candidate, block-collective (all threads call every member with the same arguments); D = sps / N is
+// argmax's only use of the sample rate (binval and energy take sps at run time)
+template <int SF, int D = 8>
 struct RsDevOps {
     const float2 *x;                   // the row
     long long n_items;
@@ -394,19 +395,19 @@ struct RsDevOps {
     RxShared *sh;
     LB_D bool in_range(long long pos) const { return pos >= 0 && pos + (long long)sps <= n_items; }
     LB_D unsigned long long argmax(long long pos, bool use_up) {
-        using C = K1Cfg<SF>;
+        using C = K1Cfg<SF, D>;
         const int tid = threadIdx.x;
         K1Args a{x + pos, use_up ? up : down, tw, 1};
         unsigned long long best = 0ull;
         float2 wtab[C::NP / C::TPS];
-        k1_combine_twiddles<SF>(a, tid, wtab);
+        k1_combine_twiddles<SF, D>(a, tid, wtab);
         for (int s = 0; s < C::S; s++) {
-            k1_pass0<SF, false>(a, 0, s, tid, smem);
+            k1_pass0<SF, false, D>(a, 0, s, tid, smem);
             __syncthreads();
-            k1_pass<SF, C::R1, C::SIG1>(a, tid, smem);
+            k1_pass<SF, C::R1, C::SIG1, D>(a, tid, smem);
             __syncthreads();
-            if (C::R2 > 1) { k1_pass<SF, (C::R2 > 1 ? C::R2 : 2), 1>(a, tid, smem); __syncthreads(); }
-            const unsigned long long k = tid < C::TPS ? k1_combine<SF>(a, s, tid, smem, wtab) : 0ull;
+            if (C::R2 > 1) { k1_pass<SF, (C::R2 > 1 ? C::R2 : 2), 1, D>(a, tid, smem); __syncthreads(); }
+            const unsigned long long k = tid < C::TPS ? k1_combine<SF, D>(a, s, tid, smem, wtab) : 0ull;
             best = k > best ? k : best;
             __syncthreads();
         }
@@ -440,7 +441,7 @@ struct RsDevOps {
 };
 
 // synchronise: one CTA per candidate slot (stream = slot / cap); synchronised frames are appended to `frames`
-template <int SF, bool DRIFT>
+template <int SF, int D, bool DRIFT>
 __global__ void __launch_bounds__(RX_THREADS)
 rs_sync_kernel(const float2 *__restrict__ iq, size_t stride, size_t n_items, const float2 *down, const float2 *up, const float2 *tw,
                RsParams p, const RsCand *__restrict__ cands, const uint32_t *__restrict__ n_cands, uint32_t cap,
@@ -451,7 +452,7 @@ rs_sync_kernel(const float2 *__restrict__ iq, size_t stride, size_t n_items, con
     const uint32_t s = blockIdx.x / cap, i = blockIdx.x % cap;
     const uint32_t nc = n_cands[s];
     if (i >= (nc < cap ? nc : cap)) return;
-    RsDevOps<SF> ops{iq + (size_t)s * stride, (long long)n_items, down, up, tw, p.sps, rs_dyn_smem, &sh};
+    RsDevOps<SF, D> ops{iq + (size_t)s * stride, (long long)n_items, down, up, tw, p.sps, rs_dyn_smem, &sh};
     const RsFrame r = rs_synchronise<DRIFT>(ops, cands[(size_t)s * cap + i], p, s);
     if (threadIdx.x == 0) {
         if (r.status == RS_INCOMPLETE) atomicMin(hold + s, (unsigned long long)(r.start > 0 ? r.start : 0));

@@ -119,7 +119,9 @@ int lora_b200_tables_commit(lora_b200_decoder *d);
  * iq: n_symbols * sps interleaved cf32.  bins[i] in [0, N), mags[i] = |tmp[bin]| (may be NULL).
  * _dev: all pointers are device pointers, the launch is asynchronous on `cuda_stream`
  * (a cudaStream_t passed as void*, NULL = default stream).
- * _host: host pointers; copies (pinned, chunked, overlapped with compute) are inside. */
+ * _host: host pointers; copies (pinned, chunked, overlapped with compute) are inside.
+ * samp_rate / bandwidth 8 (the tuned kernels of each SF) or 2 (one kernel generic in the oversampling factor), SF7..SF12;
+ * otherwise LORA_B200_EUNSUPPORTED. */
 int lora_b200_demod_fft_dev(lora_b200_decoder *d, const void *iq, size_t n_symbols,
                             uint32_t *bins, float *mags, void *cuda_stream);
 int lora_b200_demod_fft_host(lora_b200_decoder *d, const void *iq, size_t n_symbols,
@@ -129,7 +131,7 @@ int lora_b200_demod_fft_host(lora_b200_decoder *d, const void *iq, size_t n_symb
  * (> 0: bit 0), j < ppm.  The demodulated word of bin k is the receiver's: gray((k - 1) mod N), with (k - 1) mod N first
  * folded to N / 4 bins as reduced-rate symbols are (reduced = 1, ppm = SF - 2; reduced = 0: ppm = SF).  bins (may be NULL)
  * = lora_b200_demod_fft_dev's argmax of the same computation.  iq 16-byte aligned; device pointers, async on cuda_stream.
- * LORA_B200_EUNSUPPORTED unless samp_rate / bandwidth == 8 and SF7..SF12. */
+ * LORA_B200_EUNSUPPORTED unless samp_rate / bandwidth is 8 or 2 and SF7..SF12. */
 int lora_b200_demod_llr_dev(lora_b200_decoder *d, const void *iq, size_t n_symbols, int reduced, float *llrs, uint32_t *bins,
                             void *cuda_stream);
 /* The window sums the dechirp receiver's synchroniser (lora_b200_receive) measures, on their own, to check them against a
@@ -267,7 +269,8 @@ size_t lora_b200_frames_last(lora_b200_decoder *d, const lora_b200_frame **frame
  * checked.  Data windows are de-rotated by the frame's CFO and demodulated by the K1 batch kernels; the FFT demodulator's
  * (bin - 1) mod N mapping and the stream path's integer chain follow.  Explicit headers whose 5-bit checksum fails are dropped
  * (and counted); the payload CRC is not checked.  Implicit headers carry implicit_len payload bytes (0 with an implicit-header
- * decoder: LORA_B200_EINVAL).  Needs the FFT kernels (samp_rate / bandwidth == 8, SF7..SF12), else LORA_B200_EUNSUPPORTED.
+ * decoder: LORA_B200_EINVAL).  Needs the FFT kernels (samp_rate / bandwidth == 8 or 2, SF7..SF12), else LORA_B200_EUNSUPPORTED;
+ * at 2 (e.g. 500 kHz channels at 1 MS/s, or a channelizer's output at 2 samples per chip) timing is refined to +-1 sample.
  * Clock offset: a transmitter whose clock is off by delta = ppm * 1e-6 (delta > 0: fast against the receiver) sends TX symbol
  * position j (0..7 preamble, 8, 9 sync word, 10..12.25 SFD, 12.25 + k data symbol k) at receiver sample
  * start + llround(j * sps / (1 + delta)); every window of a frame is placed by this rule.  A frame's delta is

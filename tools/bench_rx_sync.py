@@ -12,7 +12,10 @@ about 36 puts the CFO beyond BW/4.
 With --soft every capture is decoded with hard and with soft decisions (lora_b200_rx_params.soft), alternating; each SF's
 points gain two SNRs 1.5 and 3 dB below its lowest, and the stages gain the soft-decision kernels (LLR demodulator time is
 part of assemble + K1).
-Usage: python tools/bench_rx_sync.py [--quick] [--ppm P | --soft]"""
+With --osr 2 the sensitivity curve is measured at fs/bw = 2 (250 kS/s, the generic K1 and LLR kernels at D = 2), and the
+real-time shape is decoded at fs/bw = 8 and at fs/bw = 2 (the same payloads, CFOs and layout, synthesised at each rate),
+alternating call by call; its results carry the suffix _osr8 / _osr2.
+Usage: python tools/bench_rx_sync.py [--quick] [--ppm P | --soft] [--osr 2]"""
 from __future__ import annotations
 
 import argparse
@@ -35,9 +38,17 @@ def sigma_for(snr_db):
     return float(np.sqrt(10 ** (-(snr_db - 10 * np.log10(FS / BW)) / 10) / 2))
 
 
+def set_osr(osr):
+    """fs = osr * BW for every capture and decoder made after the call"""
+    global FS
+    FS = float(osr * BW)
+
+
 def dec(sf, rr, **kw):
     import gr_lora_b200 as G
-    return G.decoder(FS, BW, sf, False, 4, True, rr, quiet=True, demod="fft", **kw)
+    if FS == 8 * BW:                                 # (the stream state machine's FFT demodulator exists at fs/bw = 8 only)
+        kw["demod"] = "fft"
+    return G.decoder(FS, BW, sf, False, 4, True, rr, quiet=True, **kw)
 
 
 def capture(torch, sf, n_streams, per_stream, snr, seed, n_items=None, plen=10, ppm=0.0):
@@ -45,7 +56,7 @@ def capture(torch, sf, n_streams, per_stream, snr, seed, n_items=None, plen=10, 
     from gr_lora_b200 import tx
     rr = sf >= 11
     rng = np.random.default_rng(seed)
-    sps = 8 << sf
+    sps = int(FS / BW) << sf
     flen = (12 + G.tx_frame_symbols(plen, sf, 4, False, True, rr)) * sps + sps // 4
     if n_items is None:
         n_items = per_stream * (flen + 5 * sps) + 8 * sps
@@ -57,7 +68,7 @@ def capture(torch, sf, n_streams, per_stream, snr, seed, n_items=None, plen=10, 
         cfo = [[e * CARRIER * 1e-6 for e in es] for es in sfo]
         kw["sfo_ppm"] = sfo
     gen = dec(sf, rr)
-    up = torch.from_numpy(tx.base_upchirp(sf).astype(np.complex64)).cuda()
+    up = torch.from_numpy(tx.base_upchirp(sf, BW, FS).astype(np.complex64)).cuda()
     out, placed = gen.synth_streams(pays, n_items, lead_symbols=float(rng.uniform(1, 3)), gap_symbols=4.3, cfo_hz=cfo,
                                     noise_sigma=sigma_for(snr), seed=seed, up_table_dev=up, **kw)
     torch.cuda.synchronize()
@@ -77,8 +88,8 @@ def genie_ser(torch, sf, snr, n=2048, seed=1):
     d = dec(sf, False)
     rng = np.random.default_rng(seed)
     vals = torch.from_numpy(rng.integers(0, 1 << sf, n).astype(np.int32)).cuda()
-    x = torch.empty(n * (8 << sf), dtype=torch.complex64, device="cuda")
-    up = torch.from_numpy(tx.base_upchirp(sf).astype(np.complex64)).cuda()
+    x = torch.empty(n * (int(FS / BW) << sf), dtype=torch.complex64, device="cuda")
+    up = torch.from_numpy(tx.base_upchirp(sf, BW, FS).astype(np.complex64)).cuda()
     d.tx_symbols(vals, x, n, noise_sigma=sigma_for(snr), seed=seed, up_table_dev=up)
     bins = torch.empty(n, dtype=torch.int32, device="cuda")
     d.demod_fft(x, n, bins)
@@ -124,7 +135,10 @@ def main():
     ap.add_argument("--ppm", type=float, default=0.0, help="per-frame crystal offset uniform in +-PPM at 868.1 MHz (0: none)")
     ap.add_argument("--soft", action="store_true", help="decode every capture with hard and with soft decisions, alternating, "
                     "at two more SNRs 1.5 and 3 dB below each SF's lowest point")
+    ap.add_argument("--osr", type=int, default=8, choices=(8, 2), help="fs/bw of the sensitivity curve; 2 also times the "
+                    "real-time shape at fs/bw = 8 against fs/bw = 2")
     a = ap.parse_args()
+    set_osr(a.osr)
     if a.soft and a.ppm:
         raise SystemExit("--soft and --ppm each compare two modes: give one of them")
     if abs(a.ppm) * CARRIER * 1e-6 > BW / 4:
@@ -146,6 +160,8 @@ def main():
     modes = ({"tracked": dict(carrier_hz=CARRIER), "fixed": dict(carrier_hz=0.0)} if a.ppm else
              {"hard": dict(soft=False), "soft": dict(soft=True)} if a.soft else {"": {}})
     res["soft"] = a.soft
+    if a.osr != 8:
+        res["osr"] = a.osr
     curve = {}
     for sf, pts in POINTS.items():
         rr = sf >= 11
@@ -171,25 +187,35 @@ def main():
             row.append(pt)
         curve[f"sf{sf}"] = row
     res["sensitivity"] = curve
-    # config-4 shape: 384 SF7 streams x 2 s, frames 3 dB above the sensitivity point
-    out, placed, n_items = capture(torch, 7, 384, 40, 1.0, seed=4, n_items=2_000_000, ppm=a.ppm)
-    rx = dec(7, False, n_streams=384, max_items_per_call=n_items, max_frames_per_call=64)
-    for m, kw in modes.items():
-        runs = [stages(torch, rx, out, n_items, **kw) for _ in range(a.repeats)]
-        res["stages_ms" + (m and "_" + m)] = {k: {"median": float(np.median([r[k] for r in runs])), "min": min(r[k] for r in runs),
-                                                  "max": max(r[k] for r in runs)} for k in runs[0]}
-    times = {m: [] for m in modes}
-    for _ in range(a.repeats):                       # the modes alternate, so that both see the same conditions
+    # config-4 shape: 384 SF7 streams x 2 s, frames 3 dB above the sensitivity point; with --osr 2 the same frames at both
+    # rates, the calls alternating between them
+    rates = [8, 2] if a.osr != 8 else [8]
+    sfx = (lambda d: f"_osr{d}") if a.osr != 8 else (lambda d: "")
+    shape = {}
+    for d in rates:
+        set_osr(d)
+        out, placed, n_items = capture(torch, 7, 384, 40, 1.0, seed=4, n_items=int(2 * FS), ppm=a.ppm)
+        rx = dec(7, False, n_streams=384, max_items_per_call=n_items, max_frames_per_call=64)
+        shape[d] = (out, placed, n_items, rx, FS)
         for m, kw in modes.items():
-            torch.cuda.synchronize()
-            t0 = time.perf_counter()
-            _, frames, _ = rx.receive(out, n_items=n_items, **kw)
-            times[m].append(time.perf_counter() - t0)
-            med = float(np.median(times[m]))
-            res["realtime" + (m and "_" + m)] = {
-                "streams": 384, "seconds_per_stream": n_items / FS, "frames_placed": len(placed),
-                "frames_decoded": decoded(frames, placed), "call_s_median": round(med, 4), "call_s_min": round(min(times[m]), 4),
-                "call_s_max": round(max(times[m]), 4), "realtime_factor": round(384 * n_items / FS / med, 1)}
+            runs = [stages(torch, rx, out, n_items, **kw) for _ in range(a.repeats)]
+            res["stages_ms" + (m and "_" + m) + sfx(d)] = {
+                k: {"median": float(np.median([r[k] for r in runs])), "min": min(r[k] for r in runs), "max": max(r[k] for r in runs)}
+                for k in runs[0]}
+    times = {(m, d): [] for m in modes for d in rates}
+    for _ in range(a.repeats):                       # the modes (and rates) alternate, so that all see the same conditions
+        for d in rates:
+            out, placed, n_items, rx, fs = shape[d]
+            for m, kw in modes.items():
+                torch.cuda.synchronize()
+                t0 = time.perf_counter()
+                _, frames, _ = rx.receive(out, n_items=n_items, **kw)
+                times[m, d].append(time.perf_counter() - t0)
+                med = float(np.median(times[m, d]))
+                res["realtime" + (m and "_" + m) + sfx(d)] = {
+                    "streams": 384, "seconds_per_stream": n_items / fs, "frames_placed": len(placed),
+                    "frames_decoded": decoded(frames, placed), "call_s_median": round(med, 4), "call_s_min": round(min(times[m, d]), 4),
+                    "call_s_max": round(max(times[m, d]), 4), "realtime_factor": round(384 * n_items / fs / med, 1)}
     print(json.dumps(res))
 
 
