@@ -327,9 +327,13 @@ int lora_b200_stream_state(lora_b200_decoder *d, uint32_t stream);
 int lora_b200_set_cfo_estimate(lora_b200_decoder *d, int enable);
 int lora_b200_last_cfo(lora_b200_decoder *d, uint32_t stream, float *cfo_hz, uint32_t *count);
 /* the reference's std::cout hex lines for the frames delivered by the last work call of this
- * stream (" 04 90 40" + " de ad ... (ascii)\n", decoder_impl.cc:832,872) */
+ * stream (" 04 90 40" + " de ad ... (ascii)\n", decoder_impl.cc:832,872).  A frame's header bytes are delivered together
+ * with its payload line, by the call in which the frame completes; the reference prints them as soon as the header block
+ * is decoded, so input that ends inside a frame leaves it one unterminated header print ahead. */
 int lora_b200_stdout_last(lora_b200_decoder *d, uint32_t stream, char *buf, size_t cap);
-/* per-step trace of the last work call (needs trace_capacity > 0) */
+/* per-step trace of the last work call (needs trace_capacity > 0): *n = the number of steps the stream made in that call,
+ * steps[0 .. min(*n, trace_capacity, cap)) = the FIRST of them (later steps are not recorded).  LORA_B200_EOVERFLOW when
+ * *n > trace_capacity (steps[] and *n are valid), LORA_B200_EINVAL without a trace. */
 int lora_b200_trace_read(lora_b200_decoder *d, uint32_t stream, lora_b200_step *steps, size_t cap, size_t *n);
 
 /* ---- N1 (SURVEY.md 8f): the channelizer in front of the decoder -------------------------------------

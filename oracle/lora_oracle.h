@@ -63,7 +63,7 @@ typedef struct {
     int32_t consumed;    /* items passed to consume_each                      */
     int32_t bin;         /* raw demod bin (before /4 and Gray), -1 if none    */
     int32_t fine_sync;   /* d_fine_sync at exit                               */
-    float   metric;      /* autocorr (DETECT), pearson c (FIND_SFD), else 0   */
+    float   metric;      /* autocorr (DETECT), max correlation (SYNC), pearson c (FIND_SFD), else 0 */
 } lo_step;
 
 /* lifecycle: mirrors decoder::make (include/lora/decoder.h:705, lib/decoder_impl.cc:41-122).
