@@ -64,6 +64,7 @@ SIGNATURES = {
     "lora_b200_demod_fft_dev": (_i, [_vp, _vp, _sz, _vp, _vp, _vp]),
     "lora_b200_demod_fft_host": (_i, [_vp, _vp, _sz, _vp, _vp]),
     "lora_b200_demod_llr_dev": (_i, [_vp, _vp, _sz, _i, _vp, _vp, _vp]),
+    "lora_b200_demod_fft_antennas_dev": (_i, [_vp, _vp, _u32, _u32, _sz, _sz, _vp, _vp, _vp]),
     "lora_b200_rs_window_dev": (_i, [_vp, _vp, _sz, _sz, _vp, _vp, _vp, _vp, _vp, _vp]),
     "lora_b200_demod_fft_host_sc16": (_i, [_vp, _vp, C.c_float, _sz, _vp, _vp]),
     "lora_b200_demod_gradient_dev": (_i, [_vp, _vp, _sz, _vp, _vp]),
@@ -84,6 +85,8 @@ SIGNATURES = {
     "lora_b200_frames_last": (_sz, [_vp, C.POINTER(_vp)]),
     "lora_b200_receive": (_i, [_vp, _vp, _sz, _sz, _i, C.POINTER(RxParams), C.POINTER(_sz)]),
     "lora_b200_rx_info_last": (_sz, [_vp, C.POINTER(_vp), C.POINTER(C.c_uint32)]),
+    "lora_b200_receive_antennas": (_i, [_vp, _vp, _sz, _sz, _i, _u32, C.POINTER(RxParams), C.POINTER(_sz)]),
+    "lora_b200_rx_channels_last": (_sz, [_vp, C.POINTER(_vp), C.POINTER(C.c_uint32)]),
     "lora_b200_stream_state": (_i, [_vp, _u32]),
     "lora_b200_reset": (_i, [_vp]),
     "lora_b200_set_cfo_estimate": (_i, [_vp, _i]),

@@ -75,6 +75,13 @@ class channelizer:
         p = self._L.lora_b200_channelizer_output(self._h, int(channel), C.byref(stride))
         return int(p or 0), int(stride.value)
 
+    def read_output(self, channel=0, n_items=None) -> np.ndarray:
+        """One channel's output of the last work() call, copied to a host array."""
+        n = self.n_out if n_items is None else int(n_items)
+        out = np.empty(n, np.complex64)
+        self._check(self._L.lora_b200_channelizer_read_output(self._h, int(channel), out.ctypes.data, n), "channelizer_read_output")
+        return out
+
     def work_dev(self, in_dev, n_in, out_dev, out_stride, cuda_stream=0) -> int:
         n = C.c_size_t(0)
         ptr = lambda t: int(t.data_ptr()) if hasattr(t, "data_ptr") else int(t)

@@ -56,6 +56,30 @@ int lb_k1_emulate_osr(int sf, int osr, const float2 *x, size_t n_symbols, const 
     return osr == 8 ? k1_emulate_d<8>(sf, a, bins, mags) : osr == 2 ? k1_emulate_d<2>(sf, a, bins, mags) : -1;
 }
 
+// k1_antennas_kernel<SF, D> on the host for one group: m rows of n_symbols windows, row_stride samples apart -> the argmax
+// of the combined spectrum sum_a |tmp_a|^2 and its sqrt; -1 for another SF or D
+int lb_k1_antennas_emulate_osr(int sf, int osr, const float2 *x, size_t row_stride, uint32_t m, size_t n_symbols, const float2 *chirp,
+                               const float2 *tw, uint32_t *bins, float *mags) {
+    const lb::K1Args a{x, chirp, tw, n_symbols};
+    if (osr != 8 && osr != 2) return -1;
+    switch (sf * 16 + osr) {
+    case 7 * 16 + 8: lb::k1_antennas_emulate<7, 8>(a, row_stride, m, bins, mags); break;
+    case 8 * 16 + 8: lb::k1_antennas_emulate<8, 8>(a, row_stride, m, bins, mags); break;
+    case 9 * 16 + 8: lb::k1_antennas_emulate<9, 8>(a, row_stride, m, bins, mags); break;
+    case 10 * 16 + 8: lb::k1_antennas_emulate<10, 8>(a, row_stride, m, bins, mags); break;
+    case 11 * 16 + 8: lb::k1_antennas_emulate<11, 8>(a, row_stride, m, bins, mags); break;
+    case 12 * 16 + 8: lb::k1_antennas_emulate<12, 8>(a, row_stride, m, bins, mags); break;
+    case 7 * 16 + 2: lb::k1_antennas_emulate<7, 2>(a, row_stride, m, bins, mags); break;
+    case 8 * 16 + 2: lb::k1_antennas_emulate<8, 2>(a, row_stride, m, bins, mags); break;
+    case 9 * 16 + 2: lb::k1_antennas_emulate<9, 2>(a, row_stride, m, bins, mags); break;
+    case 10 * 16 + 2: lb::k1_antennas_emulate<10, 2>(a, row_stride, m, bins, mags); break;
+    case 11 * 16 + 2: lb::k1_antennas_emulate<11, 2>(a, row_stride, m, bins, mags); break;
+    case 12 * 16 + 2: lb::k1_antennas_emulate<12, 2>(a, row_stride, m, bins, mags); break;
+    default: return -1;
+    }
+    return 0;
+}
+
 int lb_k1_emulate(int sf, const float2 *x, size_t n_symbols, const float2 *chirp, const float2 *tw,
                   uint32_t *bins, float *mags) {
     return lb_k1_emulate_osr(sf, 8, x, n_symbols, chirp, tw, bins, mags);
@@ -193,11 +217,13 @@ namespace {
 
 // the windows of rs_synchronise on the host: K1 through its CPU emulation, the bin sums as plain loops in double
 struct RsHostOps {
+    static constexpr int M = 1;
     const float2 *x;
     long long n_items;
     const float2 *down, *up, *tw;
     uint32_t sps, sf, osr;
     bool in_range(long long pos) const { return pos >= 0 && pos + (long long)sps <= n_items; }
+    void binvals(long long pos, float F, bool use_up, int bin, float2 *v) { v[0] = binval(pos, F, use_up, bin); }
     unsigned long long argmax(long long pos, bool use_up) {
         uint32_t b;
         float m;
@@ -219,6 +245,33 @@ struct RsHostOps {
         double e = 0.0;
         for (uint32_t n = 0; n < sps; n++) e += (double)x[pos + n].x * x[pos + n].x + (double)x[pos + n].y * x[pos + n].y;
         return (float)e;
+    }
+};
+
+// ... of a receiver with m antennas, rows one.x + a * one.n_items: the combined K1 argmax through k1_antennas_emulate
+struct RsHostAntOps {
+    static constexpr int M = lb::RS_MAX_ANTENNAS;
+    RsHostOps one;
+    uint32_t m;
+    bool in_range(long long pos) const { return one.in_range(pos); }
+    RsHostOps row(uint32_t a) const { RsHostOps o = one; o.x = one.x + (size_t)a * one.n_items; return o; }
+    unsigned long long argmax(long long pos, bool use_up) {
+        uint32_t b;
+        float mg;
+        lb_k1_antennas_emulate_osr((int)one.sf, (int)one.osr, one.x + pos, (size_t)one.n_items, m, 1, use_up ? one.up : one.down, one.tw, &b, &mg);
+        return lb::pack_key(mg * mg, b);
+    }
+    void binvals(long long pos, float F, bool use_up, int bin, float2 *v) {
+        for (uint32_t a = 0; a < (uint32_t)M; a++) v[a] = a < m ? row(a).binval(pos, F, use_up, bin) : make_float2(0.f, 0.f);
+    }
+    void energies(long long pos, float *e) {
+        for (uint32_t a = 0; a < (uint32_t)M; a++) e[a] = a < m ? row(a).energy(pos) : 0.f;
+    }
+    float energy(long long pos) {
+        float e[M], s = 0.f;
+        energies(pos, e);
+        for (int a = 0; a < M; a++) s += e[a];
+        return s;
     }
 };
 
@@ -252,6 +305,95 @@ void rs_host_llrs(const RsHostOps &o, const lb::RsFrame &r, uint32_t first, uint
     lb_k1_llr_emulate_osr((int)o.sf, (int)o.osr, w.data(), cnt, o.down, o.tw, reduced, llr.data(), nullptr);
 }
 
+// the receive path of lb_emul_rx_receive_osr (m = 1) and lb_emul_rx_receive_antennas (m rows of n_items each, x[a * n_items
+// ..]); with several antennas chan[f * m ..] gets each synchronised frame's channel estimates h (may be NULL)
+uint32_t rs_host_receive(const float2 *x, size_t n_items, uint32_t m, const float2 *down, const float2 *up, const float2 *tw, uint32_t sf,
+                         uint32_t osr, uint32_t cr, int implicit, int crc, int reduced_rate, uint32_t sync_word, uint32_t implicit_len,
+                         uint32_t min_preamble, float sfo_ppm, double carrier_hz, int soft, long long *start, float *cfo_bins,
+                         float *snr_db, int32_t *status, float *sfo, uint8_t *payload, uint32_t *len, float2 *chan, uint32_t cap) {
+    if (osr != 8u && osr != 2u) return 0;
+    const uint32_t N = 1u << sf, sps = osr * N;
+    const double bin_hz = 125e3 / N;
+    lb::RsParams p{sps, N, osr, sfo_ppm, min_preamble ? min_preamble : 5u, {((sync_word >> 4) & 15u) * 8u % N, (sync_word & 15u) * 8u % N},
+                   (float)N / 4.0f, carrier_hz > 0.0 ? (float)(1e6 * bin_hz / carrier_hz) : 0.0f};
+    RsHostOps o{x, (long long)n_items, down, up, tw, sps, sf, osr};
+    RsHostAntOps oa{o, m};
+    // screen
+    std::vector<uint32_t> bins[2];
+    std::vector<float> mags[2];
+    uint32_t n[2];
+    for (int ph = 0; ph < 2; ph++) {
+        n[ph] = n_items >= sps + ph * sps / 2 ? (uint32_t)((n_items - ph * sps / 2) / sps) : 0u;
+        bins[ph].resize(n[ph] + 1);
+        mags[ph].resize(n[ph] + 1);
+        if (n[ph] && m == 1) lb_k1_emulate_osr((int)sf, (int)osr, x + ph * sps / 2, n[ph], down, tw, bins[ph].data(), mags[ph].data());
+        else if (n[ph]) lb_k1_antennas_emulate_osr((int)sf, (int)osr, x + ph * sps / 2, n_items, m, n[ph], down, tw, bins[ph].data(), mags[ph].data());
+    }
+    const uint32_t *bp[2] = {bins[0].data(), bins[1].data()};
+    const float *mp[2] = {mags[0].data(), mags[1].data()};
+    std::vector<lb::RsCand> cands(64);
+    long long dropped;
+    const uint32_t nc = std::min<uint32_t>(lb::rs_detect_stream(bp, mp, n, p, cands.data(), 64, &dropped), 64u);
+    lb::RxParams rp;
+    memset(&rp, 0, sizeof rp);
+    rp.sf = sf; rp.n_bins = N; rp.n_bins_hdr = N / 4; rp.sps = sps; rp.decim = osr; rp.implicit = implicit; rp.reduced_rate = reduced_rate;
+    const uint8_t phdr1 = (uint8_t)(((cr & 7u) << 5) | (crc ? 1u << 4 : 0u));
+    uint32_t nf = 0;
+    std::vector<float2> y;                            // several antennas: the combined row sum_a w_a x_a of one frame
+    for (uint32_t c = 0; c < nc && nf < cap; c++) {
+        const bool drift = lb::rs_drift(p);
+        lb::RsFrame r = m == 1 ? (drift ? lb::rs_synchronise<true>(o, cands[c], p, 0) : lb::rs_synchronise<false>(o, cands[c], p, 0))
+                               : (drift ? lb::rs_synchronise<true>(oa, cands[c], p, 0) : lb::rs_synchronise<false>(oa, cands[c], p, 0));
+        if (r.status == lb::RS_REJECT) continue;
+        RsHostOps od = o;                             // the row the data windows are read from
+        if (m > 1 && r.status == lb::RS_OK) {
+            float2 h[lb::RS_MAX_ANTENNAS], w[lb::RS_MAX_ANTENNAS];
+            r.snr_db = drift ? lb::rs_channels<true>(oa, p, r, m, h, w) : lb::rs_channels<false>(oa, p, r, m, h, w);
+            if (chan)
+                for (uint32_t a = 0; a < m; a++) chan[(size_t)nf * m + a] = h[a];
+            y.assign(n_items, make_float2(0.f, 0.f));
+            for (size_t i = 0; i < n_items; i++)
+                for (uint32_t a = 0; a < m; a++) y[i] = lb::cfma(w[a], x[(size_t)a * n_items + i], y[i]);
+            od.x = y.data();
+        }
+        start[nf] = r.start; cfo_bins[nf] = r.cfo_bins; snr_db[nf] = r.snr_db; status[nf] = 2; len[nf] = 0;
+        if (sfo) sfo[nf] = r.sfo_ppm;
+        // end of the window of data symbol n - 1
+        auto data_end = [&](long long n) { return lb::rs_sym(r.start, lb::rs_data_j(n - 1), sps, r.sfo_ppm) + (long long)sps; };
+        if (r.status == lb::RS_OK && data_end(8) <= (long long)n_items) {
+            std::vector<uint32_t> hb, pb;
+            std::vector<float> llr;
+            if (soft) {
+                hb.resize(8);
+                rs_host_llrs(od, r, 0, 8, true, llr);
+                lb::rs_soft_header(lb::rs_code(rp, phdr1), llr.data(), hb.data(), nullptr);
+            } else {
+                rs_host_bins(od, r, 0, 8, hb);
+            }
+            lb::RxStreamState st;
+            const int32_t np = lb::rs_header(&st, rp, phdr1, hb.data(), implicit_len);
+            if (np < 0) status[nf] = 1;
+            else if (data_end(8ll + np) <= (long long)n_items) {
+                if (soft) {
+                    pb.resize((size_t)np);
+                    rs_host_llrs(od, r, 8, (uint32_t)np, reduced_rate != 0, llr);
+                    lb::rs_soft_payload(rp, phdr1, hb.data(), np, implicit_len, llr.data(), pb.data());
+                } else {
+                    rs_host_bins(od, r, 8, (uint32_t)np, pb);
+                }
+                lb::RxFrameRec fr;
+                lb::rs_frame(&st, rp, pb.data(), np, &fr, 0, nf, 1.0f);
+                const uint32_t nd = lb::decode_len_bytes(lb::decode_len_words(fr.n_cw, 0), fr.cr);
+                len[nf] = std::min<uint32_t>(fr.payload_length, 256u);
+                for (uint32_t i = 0; i < len[nf]; i++) payload[(size_t)nf * 256 + i] = i < nd ? lb::decode_byte(fr.cw, fr.n_cw, 0, fr.cr, i) : 0;
+                status[nf] = 0;
+            }
+        }
+        nf++;
+    }
+    return nf;
+}
+
 }  // namespace
 
 extern "C" {
@@ -268,71 +410,22 @@ uint32_t lb_emul_rx_receive_osr(const float2 *x, size_t n_items, const float2 *d
                                 uint32_t implicit_len, uint32_t min_preamble, float sfo_ppm, double carrier_hz, int soft,
                                 long long *start, float *cfo_bins, float *snr_db, int32_t *status, float *sfo, uint8_t *payload,
                                 uint32_t *len, uint32_t cap) {
-    if (osr != 8u && osr != 2u) return 0;
-    const uint32_t N = 1u << sf, sps = osr * N;
-    const double bin_hz = 125e3 / N;
-    lb::RsParams p{sps, N, osr, sfo_ppm, min_preamble ? min_preamble : 5u, {((sync_word >> 4) & 15u) * 8u % N, (sync_word & 15u) * 8u % N},
-                   (float)N / 4.0f, carrier_hz > 0.0 ? (float)(1e6 * bin_hz / carrier_hz) : 0.0f};
-    RsHostOps o{x, (long long)n_items, down, up, tw, sps, sf, osr};
-    // screen
-    std::vector<uint32_t> bins[2];
-    std::vector<float> mags[2];
-    uint32_t n[2];
-    for (int ph = 0; ph < 2; ph++) {
-        n[ph] = n_items >= sps + ph * sps / 2 ? (uint32_t)((n_items - ph * sps / 2) / sps) : 0u;
-        bins[ph].resize(n[ph] + 1);
-        mags[ph].resize(n[ph] + 1);
-        if (n[ph]) lb_k1_emulate_osr((int)sf, (int)osr, x + ph * sps / 2, n[ph], down, tw, bins[ph].data(), mags[ph].data());
-    }
-    const uint32_t *bp[2] = {bins[0].data(), bins[1].data()};
-    const float *mp[2] = {mags[0].data(), mags[1].data()};
-    std::vector<lb::RsCand> cands(64);
-    long long dropped;
-    const uint32_t nc = std::min<uint32_t>(lb::rs_detect_stream(bp, mp, n, p, cands.data(), 64, &dropped), 64u);
-    lb::RxParams rp;
-    memset(&rp, 0, sizeof rp);
-    rp.sf = sf; rp.n_bins = N; rp.n_bins_hdr = N / 4; rp.sps = sps; rp.decim = osr; rp.implicit = implicit; rp.reduced_rate = reduced_rate;
-    const uint8_t phdr1 = (uint8_t)(((cr & 7u) << 5) | (crc ? 1u << 4 : 0u));
-    uint32_t nf = 0;
-    for (uint32_t c = 0; c < nc && nf < cap; c++) {
-        const lb::RsFrame r = lb::rs_drift(p) ? lb::rs_synchronise<true>(o, cands[c], p, 0) : lb::rs_synchronise<false>(o, cands[c], p, 0);
-        if (r.status == lb::RS_REJECT) continue;
-        start[nf] = r.start; cfo_bins[nf] = r.cfo_bins; snr_db[nf] = r.snr_db; status[nf] = 2; len[nf] = 0;
-        if (sfo) sfo[nf] = r.sfo_ppm;
-        // end of the window of data symbol n - 1
-        auto data_end = [&](long long n) { return lb::rs_sym(r.start, lb::rs_data_j(n - 1), sps, r.sfo_ppm) + (long long)sps; };
-        if (r.status == lb::RS_OK && data_end(8) <= (long long)n_items) {
-            std::vector<uint32_t> hb, pb;
-            std::vector<float> llr;
-            if (soft) {
-                hb.resize(8);
-                rs_host_llrs(o, r, 0, 8, true, llr);
-                lb::rs_soft_header(lb::rs_code(rp, phdr1), llr.data(), hb.data(), nullptr);
-            } else {
-                rs_host_bins(o, r, 0, 8, hb);
-            }
-            lb::RxStreamState st;
-            const int32_t np = lb::rs_header(&st, rp, phdr1, hb.data(), implicit_len);
-            if (np < 0) status[nf] = 1;
-            else if (data_end(8ll + np) <= (long long)n_items) {
-                if (soft) {
-                    pb.resize((size_t)np);
-                    rs_host_llrs(o, r, 8, (uint32_t)np, reduced_rate != 0, llr);
-                    lb::rs_soft_payload(rp, phdr1, hb.data(), np, implicit_len, llr.data(), pb.data());
-                } else {
-                    rs_host_bins(o, r, 8, (uint32_t)np, pb);
-                }
-                lb::RxFrameRec fr;
-                lb::rs_frame(&st, rp, pb.data(), np, &fr, 0, nf, 1.0f);
-                const uint32_t nd = lb::decode_len_bytes(lb::decode_len_words(fr.n_cw, 0), fr.cr);
-                len[nf] = std::min<uint32_t>(fr.payload_length, 256u);
-                for (uint32_t i = 0; i < len[nf]; i++) payload[(size_t)nf * 256 + i] = i < nd ? lb::decode_byte(fr.cw, fr.n_cw, 0, fr.cr, i) : 0;
-                status[nf] = 0;
-            }
-        }
-        nf++;
-    }
-    return nf;
+    return rs_host_receive(x, n_items, 1, down, up, tw, sf, osr, cr, implicit, crc, reduced_rate, sync_word, implicit_len, min_preamble,
+                           sfo_ppm, carrier_hz, soft, start, cfo_bins, snr_db, status, sfo, payload, len, nullptr, cap);
+}
+
+// ... of one receiver with m (1..4) antennas, x[a * n_items ..] antenna a's row (lora_b200_receive_antennas): the combined
+// screen, the synchroniser over all antennas, each frame's data windows sum_a w_a x_a (rs_channels); snr_db the combined
+// SNR, chan[f * m ..] (may be NULL) the channel estimates h of synchronised frame f.  m = 1 is lb_emul_rx_receive_osr;
+// another m returns 0 frames.
+uint32_t lb_emul_rx_receive_antennas(const float2 *x, size_t n_items, uint32_t m, const float2 *down, const float2 *up, const float2 *tw,
+                                     uint32_t sf, uint32_t osr, uint32_t cr, int implicit, int crc, int reduced_rate, uint32_t sync_word,
+                                     uint32_t implicit_len, uint32_t min_preamble, float sfo_ppm, double carrier_hz, int soft,
+                                     long long *start, float *cfo_bins, float *snr_db, int32_t *status, float *sfo, uint8_t *payload,
+                                     uint32_t *len, float *chan, uint32_t cap) {
+    if (m < 1 || m > (uint32_t)lb::RS_MAX_ANTENNAS) return 0;
+    return rs_host_receive(x, n_items, m, down, up, tw, sf, osr, cr, implicit, crc, reduced_rate, sync_word, implicit_len, min_preamble,
+                           sfo_ppm, carrier_hz, soft, start, cfo_bins, snr_db, status, sfo, payload, len, (float2 *)chan, cap);
 }
 
 // lb_emul_rx_receive_osr at fs/bw = 8 (fs = 1 MHz)

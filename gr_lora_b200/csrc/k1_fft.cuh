@@ -261,6 +261,104 @@ LB_HD unsigned long long k1_combine(const K1Args &a, int s, int tid, const float
     return best;
 }
 
+// ---- several antennas: the combined spectrum P[k] = sum_a |tmp_a[k]|^2 of M windows ------------------------------------------
+// The combine phase of each antenna's window adds |.|^2 at the thread's NP/TPS positions into pw -- k1_combine's sum, the
+// same branch sums and quirk -- and once every antenna of sub-problem s is in, k1_power_key gives the first argmax of the
+// summed powers.  (k1_combine keeps its own copy of the sum: the single-antenna kernels compile exactly as before.)
+template <int SF, int D = 8>
+LB_HD void k1_combine_power(int s, int tid, const float2 *buf, const float2 *wtab, float *pw) {
+    using C = K1Cfg<SF, D>;
+    const int g = tid / C::TPS, lt = tid % C::TPS;
+    const float2 *bs = buf + g * C::SYM_STRIDE;
+#pragma unroll
+    for (int i = 0; i < C::NP / C::TPS; i++) {
+        const int p = lt + C::TPS * i;
+        const int q = k1_pos_to_bin<SF, D>(p);
+        const int pp = k1_pad(p);
+        float2 gv[D];
+#pragma unroll
+        for (int r = 0; r < D; r++) gv[r] = bs[r * C::SB + pp];
+        float2 acc = horner<D>(gv, wtab[i]);
+        if (s == 0 && q == C::NP / 2) acc = plus_quirk<D>(acc, gv, wtab[i]);
+        pw[i] += cnorm2(acc);
+    }
+}
+template <int SF, int D = 8>
+LB_HD unsigned long long k1_power_key(int s, int tid, const float *pw) {
+    using C = K1Cfg<SF, D>;
+    const int lt = tid % C::TPS;
+    unsigned long long best = 0ull;
+#pragma unroll
+    for (int i = 0; i < C::NP / C::TPS; i++) {
+        const int q = k1_pos_to_bin<SF, D>(lt + C::TPS * i);
+        const int kp = C::S * (q < C::NP / 2 ? q : q - C::NP) + s;
+        const unsigned long long key = pack_key(pw[i], (uint32_t)(kp >= 0 ? kp : C::N + kp));
+        best = key > best ? key : best;
+    }
+    return best;
+}
+
+#ifdef __CUDACC__
+// several antennas, one work item (group g, batch of G window positions) per CTA turn: for each sub-problem s the M windows
+// of every position go through pass 0 .. combine in turn and sum their |.|^2 per kept bin before the argmax.  bins / mags of
+// group g, position j at out[g * out_stride + j]; sqrt(P[bin]) is the magnitude.
+template <int SF, int D = 8>
+__global__ void __launch_bounds__(K1_THREADS, 2)
+k1_antennas_kernel(K1Args a /* x: group 0, antenna 0, position 0; n_symbols: positions per row */, size_t row_stride, uint32_t m,
+                   uint32_t n_groups, size_t out_stride, uint32_t *__restrict__ bins, float *__restrict__ mags) {
+    using C = K1Cfg<SF, D>;
+    constexpr int W_LOG = k1_log2(C::W);
+    extern __shared__ float2 k1_smem[];
+    __shared__ unsigned long long warp_best[K1_THREADS / C::W];
+    float2 *buf = k1_smem;
+    const int tid = threadIdx.x;
+    const size_t n_batches = (a.n_symbols + C::G - 1) / C::G;
+    const size_t n_work = n_batches * n_groups;
+    float2 wtab[C::NP / C::TPS];
+    k1_combine_twiddles<SF, D>(a, tid, wtab);
+    for (size_t w = blockIdx.x; w < n_work; w += gridDim.x) {
+        const size_t g = w / n_batches, batch = w % n_batches;
+        unsigned long long best = 0ull;
+        for (int s = 0; s < C::S; s++) {
+            float pw[C::NP / C::TPS];
+#pragma unroll
+            for (int i = 0; i < C::NP / C::TPS; i++) pw[i] = 0.f;
+            for (uint32_t ant = 0; ant < m; ant++) {
+                K1Args aa = a;
+                aa.x = a.x + (g * m + ant) * row_stride;
+                k1_pass0<SF, true, D>(aa, batch, s, tid, buf);
+                __syncthreads();
+                k1_pass<SF, C::R1, C::SIG1, D>(aa, tid, buf);
+                __syncthreads();
+                if (C::R2 > 1) {
+                    k1_pass<SF, (C::R2 > 1 ? C::R2 : 2), 1, D>(aa, tid, buf);
+                    __syncthreads();
+                }
+                k1_combine_power<SF, D>(s, tid, buf, wtab, pw);
+                __syncthreads();
+            }
+            const unsigned long long k = k1_power_key<SF, D>(s, tid, pw);
+            best = k > best ? k : best;
+        }
+        best = group_max_key<C::W>(best);
+        if ((tid & (C::W - 1)) == 0) warp_best[tid >> W_LOG] = best;
+        __syncthreads();
+        if (tid < C::G) {
+            constexpr int WPS = C::TPS / C::W;
+            unsigned long long bb = 0ull;
+#pragma unroll
+            for (int k = 0; k < WPS; k++) {
+                const unsigned long long o = warp_best[tid * WPS + k];
+                bb = o > bb ? o : bb;
+            }
+            const size_t sym = batch * C::G + tid;
+            if (sym < a.n_symbols) k1_store(bins, mags, g * out_stride + sym, bb);
+        }
+        // warp_best is rewritten only after the next work item's passes and their __syncthreads
+    }
+}
+#endif  // __CUDACC__
+
 #ifdef __CUDACC__
 // ---- the kernel: persistent CTAs over (batch, s) work items ------------------------------
 // D = 8: fs/bw = 8; D = 2: fs/bw = 2, where one symbol's combine spans fewer than 32 lanes at SF7 and SF8 and each group
@@ -339,6 +437,45 @@ inline void k1_emulate(const K1Args &a, uint32_t *bins, float *mags) {
     }
     for (size_t i = 0; i < a.n_symbols; i++) k1_store(bins, mags, i, packed[i]);
     delete[] buf;
+    delete[] packed;
+}
+
+// ... and of k1_antennas_kernel: M rows of n_symbols windows each, row_stride apart, into bins / mags[n_symbols]
+template <int SF, int D = 8>
+inline void k1_antennas_emulate(const K1Args &a, size_t row_stride, uint32_t m, uint32_t *bins, float *mags) {
+    using C = K1Cfg<SF, D>;
+    constexpr int NPT = C::NP / C::TPS;
+    float2 *buf = new float2[C::SMEM_ELEMS];
+    float *pw = new float[K1_THREADS * NPT];
+    const size_t n_batches = (a.n_symbols + C::G - 1) / C::G;
+    unsigned long long *packed = new unsigned long long[n_batches * C::G]();
+    for (size_t batch = 0; batch < n_batches; batch++) {
+        for (int s = 0; s < C::S; s++) {
+            for (int i = 0; i < K1_THREADS * NPT; i++) pw[i] = 0.f;
+            for (uint32_t ant = 0; ant < m; ant++) {
+                K1Args aa = a;
+                aa.x = a.x + ant * row_stride;
+                for (int i = 0; i < C::SMEM_ELEMS; i++) buf[i] = make_float2(NAN, NAN);
+                for (int t = 0; t < K1_THREADS; t++) k1_pass0<SF, true, D>(aa, batch, s, t, buf);
+                for (int t = 0; t < K1_THREADS; t++) k1_pass<SF, C::R1, C::SIG1, D>(aa, t, buf);
+                if (C::R2 > 1)
+                    for (int t = 0; t < K1_THREADS; t++) k1_pass<SF, (C::R2 > 1 ? C::R2 : 2), 1, D>(aa, t, buf);
+                for (int t = 0; t < K1_THREADS; t++) {
+                    float2 wtab[NPT];
+                    k1_combine_twiddles<SF, D>(aa, t, wtab);
+                    k1_combine_power<SF, D>(s, t, buf, wtab, pw + t * NPT);
+                }
+            }
+            for (int t = 0; t < K1_THREADS; t++) {
+                const unsigned long long k = k1_power_key<SF, D>(s, t, pw + t * NPT);
+                const size_t sym = batch * C::G + t / C::TPS;
+                if (k > packed[sym]) packed[sym] = k;
+            }
+        }
+    }
+    for (size_t i = 0; i < a.n_symbols; i++) k1_store(bins, mags, i, packed[i]);
+    delete[] buf;
+    delete[] pw;
     delete[] packed;
 }
 

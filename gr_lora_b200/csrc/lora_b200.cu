@@ -139,6 +139,11 @@ struct lora_b200_decoder : A1Params {
     DeviceBuffer<RxFrameOut> d_rs_out;
     std::vector<lora_b200_rx_info> rs_info;
     uint32_t rs_hdr_drops = 0;
+    // lora_b200_receive_antennas with several antennas: per synchronised frame h[4] | w[4] (rs_sync_antennas_kernel), and
+    // the published frames' h (rs_chan_m per frame) for lora_b200_rx_channels_last
+    DeviceBuffer<float2> d_rs_chan;
+    std::vector<float2> rs_chan;
+    uint32_t rs_chan_m = 1;
 };
 
 namespace {
@@ -475,6 +480,7 @@ int rx_finish(lora_b200_decoder *d, uint32_t stream_base, uint32_t n_launch, siz
     });
     d->h_sorted.resize(n_frames);
     d->rs_info.clear();                           // (lora_b200_rx_info_last describes lora_b200_receive calls only)
+    d->rs_chan.clear();
     for (uint32_t k = 0; k < n_frames; k++) {
         const RxFrameOut &f = d->h_frames[order[k]];
         d->h_sorted[k] = f;
@@ -1083,26 +1089,39 @@ int lora_b200_tx_frames_sfo_dev(lora_b200_decoder *d, const void *up_table, cons
 }  // extern "C"
 
 // ---- lora_b200_receive: the dechirp-synchronised receiver (rx_sync.cuh), every launch on rx_stream ----------------------
+// one receiver per stream (m = 1: rs_sync_kernel), or per group of m antenna rows (rs_sync_antennas_kernel)
 template <int SF, int D, bool DRIFT>
-static int rs_launch_sync(lora_b200_decoder *d, const float2 *x, size_t stride, size_t n_items, const RsParams &rp, uint32_t cap) {
-    static DeviceOnce once;
+static int rs_launch_sync(lora_b200_decoder *d, const float2 *x, size_t stride, size_t n_items, const RsParams &rp, uint32_t cap,
+                          uint32_t m) {
     const size_t smem = sizeof(float2) * K1Cfg<SF, D>::SMEM_ELEMS;
-    CU(once(d->device, [&] { return cudaFuncSetAttribute(rs_sync_kernel<SF, D, DRIFT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem); }));
-    rs_sync_kernel<SF, D, DRIFT><<<d->cfg.n_streams * cap, RX_THREADS, smem, d->rx_stream>>>(
-        x, stride, n_items, tab<float2>(d, d->toff.down), tab<float2>(d, d->toff.up), tab<float2>(d, d->toff.tw), rp, d->d_rs_cands,
-        d->d_rs_ncand, cap, d->d_rs_frames, d->d_rs_nframes, d->cfg.n_streams * cap, d->d_rs_hold);
+    const uint32_t ng = d->cfg.n_streams / m;
+    if (m == 1) {
+        static DeviceOnce once;
+        CU(once(d->device, [&] { return cudaFuncSetAttribute(rs_sync_kernel<SF, D, DRIFT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem); }));
+        rs_sync_kernel<SF, D, DRIFT><<<d->cfg.n_streams * cap, RX_THREADS, smem, d->rx_stream>>>(
+            x, stride, n_items, tab<float2>(d, d->toff.down), tab<float2>(d, d->toff.up), tab<float2>(d, d->toff.tw), rp, d->d_rs_cands,
+            d->d_rs_ncand, cap, d->d_rs_frames, d->d_rs_nframes, d->cfg.n_streams * cap, d->d_rs_hold);
+        return launched(d);
+    }
+    static DeviceOnce once_m;
+    CU(once_m(d->device, [&] {
+        return cudaFuncSetAttribute(rs_sync_antennas_kernel<SF, D, DRIFT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    }));
+    rs_sync_antennas_kernel<SF, D, DRIFT><<<ng * cap, RX_THREADS, smem, d->rx_stream>>>(
+        x, stride, n_items, m, tab<float2>(d, d->toff.down), tab<float2>(d, d->toff.up), tab<float2>(d, d->toff.tw), rp, d->d_rs_cands,
+        d->d_rs_ncand, cap, d->d_rs_frames, d->d_rs_nframes, ng * cap, d->d_rs_hold, d->d_rs_chan);
     return launched(d);
 }
 
 template <int D, bool DRIFT>
-static int rs_sync_sf(lora_b200_decoder *d, const float2 *x, size_t stride, size_t n_items, const RsParams &rp, uint32_t cap) {
+static int rs_sync_sf(lora_b200_decoder *d, const float2 *x, size_t stride, size_t n_items, const RsParams &rp, uint32_t cap, uint32_t m) {
     switch (d->cfg.sf) {
-    case 7: return rs_launch_sync<7, D, DRIFT>(d, x, stride, n_items, rp, cap);
-    case 8: return rs_launch_sync<8, D, DRIFT>(d, x, stride, n_items, rp, cap);
-    case 9: return rs_launch_sync<9, D, DRIFT>(d, x, stride, n_items, rp, cap);
-    case 10: return rs_launch_sync<10, D, DRIFT>(d, x, stride, n_items, rp, cap);
-    case 11: return rs_launch_sync<11, D, DRIFT>(d, x, stride, n_items, rp, cap);
-    case 12: return rs_launch_sync<12, D, DRIFT>(d, x, stride, n_items, rp, cap);
+    case 7: return rs_launch_sync<7, D, DRIFT>(d, x, stride, n_items, rp, cap, m);
+    case 8: return rs_launch_sync<8, D, DRIFT>(d, x, stride, n_items, rp, cap, m);
+    case 9: return rs_launch_sync<9, D, DRIFT>(d, x, stride, n_items, rp, cap, m);
+    case 10: return rs_launch_sync<10, D, DRIFT>(d, x, stride, n_items, rp, cap, m);
+    case 11: return rs_launch_sync<11, D, DRIFT>(d, x, stride, n_items, rp, cap, m);
+    case 12: return rs_launch_sync<12, D, DRIFT>(d, x, stride, n_items, rp, cap, m);
     }
     return fail(LORA_B200_EUNSUPPORTED, "unsupported SF %u", d->cfg.sf);
 }
@@ -1110,16 +1129,63 @@ static int rs_sync_sf(lora_b200_decoder *d, const float2 *x, size_t stride, size
 // without a clock offset the synchroniser runs its DRIFT = false instantiation, which does no drift arithmetic; D = sps / N
 // (8 or 2) selects the K1 phase functions of its argmax windows
 template <int D>
-static int rs_sync_d(lora_b200_decoder *d, const float2 *x, size_t stride, size_t n_items, const RsParams &rp, uint32_t cap) {
-    return rs_drift(rp) ? rs_sync_sf<D, true>(d, x, stride, n_items, rp, cap) : rs_sync_sf<D, false>(d, x, stride, n_items, rp, cap);
+static int rs_sync_d(lora_b200_decoder *d, const float2 *x, size_t stride, size_t n_items, const RsParams &rp, uint32_t cap, uint32_t m) {
+    return rs_drift(rp) ? rs_sync_sf<D, true>(d, x, stride, n_items, rp, cap, m) : rs_sync_sf<D, false>(d, x, stride, n_items, rp, cap, m);
 }
-static int rs_sync(lora_b200_decoder *d, const float2 *x, size_t stride, size_t n_items, const RsParams &rp, uint32_t cap) {
-    return d->k1_osr2 ? rs_sync_d<2>(d, x, stride, n_items, rp, cap) : rs_sync_d<8>(d, x, stride, n_items, rp, cap);
+static int rs_sync(lora_b200_decoder *d, const float2 *x, size_t stride, size_t n_items, const RsParams &rp, uint32_t cap, uint32_t m) {
+    return d->k1_osr2 ? rs_sync_d<2>(d, x, stride, n_items, rp, cap, m) : rs_sync_d<8>(d, x, stride, n_items, rp, cap, m);
 }
 
-extern "C" {
+// the combined screen of ng receivers with m antennas: k1_antennas_kernel over the n_win windows of each row (rows `stride`
+// apart), receiver g's results at bins / mags[g * out_stride ..]
+template <int SF, int D>
+static int rs_screen_launch(lora_b200_decoder *d, const float2 *x, size_t n_win, size_t stride, uint32_t m, uint32_t ng, size_t out_stride,
+                            uint32_t *bins, float *mags, cudaStream_t st) {
+    using C = K1Cfg<SF, D>;
+    static DeviceOnce once;
+    const size_t smem = sizeof(float2) * C::SMEM_ELEMS;
+    CU(once(d->device, [&] { return cudaFuncSetAttribute(k1_antennas_kernel<SF, D>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem); }));
+    const size_t n_work = (n_win + C::G - 1) / C::G * ng;
+    const int grid = (int)std::min<size_t>(n_work, (size_t)d->n_sms * 2);
+    k1_antennas_kernel<SF, D><<<grid, K1_THREADS, smem, st>>>(K1Args{x, tab<float2>(d, d->toff.down), tab<float2>(d, d->toff.tw), n_win},
+                                                             stride, m, ng, out_stride, bins, mags);
+    return launched(d);
+}
+template <int D>
+static int rs_screen_d(lora_b200_decoder *d, const float2 *x, size_t n_win, size_t stride, uint32_t m, uint32_t ng, size_t out_stride,
+                       uint32_t *bins, float *mags, cudaStream_t st) {
+    switch (d->cfg.sf) {
+    case 7: return rs_screen_launch<7, D>(d, x, n_win, stride, m, ng, out_stride, bins, mags, st);
+    case 8: return rs_screen_launch<8, D>(d, x, n_win, stride, m, ng, out_stride, bins, mags, st);
+    case 9: return rs_screen_launch<9, D>(d, x, n_win, stride, m, ng, out_stride, bins, mags, st);
+    case 10: return rs_screen_launch<10, D>(d, x, n_win, stride, m, ng, out_stride, bins, mags, st);
+    case 11: return rs_screen_launch<11, D>(d, x, n_win, stride, m, ng, out_stride, bins, mags, st);
+    case 12: return rs_screen_launch<12, D>(d, x, n_win, stride, m, ng, out_stride, bins, mags, st);
+    }
+    return fail(LORA_B200_EUNSUPPORTED, "unsupported SF %u", d->cfg.sf);
+}
+static int rs_screen(lora_b200_decoder *d, const float2 *x, size_t n_win, size_t stride, uint32_t m, uint32_t ng, size_t out_stride,
+                     uint32_t *bins, float *mags, cudaStream_t st) {
+    return d->k1_osr2 ? rs_screen_d<2>(d, x, n_win, stride, m, ng, out_stride, bins, mags, st)
+                      : rs_screen_d<8>(d, x, n_win, stride, m, ng, out_stride, bins, mags, st);
+}
 
-int lora_b200_receive(lora_b200_decoder *d, const void *iq, size_t n_items, size_t stride_items, int host_ptr,
+// the data windows of frames [slots], as rs_assemble_kernel (m = 1) or combined over m antennas
+static int rs_assemble(lora_b200_decoder *d, const float2 *x, size_t stride, size_t n_items, uint32_t m, const RsFrame *frames,
+                       const float2 *chan, uint32_t n_frames, const uint32_t *idx, uint32_t first, const uint32_t *offs, uint32_t off_base,
+                       const uint32_t *cnts) {
+    const int grid = std::min<int>((int)n_frames, d->n_sms * 8);
+    if (m == 1)
+        rs_assemble_kernel<<<grid, 256, 0, d->rx_stream>>>(x, stride, (long long)n_items, frames, n_frames, idx, first, offs, off_base,
+                                                           cnts, d->sps, d->d_rs_win);
+    else
+        rs_assemble_antennas_kernel<<<grid, 256, 0, d->rx_stream>>>(x, stride, (long long)n_items, m, frames, chan, n_frames, idx, first,
+                                                                    offs, off_base, cnts, d->sps, d->d_rs_win);
+    return launched(d);
+}
+
+// lora_b200_receive (m = 1) and lora_b200_receive_antennas: the receiver of group g reads rows g m .. g m + m - 1
+static int rs_receive(lora_b200_decoder *d, const void *iq, size_t n_items, size_t stride_items, int host_ptr, uint32_t m,
                       const lora_b200_rx_params *prm, size_t *consumed) {
     if (!d || !consumed || (!iq && n_items)) return fail(LORA_B200_EINVAL, "null argument");
     if (stride_items < n_items) return fail(LORA_B200_EINVAL, "stride_items %zu < n_items %zu", stride_items, n_items);
@@ -1136,7 +1202,8 @@ int lora_b200_receive(lora_b200_decoder *d, const void *iq, size_t n_items, size
         return fail(LORA_B200_EINVAL, "carrier_hz must be 0 or above the sample rate %g, got %g", d->samples_per_second, P.carrier_hz);
     if (P.soft > 1u) return fail(LORA_B200_EINVAL, "soft must be 0 or 1, got %u", (unsigned)P.soft);
     CU(cudaSetDevice(d->device));
-    const uint32_t ns = d->cfg.n_streams, sps = d->sps, N = d->n_bins, cap = d->cfg.max_frames_per_call;
+    // rows: ns; receivers (groups of m antenna rows): ng.  m = 1 is lora_b200_receive, launch for launch.
+    const uint32_t rows = d->cfg.n_streams, ns = rows / m, sps = d->sps, N = d->n_bins, cap = d->cfg.max_frames_per_call;
     const bool soft = P.soft != 0;
     const uint8_t sw = P.sync_word ? P.sync_word : 0x12;
     const float fs = (float)d->samples_per_second, bin_hz = fs / (float)sps;
@@ -1149,6 +1216,8 @@ int lora_b200_receive(lora_b200_decoder *d, const void *iq, size_t n_items, size
     d->rs_info.clear();
     d->h_sorted.clear();
     d->rs_hdr_drops = 0;
+    d->rs_chan.clear();
+    d->rs_chan_m = m;
     const size_t guard = (size_t)(rp.min_preamble + 4u) * sps, none = ~(size_t)0;
     std::vector<size_t> end_pub(ns, 0), hold(ns, none);
     auto finish = [&]() {
@@ -1166,16 +1235,30 @@ int lora_b200_receive(lora_b200_decoder *d, const void *iq, size_t n_items, size
     size_t stride = stride_items;
     if (host_ptr || stride % sps || ((uintptr_t)iq & 15u)) {
         stride = (n_items + sps - 1) / sps * sps;
-        CU(d->d_rs_stage.reserve(stride * ns));
-        CU(cudaMemcpy2DAsync(d->d_rs_stage, sizeof(float2) * stride, iq, sizeof(float2) * stride_items, sizeof(float2) * n_items, ns,
+        CU(d->d_rs_stage.reserve(stride * rows));
+        CU(cudaMemcpy2DAsync(d->d_rs_stage, sizeof(float2) * stride, iq, sizeof(float2) * stride_items, sizeof(float2) * n_items, rows,
                              host_ptr ? cudaMemcpyHostToDevice : cudaMemcpyDeviceToDevice, st));
         x = d->d_rs_stage;
     }
-    const size_t span = (ns - 1) * stride + n_items, nw[2] = {span / sps, (span - sps / 2) / sps};
-    for (int ph = 0; ph < 2; ph++) {
-        CU(d->d_rs_bins[ph].reserve(nw[ph] + 1));
-        CU(d->d_rs_mags[ph].reserve(nw[ph] + 1));
-        if (int rc = dispatch_k1(d, d->k1s[0], x + ph * (sps / 2), nw[ph], d->d_rs_bins[ph], d->d_rs_mags[ph], st)) return rc;
+    if (m == 1) {
+        const size_t span = (ns - 1) * stride + n_items, nw[2] = {span / sps, (span - sps / 2) / sps};
+        for (int ph = 0; ph < 2; ph++) {
+            CU(d->d_rs_bins[ph].reserve(nw[ph] + 1));
+            CU(d->d_rs_mags[ph].reserve(nw[ph] + 1));
+            if (int rc = dispatch_k1(d, d->k1s[0], x + ph * (sps / 2), nw[ph], d->d_rs_bins[ph], d->d_rs_mags[ph], st)) return rc;
+        }
+    } else {
+        // the combined screen: receiver g's window j of phase ph at bins[ph][g * stride / sps + j], as rs_detect_kernel reads
+        // the screen of one row (only the windows it reads are computed)
+        const size_t nw[2] = {n_items / sps, n_items >= sps + sps / 2 ? (n_items - sps / 2) / sps : 0};
+        for (int ph = 0; ph < 2; ph++) {
+            CU(d->d_rs_bins[ph].reserve((size_t)ns * (stride / sps) + 1));
+            CU(d->d_rs_mags[ph].reserve((size_t)ns * (stride / sps) + 1));
+            if (nw[ph] == 0) continue;
+            if (int rc = rs_screen(d, x + ph * (sps / 2), nw[ph], stride, m, ns, stride / sps, d->d_rs_bins[ph], d->d_rs_mags[ph], st))
+                return rc;
+        }
+        CU(d->d_rs_chan.reserve((size_t)ns * cap * 2 * RS_MAX_ANTENNAS));
     }
     // detect, synchronise
     const uint32_t fcap = ns * cap;
@@ -1190,7 +1273,7 @@ int lora_b200_receive(lora_b200_decoder *d, const void *iq, size_t n_items, size
     rs_detect_kernel<<<(ns + 127) / 128, 128, 0, st>>>(d->d_rs_bins[0], d->d_rs_mags[0], d->d_rs_bins[1], d->d_rs_mags[1], stride, n_items,
                                                        ns, rp, d->d_rs_cands, cap, d->d_rs_ncand, d->d_rs_dropped);
     if (int rc = launched(d)) return rc;
-    if (int rc = rs_sync(d, x, stride, n_items, rp, cap)) return rc;
+    if (int rc = rs_sync(d, x, stride, n_items, rp, cap, m)) return rc;
     uint32_t n_sync = 0;
     std::vector<long long> dropped(ns);
     std::vector<unsigned long long> shold(ns);
@@ -1211,12 +1294,11 @@ int lora_b200_receive(lora_b200_decoder *d, const void *iq, size_t n_items, size
     // soft decisions: LLRs of ppm values per window (sf - 2 in the header round), corrected into the bins afterwards
     const uint32_t hppm = d->cfg.sf - 2u, pppm = d->cfg.reduced_rate ? hppm : d->cfg.sf;
     if (soft) CU(d->d_rs_llr.reserve((size_t)n_sync * 8 * hppm));
-    const int agrid = d->n_sms * 8;
     for (uint32_t f0 = 0; f0 < n_sync; f0 += (uint32_t)(win_cap / 8)) {
         const uint32_t nb = (uint32_t)std::min<size_t>(win_cap / 8, n_sync - f0);
-        rs_assemble_kernel<<<std::min<int>((int)nb, agrid), 256, 0, st>>>(x, stride, (long long)n_items, d->d_rs_frames + f0, nb, nullptr, 0,
-                                                                          nullptr, 0, nullptr, sps, d->d_rs_win);
-        if (int rc = launched(d)) return rc;
+        if (int rc = rs_assemble(d, x, stride, n_items, m, d->d_rs_frames + f0, m > 1 ? d->d_rs_chan + (size_t)f0 * 2 * RS_MAX_ANTENNAS : nullptr,
+                                 nb, nullptr, 0, nullptr, 0, nullptr))
+            return rc;
         if (soft) {
             if (int rc = dispatch_llr(d, d->d_rs_win, (size_t)nb * 8, true, d->d_rs_llr + (size_t)f0 * 8 * hppm, nullptr, st)) return rc;
         } else if (int rc = dispatch_k1(d, d->k1s[0], d->d_rs_win, (size_t)nb * 8, d->d_rs_hbins + (size_t)f0 * 8, nullptr, st)) {
@@ -1288,10 +1370,9 @@ int lora_b200_receive(lora_b200_decoder *d, const void *iq, size_t n_items, size
         uint32_t g1 = g0, w = 0;
         while (g1 < np && w + tabh[3 * np + g1] <= pwin_cap) w += tabh[3 * np + g1++];
         if (w) {
-            rs_assemble_kernel<<<std::min<int>((int)(g1 - g0), agrid), 256, 0, st>>>(x, stride, (long long)n_items, d->d_rs_frames, g1 - g0,
-                                                                                    t_pub + g0, 8, t_off + g0, tabh[2 * np + g0], t_cnt + g0,
-                                                                                    sps, d->d_rs_win);
-            if (int rc = launched(d)) return rc;
+            if (int rc = rs_assemble(d, x, stride, n_items, m, d->d_rs_frames, d->d_rs_chan, g1 - g0, t_pub + g0, 8, t_off + g0,
+                                     tabh[2 * np + g0], t_cnt + g0))
+                return rc;
             const size_t o = tabh[2 * np + g0];
             if (soft) {
                 if (int rc = dispatch_llr(d, d->d_rs_win, w, d->cfg.reduced_rate != 0, d->d_rs_llr + o * pppm, nullptr, st)) return rc;
@@ -1319,6 +1400,11 @@ int lora_b200_receive(lora_b200_decoder *d, const void *iq, size_t n_items, size
     if (int rc = launched(d)) return rc;
     d->h_sorted.resize(np);
     CU(cudaMemcpyAsync(d->h_sorted.data(), d->d_rs_out, sizeof(RxFrameOut) * np, cudaMemcpyDeviceToHost, st));
+    std::vector<float2> chan;
+    if (m > 1) {
+        chan.resize((size_t)n_sync * 2 * RS_MAX_ANTENNAS);
+        CU(cudaMemcpyAsync(chan.data(), d->d_rs_chan, sizeof(float2) * chan.size(), cudaMemcpyDeviceToHost, st));
+    }
     CU(cudaStreamSynchronize(st));
     d->rs_info.resize(np);
     for (uint32_t k = 0; k < np; k++) {
@@ -1326,8 +1412,45 @@ int lora_b200_receive(lora_b200_decoder *d, const void *iq, size_t n_items, size
         const long long d0 = rs_sym(r.start, rs_data_j(0), sps, r.sfo_ppm);
         d->rs_info[k] = lora_b200_rx_info{(uint64_t)r.start, (uint64_t)d0, r.stream, r.cfo_bins * bin_hz, r.snr_db, r.sfo_ppm};
         end_pub[r.stream] = std::max(end_pub[r.stream], (size_t)data_end(r, 8ll + r.n_payload));
+        if (m > 1) d->rs_chan.insert(d->rs_chan.end(), chan.begin() + (size_t)pub[k] * 2 * RS_MAX_ANTENNAS,
+                                     chan.begin() + (size_t)pub[k] * 2 * RS_MAX_ANTENNAS + m);
     }
     return finish();
+}
+
+extern "C" {
+
+int lora_b200_receive(lora_b200_decoder *d, const void *iq, size_t n_items, size_t stride_items, int host_ptr,
+                      const lora_b200_rx_params *prm, size_t *consumed) {
+    return rs_receive(d, iq, n_items, stride_items, host_ptr, 1, prm, consumed);
+}
+
+int lora_b200_receive_antennas(lora_b200_decoder *d, const void *iq, size_t n_items, size_t stride_items, int host_ptr,
+                               uint32_t n_antennas, const lora_b200_rx_params *p, size_t *consumed) {
+    if (!d) return fail(LORA_B200_EINVAL, "null argument");
+    if (n_antennas < 1 || n_antennas > (uint32_t)RS_MAX_ANTENNAS || d->cfg.n_streams % n_antennas)
+        return fail(LORA_B200_EINVAL, "n_antennas must be 1..%d and divide n_streams %u, got %u", RS_MAX_ANTENNAS, d->cfg.n_streams,
+                    n_antennas);
+    return rs_receive(d, iq, n_items, stride_items, host_ptr, n_antennas, p, consumed);
+}
+
+size_t lora_b200_rx_channels_last(lora_b200_decoder *d, const float **h, uint32_t *n_antennas) {
+    if (!d || !h) { fail(LORA_B200_EINVAL, "null argument"); return 0; }
+    *h = reinterpret_cast<const float *>(d->rs_chan.data());
+    if (n_antennas) *n_antennas = d->rs_chan_m;
+    return d->rs_chan_m > 1 ? d->rs_chan.size() / d->rs_chan_m : 0;
+}
+
+int lora_b200_demod_fft_antennas_dev(lora_b200_decoder *d, const void *iq, uint32_t n_groups, uint32_t n_antennas, size_t n_symbols,
+                                     size_t row_stride_items, uint32_t *bins, float *mags, void *cuda_stream) {
+    if (!d || (n_symbols && n_groups && (!iq || !bins || !mags))) return fail(LORA_B200_EINVAL, "null argument");
+    if (!d->k1_ok && !d->k1_osr2) return fail(LORA_B200_EUNSUPPORTED, "the combined screen needs samp_rate/bandwidth == 8 or 2 and SF7..SF12");
+    if (n_antennas < 1 || n_antennas > (uint32_t)RS_MAX_ANTENNAS) return fail(LORA_B200_EINVAL, "n_antennas must be 1..%d, got %u", RS_MAX_ANTENNAS, n_antennas);
+    if (row_stride_items < n_symbols * d->sps || row_stride_items % 2 || ((uintptr_t)iq & 15u))
+        return fail(LORA_B200_EINVAL, "rows must hold n_symbols windows, start 16-byte aligned and lie an even number of samples apart");
+    CU(cudaSetDevice(d->device));
+    if (n_symbols == 0 || n_groups == 0) return LORA_B200_OK;
+    return rs_screen(d, (const float2 *)iq, n_symbols, row_stride_items, n_antennas, n_groups, n_symbols, bins, mags, (cudaStream_t)cuda_stream);
 }
 
 static_assert(sizeof(lora_b200_rx_info) == 32 && sizeof(lora_b200_rx_params) == 32 && offsetof(lora_b200_rx_params, soft) == 1 &&

@@ -139,12 +139,18 @@ LB_HD uint32_t rs_detect_stream(const uint32_t *const bins[2], const float *cons
 }
 
 // ---- synchronise ---------------------------------------------------------------------------------------------------------
-// Ops gives the procedure its windows (block-collective on the device, plain loops on the host):
+// Ops gives the procedure its windows (block-collective on the device, plain loops on the host).  A receiver may have
+// several antennas (rows) sharing one timing and CFO; Ops::M is how many values binvals writes (1 for one row; with
+// fewer antennas than M the rest are 0):
 //   bool in_range(long long pos)                       window [pos, pos + sps) inside the row
-//   unsigned long long argmax(long long pos, bool up)  K1 argmax key of the raw window, dechirped with the down (up) chirp
-//   float2 binval(long long pos, float F, bool up, int bin)   bin `bin` (signed, -N/2..N/2) of the window de-rotated by F bins
-//   float energy(long long pos)                        sum |x|^2 over the window
+//   unsigned long long argmax(long long pos, bool up)  K1 argmax key of the raw window, dechirped with the down (up) chirp;
+//                                                      over several antennas the key of the summed |tmp_a|^2
+//   void binvals(long long pos, float F, bool up, int bin, float2 *v)   v[a]: bin `bin` (signed, -N/2..N/2) of antenna a's
+//                                                      window de-rotated by F bins
+//   float energy(long long pos)                        sum |x|^2 over the window (of every antenna)
 // The dechirp tables are (1 + 1j) e^{+-j phase}: |table|^2 = 2.
+constexpr int RS_MAX_ANTENNAS = 4;
+
 LB_HD float rs_phase_rev(float2 z) { return atan2f(z.y, z.x) * 0.15915494309189535f; }   // arg / 2 pi
 
 // score of a hypothesis (start rs_sym(t, m), CFO F bins, windows placed with its clock offset): energy at the expected bins
@@ -162,7 +168,9 @@ LB_HD float rs_score(Ops &ops, const RsParams &p, long long t, int m, float F) {
         const long long pos = rs_pos<DRIFT>(t, i + m, p.sps, ppm);
         if (pos < 0 || !ops.in_range(pos)) continue;
         const int bin = i == 8 ? rs_smod((int)p.sw[0], N) : i == 9 ? rs_smod((int)p.sw[1], N) : 0;
-        s += cnorm2(ops.binval(pos, F, i >= 10, bin));
+        float2 v[Ops::M];
+        ops.binvals(pos, F, i >= 10, bin, v);
+        for (int a = 0; a < Ops::M; a++) s += cnorm2(v[a]);
     }
     return s;
 }
@@ -198,13 +206,17 @@ LB_HD RsFrame rs_synchronise(Ops &ops, const RsCand &c, const RsParams &p, uint3
     const long long t0 = DRIFT ? c.p_last - (long long)lrintf(tau * decim) - rs_pos<DRIFT>(0, 10 - kbest, p.sps, rc)
                                : c.p_last + kbest * sps - (long long)lrintf(tau * decim) - 10 * sps;
     // fractional CFO: phase advance of the preamble peak from symbol to symbol (its residual modulo one bin)
-    float2 z = make_float2(0.f, 0.f), prev = make_float2(0.f, 0.f);
+    float2 z = make_float2(0.f, 0.f), prev[Ops::M];
+    for (int a = 0; a < Ops::M; a++) prev[a] = make_float2(0.f, 0.f);
     for (int i = 1; i <= 6; i++) {
         const long long pos = rs_pos<DRIFT>(t0, i, p.sps, rc);
         if (pos < 0 || !ops.in_range(pos)) continue;
-        const float2 x = ops.binval(pos, Fc, false, 0);
-        if (i > 1) z = cadd(z, cmul(x, cconj(prev)));
-        prev = x;
+        float2 x[Ops::M];
+        ops.binvals(pos, Fc, false, 0, x);
+        for (int a = 0; a < Ops::M; a++) {
+            if (i > 1) z = cadd(z, cmul(x[a], cconj(prev[a])));
+            prev[a] = x[a];
+        }
     }
     const float eps = rs_phase_rev(z);
     float best_s = -1.f, Fb = 0.f;
@@ -234,10 +246,16 @@ LB_HD RsFrame rs_synchronise(Ops &ops, const RsCand &c, const RsParams &p, uint3
     for (int i = 0; i < 8; i++) {
         const long long pos = rs_pos<DRIFT>(tf, i, p.sps, rb);
         if (pos < 0 || !ops.in_range(pos)) continue;
-        const float2 x = ops.binval(pos, Fb, false, 0);
-        if (npk) z = cadd(z, cmul(x, cconj(prev)));
-        prev = x;
-        if (i >= 1 && i <= 6) { pk += cnorm2(x); en += ops.energy(pos); }
+        float2 x[Ops::M];
+        ops.binvals(pos, Fb, false, 0, x);
+        for (int a = 0; a < Ops::M; a++) {
+            if (npk) z = cadd(z, cmul(x[a], cconj(prev[a])));
+            prev[a] = x[a];
+        }
+        if (i >= 1 && i <= 6) {
+            for (int a = 0; a < Ops::M; a++) pk += cnorm2(x[a]);
+            en += ops.energy(pos);
+        }
         npk++;
     }
     const float F = Fb + rs_phase_rev(z);
@@ -259,6 +277,61 @@ LB_HD RsFrame rs_synchronise(Ops &ops, const RsCand &c, const RsParams &p, uint3
     r.start = tf; r.cfo_bins = F; r.snr_db = 10.0f * log10f(S / s2 * decim); r.sfo_ppm = rs_ppm_of<DRIFT>(p, F);
     r.status = RS_OK;
     return r;
+}
+
+// ---- several antennas: channel estimates and maximum-ratio combining weights ------------------------------------------------
+// At a synchronised frame's final timing and CFO, per antenna a of the m = Ops::M-or-fewer rows (energies(pos, e): e[a] =
+// sum |x_a|^2 over the window):
+//   h[a]  = the mean of its de-rotated preamble peaks binval_a(i, F, 0) over windows 1..6, over (1 + j) sps: the amplitude
+//           per sample, with a phase whose reference is common to the frame's antennas
+//   s2[a] = its noise power per sample, from window energy minus peak as rs_synchronise's SNR estimate (floored at 60 dB
+//           below the strongest antenna's energy, so that noiseless rows keep finite weights)
+//   w[a]  = conj(h[a]) / s2[a], scaled to sum |w|^2 = 1: y = sum_a w[a] x_a has the noise power of one antenna when all
+//           are alike, and the scale of one frame's y does not move any decision of the decoder
+// Returns the combined (post-MRC) SNR in dB in the LoRa bandwidth: the sum of the antennas' SNRs.
+#ifdef __CUDACC__
+#pragma nv_exec_check_disable
+#endif
+template <bool DRIFT, class Ops>
+LB_HD float rs_channels(Ops &ops, const RsParams &p, const RsFrame &r, uint32_t m, float2 *h, float2 *w) {
+    const float sps = (float)p.sps;
+    float2 acc[Ops::M];
+    float pk[Ops::M], en[Ops::M];
+    for (int a = 0; a < Ops::M; a++) { acc[a] = make_float2(0.f, 0.f); pk[a] = 0.f; en[a] = 0.f; }
+    int nw = 0;
+    for (int i = 1; i <= 6; i++) {
+        const long long pos = rs_pos<DRIFT>(r.start, i, p.sps, r.sfo_ppm);
+        if (pos < 0 || !ops.in_range(pos)) continue;
+        float2 x[Ops::M];
+        float e[Ops::M];
+        ops.binvals(pos, r.cfo_bins, false, 0, x);
+        ops.energies(pos, e);
+        for (int a = 0; a < Ops::M; a++) { acc[a] = cadd(acc[a], x[a]); pk[a] += cnorm2(x[a]); en[a] += e[a]; }
+        nw++;
+    }
+    const float nwf = nw ? (float)nw : 1.f;
+    float s2[Ops::M], emax = 0.f, snr = 0.f;
+    for (int a = 0; a < (int)m; a++) emax = fmaxf(emax, en[a] / nwf / sps);
+    for (int a = 0; a < (int)m; a++) {
+        const float px = pk[a] / (2.0f * nwf) / sps, e = en[a] / nwf;          // |table|^2 = 2
+        s2[a] = fmaxf(fmaxf((e - px) / (sps - 1.0f), 1e-6f * emax), 1e-30f);
+        const float S = fmaxf((px - s2[a]) / sps, 1e-30f);
+        snr += S / s2[a];
+        // mean peak / ((1 + j) sps) = mean peak (1 - j) / (2 sps)
+        const float2 c = make_float2(acc[a].x / nwf, acc[a].y / nwf);
+        h[a] = make_float2((c.x + c.y) / (2.0f * sps), (c.y - c.x) / (2.0f * sps));
+    }
+    float s2min = s2[0];
+    for (int a = 1; a < (int)m; a++) s2min = fminf(s2min, s2[a]);
+    float norm = 0.f;
+    for (int a = 0; a < (int)m; a++) {
+        w[a] = make_float2(h[a].x * (s2min / s2[a]), -h[a].y * (s2min / s2[a]));
+        norm += cnorm2(w[a]);
+    }
+    const float k = norm > 0.f ? 1.0f / sqrtf(norm) : 0.f;
+    for (int a = 0; a < (int)m; a++) w[a] = norm > 0.f ? make_float2(w[a].x * k, w[a].y * k) : make_float2(a == 0 ? 1.f : 0.f, 0.f);
+    for (int a = (int)m; a < Ops::M; a++) { h[a] = make_float2(0.f, 0.f); w[a] = make_float2(0.f, 0.f); }
+    return 10.0f * log10f(snr * (float)p.decim);
 }
 
 // ---- the integer chain of one frame -------------------------------------------------------------------------------------
@@ -387,6 +460,7 @@ __global__ void rs_detect_kernel(const uint32_t *__restrict__ bins0, const float
 // argmax's only use of the sample rate (binval and energy take sps at run time)
 template <int SF, int D = 8>
 struct RsDevOps {
+    static constexpr int M = 1;
     const float2 *x;                   // the row
     long long n_items;
     const float2 *down, *up, *tw;
@@ -432,11 +506,105 @@ struct RsDevOps {
         block_sum<2>(v, *sh);
         return make_float2(v[0], v[1]);
     }
+    LB_D void binvals(long long pos, float F, bool use_up, int bin, float2 *v) { v[0] = binval(pos, F, use_up, bin); }
     LB_D float energy(long long pos) {
         float v[1] = {0.f};
         for (uint32_t n = threadIdx.x; n < sps; n += RX_THREADS) { const float2 a = x[pos + n]; v[0] += a.x * a.x + a.y * a.y; }
         block_sum<1>(v, *sh);
         return v[0];
+    }
+};
+
+// the windows of one candidate of a receiver with m <= RS_MAX_ANTENNAS antennas, rows one.x + a * stride: argmax of the
+// combined spectrum (the phase functions of k1_antennas_kernel on one window position), binval and energy per antenna
+template <int SF, int D = 8>
+struct RsAntOps {
+    static constexpr int M = RS_MAX_ANTENNAS;
+    RsDevOps<SF, D> one;               // antenna 0
+    size_t stride;
+    uint32_t m;
+    LB_D bool in_range(long long pos) const { return one.in_range(pos); }
+    static_assert(M == 4, "binvals reduces 2 M sums as two block_sum<4>");
+    LB_D unsigned long long argmax(long long pos, bool use_up) {
+        using C = K1Cfg<SF, D>;
+        const int tid = threadIdx.x;
+        K1Args a{one.x + pos, use_up ? one.up : one.down, one.tw, 1};
+        unsigned long long best = 0ull;
+        float2 wtab[C::NP / C::TPS];
+        k1_combine_twiddles<SF, D>(a, tid, wtab);
+        for (int s = 0; s < C::S; s++) {
+            float pw[C::NP / C::TPS];
+            for (int i = 0; i < C::NP / C::TPS; i++) pw[i] = 0.f;
+            for (uint32_t ant = 0; ant < m; ant++) {
+                K1Args aa = a;
+                aa.x = a.x + ant * stride;
+                k1_pass0<SF, false, D>(aa, 0, s, tid, one.smem);
+                __syncthreads();
+                k1_pass<SF, C::R1, C::SIG1, D>(aa, tid, one.smem);
+                __syncthreads();
+                if (C::R2 > 1) { k1_pass<SF, (C::R2 > 1 ? C::R2 : 2), 1, D>(aa, tid, one.smem); __syncthreads(); }
+                if (tid < C::TPS) k1_combine_power<SF, D>(s, tid, one.smem, wtab, pw);
+                __syncthreads();
+            }
+            const unsigned long long k = tid < C::TPS ? k1_power_key<SF, D>(s, tid, pw) : 0ull;
+            best = k > best ? k : best;
+        }
+        return block_max_key(best, *one.sh);
+    }
+    // every antenna's bin in one pass over the window: the de-rotation and bin twiddle of sample n are formed once and
+    // applied to the m rows, and the 2m sums go through block_sum four at a time (one reduction for m <= 2, two for m > 2)
+    LB_D void binvals(long long pos, float F, bool use_up, int bin, float2 *v) {
+        const uint32_t sps = one.sps;
+        const float2 *ch = use_up ? one.up : one.down;
+        double base = (double)F * (double)pos / (double)sps;
+        base -= floor(base);
+        const float fb = (float)base, fr = F / (float)sps;
+        const uint32_t kb = (uint32_t)((bin % (int)sps) + (int)sps) % sps;
+        float s[2 * M];
+#pragma unroll
+        for (int k = 0; k < 2 * M; k++) s[k] = 0.f;
+        for (uint32_t n = threadIdx.x; n < sps; n += RX_THREADS) {
+            float t = fmaf(fr, (float)n, fb);
+            t -= floorf(t);
+            float sn, cs;
+            sincospif(-2.0f * t, &sn, &cs);
+            float2 q = cmul(__ldg(ch + n), make_float2(cs, sn));
+            if (kb) q = cmul(q, __ldg(one.tw + (size_t)((unsigned long long)kb * n % sps)));
+#pragma unroll
+            for (int a = 0; a < M; a++) {
+                if (a < (int)m) {
+                    const float2 y = cmul(one.x[(size_t)a * stride + pos + n], q);
+                    s[2 * a] += y.x; s[2 * a + 1] += y.y;
+                }
+            }
+        }
+        float r[4] = {s[0], s[1], s[2], s[3]};
+        block_sum<4>(r, *one.sh);
+        v[0] = make_float2(r[0], r[1]); v[1] = make_float2(r[2], r[3]);
+        if (m > 2) {
+            float r2[4] = {s[4], s[5], s[6], s[7]};
+            block_sum<4>(r2, *one.sh);
+            v[2] = make_float2(r2[0], r2[1]); v[3] = make_float2(r2[2], r2[3]);
+        } else {
+            v[2] = v[3] = make_float2(0.f, 0.f);
+        }
+    }
+    LB_D void energies(long long pos, float *e) {
+        float s[4] = {0.f, 0.f, 0.f, 0.f};
+        for (uint32_t n = threadIdx.x; n < one.sps; n += RX_THREADS) {
+#pragma unroll
+            for (int a = 0; a < M; a++) {
+                if (a < (int)m) { const float2 x = one.x[(size_t)a * stride + pos + n]; s[a] += x.x * x.x + x.y * x.y; }
+            }
+        }
+        block_sum<4>(s, *one.sh);
+        for (int a = 0; a < M; a++) e[a] = s[a];
+    }
+    LB_D float energy(long long pos) {
+        float e[M], s = 0.f;
+        energies(pos, e);
+        for (int a = 0; a < M; a++) s += e[a];
+        return s;
     }
 };
 
@@ -459,6 +627,39 @@ rs_sync_kernel(const float2 *__restrict__ iq, size_t stride, size_t n_items, con
         if (r.status == RS_OK) {
             const uint32_t slot = atomicAdd(n_frames, 1u);
             if (slot < frame_cap) frames[slot] = r;
+        }
+    }
+}
+
+// ... of receivers with m antennas each (group s: rows s * m .. s * m + m - 1): the same procedure over RsAntOps, then the
+// channel estimates and combining weights (rs_channels) of every synchronised frame into chan[slot][0..4) (h) and
+// chan[slot][4..8) (w); snr_db is the combined SNR
+template <int SF, int D, bool DRIFT>
+__global__ void __launch_bounds__(RX_THREADS)
+rs_sync_antennas_kernel(const float2 *__restrict__ iq, size_t stride, size_t n_items, uint32_t m, const float2 *down, const float2 *up,
+                        const float2 *tw, RsParams p, const RsCand *__restrict__ cands, const uint32_t *__restrict__ n_cands, uint32_t cap,
+                        RsFrame *__restrict__ frames, uint32_t *__restrict__ n_frames, uint32_t frame_cap,
+                        unsigned long long *__restrict__ hold, float2 *__restrict__ chan) {
+    extern __shared__ float2 rs_dyn_smem[];
+    __shared__ RxShared sh;
+    const uint32_t s = blockIdx.x / cap, i = blockIdx.x % cap;
+    const uint32_t nc = n_cands[s];
+    if (i >= (nc < cap ? nc : cap)) return;
+    RsAntOps<SF, D> ops{{iq + (size_t)s * m * stride, (long long)n_items, down, up, tw, p.sps, rs_dyn_smem, &sh}, stride, m};
+    RsFrame r = rs_synchronise<DRIFT>(ops, cands[(size_t)s * cap + i], p, s);
+    float2 h[RS_MAX_ANTENNAS], w[RS_MAX_ANTENNAS];
+    if (r.status == RS_OK) r.snr_db = rs_channels<DRIFT>(ops, p, r, m, h, w);
+    if (threadIdx.x == 0) {
+        if (r.status == RS_INCOMPLETE) atomicMin(hold + s, (unsigned long long)(r.start > 0 ? r.start : 0));
+        if (r.status == RS_OK) {
+            const uint32_t slot = atomicAdd(n_frames, 1u);
+            if (slot < frame_cap) {
+                frames[slot] = r;
+                for (int a = 0; a < RS_MAX_ANTENNAS; a++) {
+                    chan[(size_t)slot * 2 * RS_MAX_ANTENNAS + a] = h[a];
+                    chan[(size_t)slot * 2 * RS_MAX_ANTENNAS + RS_MAX_ANTENNAS + a] = w[a];
+                }
+            }
         }
     }
 }
@@ -508,6 +709,40 @@ __global__ void rs_assemble_kernel(const float2 *__restrict__ iq, size_t stride,
                 float sn, cs;
                 sincospif(-2.0f * (float)t, &sn, &cs);
                 o[r] = n < n_items ? cmul(x[n], make_float2(cs, sn)) : make_float2(0.f, 0.f);
+            }
+        }
+    }
+}
+
+// ... of receivers with m antennas: window sample n of frame f (slot frames[idx[f]], or f) is
+// sum_a w_a x_a[n] de-rotated by the frame's CFO, rows fr.stream * m + a, w_a = chan[slot][4 + a] (rs_sync_antennas_kernel)
+__global__ void rs_assemble_antennas_kernel(const float2 *__restrict__ iq, size_t stride, long long n_items, uint32_t m,
+                                            const RsFrame *__restrict__ frames, const float2 *__restrict__ chan, uint32_t n_frames,
+                                            const uint32_t *__restrict__ idx, uint32_t first, const uint32_t *__restrict__ offs,
+                                            uint32_t off_base, const uint32_t *__restrict__ cnts, uint32_t sps, float2 *__restrict__ out) {
+    for (uint32_t f = blockIdx.x; f < n_frames; f += gridDim.x) {
+        const uint32_t slot = idx ? idx[f] : f;
+        const RsFrame fr = frames[slot];
+        const uint32_t off = offs ? offs[f] - off_base : f * 8u, cnt = cnts ? cnts[f] : 8u;
+        const float2 *x = iq + (size_t)fr.stream * m * stride;
+        float2 w[RS_MAX_ANTENNAS];
+        for (int a = 0; a < RS_MAX_ANTENNAS; a++) w[a] = chan[(size_t)slot * 2 * RS_MAX_ANTENNAS + RS_MAX_ANTENNAS + a];
+        const double rev = (double)fr.cfo_bins / (double)sps;
+        for (uint32_t k = 0; k < cnt; k++) {
+            const long long ws = rs_sym(fr.start, rs_data_j((long long)first + k), sps, fr.sfo_ppm);
+            float2 *o = out + ((size_t)off + k) * sps;
+            for (uint32_t r = threadIdx.x; r < sps; r += blockDim.x) {
+                const long long n = ws + (long long)r;
+                if (n >= n_items) { o[r] = make_float2(0.f, 0.f); continue; }
+                double t = rev * (double)n;
+                t -= floor(t);
+                float sn, cs;
+                sincospif(-2.0f * (float)t, &sn, &cs);
+                float2 y = make_float2(0.f, 0.f);
+#pragma unroll
+                for (int a = 0; a < RS_MAX_ANTENNAS; a++)
+                    if (a < (int)m) y = cfma(w[a], x[(size_t)a * stride + n], y);
+                o[r] = cmul(y, make_float2(cs, sn));
             }
         }
     }

@@ -181,7 +181,7 @@ class decoder:
                               ("sfo_ppm", "<f4")])       # struct lora_b200_rx_info
 
     def receive(self, iq, n_items=None, stride_items=None, host=None, sync_word=0x12, implicit_len=0, min_preamble=0,
-                max_cfo_hz=0.0, sfo_ppm=0.0, carrier_hz=0.0, soft=False):
+                max_cfo_hz=0.0, sfo_ppm=0.0, carrier_hz=0.0, soft=False, antennas=1):
         """The dechirp-synchronised receiver (lora_b200_receive): decodes frames below the noise floor.  ``iq`` as for
         work_batch (host ndarray [n_streams, n_items] or a device tensor / pointer).  Returns (consumed, frames, info):
         consumed[s] = where stream s must be re-presented from, frames = FRAME_DTYPE records, info = RX_INFO_DTYPE records
@@ -189,7 +189,11 @@ class decoder:
         one per frame.  Clock offset of a frame: sfo_ppm, plus its CFO / carrier_hz when carrier_hz (the channel's RF
         frequency) is given -- one crystal sets a radio's carrier and its sample clock.  soft: decode every code word from
         its bits' LLRs (the spectrum of each data window, demod_llr) to the most likely nibble, instead of from the argmax.
-        ``self.header_drops`` counts the explicit headers of the call whose checksum failed."""
+        ``self.header_drops`` counts the explicit headers of the call whose checksum failed.
+        antennas = M (1..4, dividing n_streams): rows g M .. g M + M - 1 are the phase-coherent antennas of receiver g
+        (lora_b200_receive_antennas): combined screen and synchronisation, maximum-ratio-combined data windows; consumed has
+        one entry per receiver, frames and info carry stream = g and the combined SNR, and rx_channels_last() gives each
+        frame's channel estimates."""
         if isinstance(iq, np.ndarray):
             x = np.ascontiguousarray(iq, dtype=np.complex64)
             assert x.ndim == 2 and x.shape[0] == self.n_streams
@@ -203,15 +207,31 @@ class decoder:
                 stride_items = n_items
         p = N.RxParams(sync_word=int(sync_word) & 0xFF, implicit_len=int(implicit_len), min_preamble=int(min_preamble),
                        max_cfo_hz=float(max_cfo_hz), sfo_ppm=float(sfo_ppm), carrier_hz=float(carrier_hz), soft=int(soft))
-        consumed = np.zeros(self.n_streams, dtype=np.uint64)
-        N.check(self._L.lora_b200_receive(self._h, ptr, int(n_items), int(stride_items), host, C.byref(p),
-                                          consumed.ctypes.data_as(C.POINTER(C.c_size_t))), "lora_b200_receive")
+        m = int(antennas)
+        consumed = np.zeros(max(self.n_streams // m, 1) if m > 0 else 1, dtype=np.uint64)
+        cptr = consumed.ctypes.data_as(C.POINTER(C.c_size_t))
+        if m == 1:
+            N.check(self._L.lora_b200_receive(self._h, ptr, int(n_items), int(stride_items), host, C.byref(p), cptr), "lora_b200_receive")
+        else:
+            N.check(self._L.lora_b200_receive_antennas(self._h, ptr, int(n_items), int(stride_items), host, m, C.byref(p), cptr),
+                    "lora_b200_receive_antennas")
         iptr, drops = C.c_void_p(0), C.c_uint32(0)
         n = int(self._L.lora_b200_rx_info_last(self._h, C.byref(iptr), C.byref(drops)))
         info = (np.frombuffer(C.string_at(iptr.value, n * self.RX_INFO_DTYPE.itemsize), dtype=self.RX_INFO_DTYPE) if n
                 else np.zeros(0, self.RX_INFO_DTYPE))
         self.header_drops = int(drops.value)
         return consumed.astype(np.int64), self.frames_last(), info
+
+    def rx_channels_last(self) -> np.ndarray:
+        """[n_frames, M] complex64: each antenna's channel estimate for every frame of the last receive(..., antennas=M) call,
+        parallel to its frames (lora_b200_rx_channels_last): the mean preamble peak over (1 + j) sps, the amplitude per
+        sample with a phase reference common to the frame's antennas.  Empty after a one-antenna call."""
+        ptr, m = C.c_void_p(0), C.c_uint32(0)
+        n = int(self._L.lora_b200_rx_channels_last(self._h, C.byref(ptr), C.byref(m)))
+        m = max(int(m.value), 1)
+        if n == 0:
+            return np.zeros((0, m), np.complex64)
+        return np.frombuffer(C.string_at(ptr.value, n * m * 8), dtype=np.complex64).reshape(n, m).copy()
 
     def _emit_stdout(self, stream):
         if self.quiet:
@@ -267,6 +287,14 @@ class decoder:
         """K1 on device memory: dechirp + FFT + argmax of n_symbols aligned windows."""
         N.check(self._L.lora_b200_demod_fft_dev(self._h, _dev_ptr(iq_dev), int(n_symbols), _dev_ptr(bins_dev),
                                                _dev_ptr(mags_dev), int(cuda_stream)), "lora_b200_demod_fft_dev")
+
+    def demod_fft_antennas(self, iq_dev, n_groups, n_antennas, n_symbols, row_stride, bins_dev, mags_dev, cuda_stream=0):
+        """The combined screen of the several-antenna receiver (lora_b200_demod_fft_antennas_dev): n_groups groups of n_antennas
+        rows (row_stride items apart) of n_symbols aligned windows; bins_dev / mags_dev[g * n_symbols + i] = the first argmax
+        of sum_a |tmp_a|^2 over the group's windows i and its square root."""
+        N.check(self._L.lora_b200_demod_fft_antennas_dev(self._h, _dev_ptr(iq_dev), int(n_groups), int(n_antennas), int(n_symbols),
+                                                        int(row_stride), _dev_ptr(bins_dev), _dev_ptr(mags_dev), int(cuda_stream)),
+                "lora_b200_demod_fft_antennas_dev")
 
     def demod_llr(self, iq_dev, n_symbols, llrs_dev, bins_dev=None, reduced=False, cuda_stream=0):
         """Soft output of n_symbols aligned windows (lora_b200_demod_llr_dev): llrs_dev[i * ppm + j] = the max-log LLR of bit

@@ -9,10 +9,17 @@ import numpy as np
 from .decoder import decoder
 
 
+class _DeviceRow:
+    """A zero-copy view of n complex64 samples at a device address, for torch.as_tensor."""
+
+    def __init__(self, ptr, n):
+        self.__cuda_array_interface__ = {"shape": (int(n),), "typestr": "<c8", "data": (int(ptr), False), "version": 3}
+
+
 class lora_receiver:
     def __init__(self, samp_rate, center_freq, channel_list, bandwidth, sf, implicit, cr, crc, reduced_rate=False,
                  conj=False, decimation=1, disable_channelization=False, disable_drift_correction=False, cfo_feedback=False,
-                 sync="reference", sync_word=0x12, implicit_len=0, clock_from_carrier=False, soft=False, **decoder_kw):
+                 sync="reference", sync_word=0x12, implicit_len=0, clock_from_carrier=False, soft=False, antennas=1, **decoder_kw):
         self.samp_rate, self.center_freq, self.channel_list = samp_rate, center_freq, list(channel_list)
         self.bandwidth, self.sf, self.implicit, self.cr, self.crc = bandwidth, sf, implicit, cr, crc
         self.decimation, self.conj = decimation, conj
@@ -31,22 +38,32 @@ class lora_receiver:
         if soft and sync != "dechirp":
             raise ValueError("soft needs sync='dechirp' (the reference state machine makes hard decisions)")
         self.soft = bool(soft)
+        # antennas = M: run() takes an (M, n) capture of M phase-coherent antennas (one LO, one sample clock) and the dechirp
+        # receiver combines them (decoder.receive(..., antennas=M)); with the channelizer every antenna gets its own
+        # channelizer, which filters and rotates it exactly as the others, so the combining weights stay meaningful
+        if antennas != 1 and sync != "dechirp":
+            raise ValueError("antennas needs sync='dechirp' (the reference state machine has one input)")
+        self.antennas = int(antennas)
         self.disable_channelization = disable_channelization
         self.disable_drift_correction = disable_drift_correction
         self.channelizer = None
         if not disable_channelization:
             # python/lora_receiver.py:52: lora.channelizer(samp_rate, center_freq, channel_list, bandwidth, decimation)
             from .channelizer import channelizer
-            self.channelizer = channelizer(samp_rate, center_freq, self.channel_list, bandwidth, decimation,
-                                           device=decoder_kw.get("device", -1))
+            self.channelizers = [channelizer(samp_rate, center_freq, self.channel_list, bandwidth, decimation,
+                                             device=decoder_kw.get("device", -1)) for _ in range(self.antennas)]
+            self.channelizer = self.channelizers[0]
             if conj:                                 # channelizer -> conjugate_cc -> decoder (:62-63,70-75), conjugated on the device
-                self.channelizer.set_conjugate(True)
+                for ch in self.channelizers:
+                    ch.set_conjugate(True)
         if disable_channelization and decimation != 1:
             raise NotImplementedError("fractional_resampler_cc path (python/lora_receiver.py:58-61) is host plumbing, not built")
         # python/lora_receiver.py:53
+        if self.antennas != 1:
+            decoder_kw.setdefault("n_streams", self.antennas)
         self.decoder = decoder(samp_rate / decimation, bandwidth, sf, implicit, cr, crc, reduced_rate,
                                disable_drift_correction, **decoder_kw)
-        if self.decoder.n_streams != 1:
+        if self.decoder.n_streams != self.antennas:
             raise ValueError("lora_receiver feeds one channel (channel_list[0]) to one decoder stream, like the reference; "
                              "use decoder(..., n_streams=N).work_batch for many channels")
         self.frames = self.decoder.frames            # hier-block message port 'frames' (:56,:68)
@@ -74,6 +91,8 @@ class lora_receiver:
         """Whole capture through (channelizer ->) [conj ->] decoder.  With the channelizer the filtered IQ
         stays in device memory: the decoder consumes the channelizer's output buffer directly.  Only
         channel_list[0] reaches the decoder, as in the reference (lib/channelizer_impl.cc:47,56-57)."""
+        if self.antennas != 1:
+            return self._run_antennas(samples)
         if self.channelizer is None:
             if self.sync == "dechirp":
                 x = np.ascontiguousarray(self._front(samples), np.complex64)
@@ -102,7 +121,27 @@ class lora_receiver:
                 self.channelizer.apply_cfo(cfo)      # channelizer_impl::apply_cfo, lib/channelizer_impl.cc:68-71
         return pos_out * self.decimation
 
-    def _run_dechirp(self, src, n_out, limit):
+    def _run_antennas(self, samples):
+        """An (M, n) capture: each row through its own channelizer, the M filtered rows gathered into one device buffer (device
+        to device copies), or the rows straight through; then the dechirp receiver over the M rows as one receiver."""
+        x = np.asarray(samples, dtype=np.complex64)
+        if x.ndim != 2 or x.shape[0] != self.antennas:
+            raise ValueError(f"antennas={self.antennas} needs an ({self.antennas}, n) capture, got shape {x.shape}")
+        limit = int(self.decoder.cfg.max_items_per_call or (1 << 20))
+        if self.channelizer is None:
+            return self._run_dechirp(np.ascontiguousarray(self._front(x)), x.shape[1], limit)
+        import torch
+        x = x[:, : (x.shape[1] // self.decimation) * self.decimation]
+        dev = torch.device("cuda", self.decoder.cfg.device if self.decoder.cfg.device >= 0 else torch.cuda.current_device())
+        n_out = [ch.work(row) for ch, row in zip(self.channelizers, x)]
+        rows = torch.empty((self.antennas, n_out[0]), dtype=torch.complex64, device=dev)
+        torch.cuda.synchronize(dev)                  # (the channelizers run on their own streams)
+        for a, ch in enumerate(self.channelizers):
+            rows[a].copy_(torch.as_tensor(_DeviceRow(ch.output_ptr(0)[0], n_out[0]), device=dev))
+        torch.cuda.synchronize(dev)                  # (receive reads device input on its own stream)
+        return self._run_dechirp(int(rows.data_ptr()), n_out[0], limit, stride=n_out[0]) * self.decimation
+
+    def _run_dechirp(self, src, n_out, limit, stride=None):
         """decoder.receive over the channelizer's device output (src: its address) or a host capture (src: ndarray), call by
         call under the consumed rule; every frame is published on the 'frames' port.  Returns the samples consumed.
         A call that consumes nothing while samples remain holds a frame longer than its chunk: the next call presents a
@@ -113,9 +152,13 @@ class lora_receiver:
             carrier = float(self.center_freq if self.channelizer is None else self.channel_list[0])
         while pos < n_out:
             n = min(n, n_out - pos)
-            part = src[None, pos: pos + n] if isinstance(src, np.ndarray) else src + 8 * pos
-            c, frames, _ = self.decoder.receive(part, n_items=n, stride_items=n, host=0, sync_word=self.sync_word,
-                                                implicit_len=self.implicit_len, carrier_hz=carrier, soft=self.soft)
+            if isinstance(src, np.ndarray):
+                part = src[None, pos: pos + n] if src.ndim == 1 else src[:, pos: pos + n]
+            else:
+                part = src + 8 * pos
+            c, frames, _ = self.decoder.receive(part, n_items=n, stride_items=n if stride is None else stride, host=0, sync_word=self.sync_word,
+                                                implicit_len=self.implicit_len, carrier_hz=carrier, soft=self.soft,
+                                                antennas=self.antennas)
             for f in frames:
                 self.decoder._publish(int(f["stream"]), bytes(f["bytes"][: int(f["len"])]))
             c = int(c[0])

@@ -141,6 +141,13 @@ int lora_b200_demod_llr_dev(lora_b200_decoder *d, const void *iq, size_t n_symbo
  * (float2[n]) and energy are device pointers, pos, cfo_bins, up and bin host arrays; returns when the results are written. */
 int lora_b200_rs_window_dev(lora_b200_decoder *d, const void *iq, size_t n_items, size_t n, const int64_t *pos, const float *cfo_bins,
                             const int32_t *up, const int32_t *bin, void *out, float *energy);
+/* The combined screen of the dechirp receiver with several antennas (lora_b200_receive_antennas) on its own, so that it can be
+ * held to a reference: n_groups groups of n_antennas (1..4) rows, row r = iq + r * row_stride_items, each holding n_symbols
+ * aligned windows of sps samples.  For window i of group g, with tmp_a the kept bins of lora_b200_demod_fft_dev's spectrum of
+ * antenna a's window, P[k] = sum_a |tmp_a[k]|^2: bins[g * n_symbols + i] = the first argmax of P, mags[..] = sqrt(P[bin]).
+ * iq 16-byte aligned, row_stride_items even and >= n_symbols * sps; device pointers, async on cuda_stream. */
+int lora_b200_demod_fft_antennas_dev(lora_b200_decoder *d, const void *iq, uint32_t n_groups, uint32_t n_antennas, size_t n_symbols,
+                                     size_t row_stride_items, uint32_t *bins, float *mags, void *cuda_stream);
 /* SDR-native ingest: iq_sc16 = interleaved little-endian int16 I/Q (what a USRP / file source delivers before the
  * host-side conversion to gr_complex); the device converts x * scale right after the copy, so PCIe moves 4 instead of
  * 8 bytes per sample.  Results equal lora_b200_demod_fft_host on the host-converted buffer bit for bit. */
@@ -279,7 +286,8 @@ size_t lora_b200_frames_last(lora_b200_decoder *d, const lora_b200_frame **frame
  * fixed per frame, which holds while ppm x frame length stays below about a quarter chip.  sfo_ppm must be finite within
  * +-500 and carrier_hz 0 or finite and above the sample rate, else LORA_B200_EINVAL.
  * Limits: |CFO| <= max_cfo_hz <= BW / 4, no blind drift estimation (the clock offset is given or follows the CFO), data
- * windows placed to the nearest sample, one frame at a time per stream, the decoder's SF only.  The stream state machine's
+ * windows placed to the nearest sample, one frame at a time per stream, the decoder's SF only, several antennas per receiver
+ * through lora_b200_receive_antennas (below).  The stream state machine's
  * per-stream state is not touched.
  * Streaming: a frame is published only when its last sample lies inside the call; consumed[s] is where the caller must
  * re-present stream s from: the earliest preamble whose frame was incomplete, else n_items minus a guard of
@@ -316,6 +324,23 @@ int lora_b200_receive(lora_b200_decoder *d, const void *iq, size_t n_items, size
 /* per published frame of the last lora_b200_receive call, parallel to lora_b200_frames_last; *hdr_drops (may be NULL) =
  * synchronised explicit-header frames dropped for a failed header checksum */
 size_t lora_b200_rx_info_last(lora_b200_decoder *d, const lora_b200_rx_info **info, uint32_t *hdr_drops);
+/* The dechirp receiver on several phase-coherent antennas per receiver (one LO and one sample clock, e.g. both RX channels of
+ * a B210): rows g * n_antennas .. g * n_antennas + n_antennas - 1 of iq ([n_streams][n_items], as lora_b200_receive) are
+ * the antennas of receiver g.  Timing and CFO are common to a receiver's antennas: the screen takes the argmax of the
+ * combined spectrum sum_a |tmp_a[k]|^2, the synchroniser sums its statistics over the antennas, and each frame's data
+ * windows are y = sum_a w_a x_a with maximum-ratio weights w_a = conj(h_a) / noise_a (scaled to sum |w_a|^2 = 1) from the
+ * per-antenna channel h_a and noise power measured on the preamble; y then goes through the demodulators, soft decisions and
+ * decoding of lora_b200_receive unchanged.  Receiver g gets one consumed[g] (consumed has n_streams / n_antennas entries),
+ * frames and rx_info with stream == g, and snr_db = the combined (post-MRC) SNR, the sum of the antennas' SNRs.
+ * n_antennas must be 1..4 and divide n_streams, else LORA_B200_EINVAL; everything else as lora_b200_receive.
+ * n_antennas == 1 is lora_b200_receive. */
+int lora_b200_receive_antennas(lora_b200_decoder *d, const void *iq, size_t n_items, size_t stride_items, int host_ptr,
+                               uint32_t n_antennas, const lora_b200_rx_params *p, size_t *consumed /* [n_streams / n_antennas] */);
+/* per published frame of the last receive_antennas call, parallel to lora_b200_frames_last: n_antennas complex channel
+ * estimates (float2: re, im), in row order -- the mean preamble peak of each antenna over (1 + j) sps, the amplitude per
+ * sample with a phase reference common to the frame's antennas.  *n_antennas (may be NULL) = that call's n_antennas.
+ * Returns the number of frames; 0 after lora_b200_receive, after n_antennas == 1 (no weights to form) and after work calls. */
+size_t lora_b200_rx_channels_last(lora_b200_decoder *d, const float **h, uint32_t *n_antennas);
 /* current state of a stream (LORA_B200_DETECT ...) */
 int lora_b200_stream_state(lora_b200_decoder *d, uint32_t stream);
 /* N4 (SURVEY.md 8f): the CFO estimate the reference computes in experimental_determine_cfo (lib/decoder_impl.cc:730-738:
