@@ -31,7 +31,8 @@ class TxFrame(C.Structure):
 
 class RxParams(C.Structure):
     """struct lora_b200_rx_params (include/lora_b200.h)."""
-    _fields_ = [("sync_word", C.c_uint8), ("soft", C.c_uint8), ("reserved0", C.c_uint8 * 2), ("implicit_len", C.c_uint32),
+    _fields_ = [("sync_word", C.c_uint8), ("soft", C.c_uint8), ("crc_list", C.c_uint8), ("reserved0", C.c_uint8 * 1),
+                ("implicit_len", C.c_uint32),
                 ("min_preamble", C.c_uint32),
                 ("max_cfo_hz", C.c_float), ("sfo_ppm", C.c_float), ("reserved1", C.c_uint32), ("carrier_hz", C.c_double)]
 
@@ -40,6 +41,7 @@ FRAME_CB = C.CFUNCTYPE(None, C.c_void_p, C.c_uint32, C.POINTER(C.c_uint8), C.c_s
 
 OK, EINVAL, ECUDA, ENOMEM, EUNSUPPORTED, EOVERFLOW = 0, -1, -2, -3, -4, -5
 DEMOD_GRADIENT, DEMOD_FFT = 0, 1
+CRC_NONE, CRC_OK, CRC_BAD, CRC_RECOVERED = 0, 1, 2, 3      # lora_b200_frames_crc_last
 STATES = ["DETECT", "SYNC", "FIND_SFD", "PAUSE", "DECODE_HEADER", "DECODE_PAYLOAD", "STOP"]
 
 # every symbol include/lora_b200.h declares: name -> (restype, argtypes)
@@ -83,6 +85,7 @@ SIGNATURES = {
     "lora_b200_work_batch_sc16": (_i, [_vp, _vp, C.c_float, _sz, _sz, _i, C.POINTER(_sz), FRAME_CB, _vp]),
     "lora_b200_work_batch_sc8": (_i, [_vp, _vp, C.c_float, _sz, _sz, _i, C.POINTER(_sz), FRAME_CB, _vp]),
     "lora_b200_frames_last": (_sz, [_vp, C.POINTER(_vp)]),
+    "lora_b200_frames_crc_last": (_sz, [_vp, C.POINTER(_vp)]),
     "lora_b200_receive": (_i, [_vp, _vp, _sz, _sz, _i, C.POINTER(RxParams), C.POINTER(_sz)]),
     "lora_b200_rx_info_last": (_sz, [_vp, C.POINTER(_vp), C.POINTER(C.c_uint32)]),
     "lora_b200_receive_antennas": (_i, [_vp, _vp, _sz, _sz, _i, _u32, C.POINTER(RxParams), C.POINTER(_sz)]),

@@ -305,12 +305,58 @@ void rs_host_llrs(const RsHostOps &o, const lb::RsFrame &r, uint32_t first, uint
     lb_k1_llr_emulate_osr((int)o.sf, (int)o.osr, w.data(), cnt, o.down, o.tw, reduced, llr.data(), nullptr);
 }
 
+// rs_crc_list_kernel's procedure as plain loops: the whole list sorted, every subset in turn.  Corrects hb[8] and pb[n_payload]
+// in place; returns 1 when the frame was recovered.
+int rs_host_crc_list(const lb::RxParams &rp, uint8_t phdr1, uint32_t implicit_len, uint32_t K, int32_t n_payload, const float *hllr,
+                     const float *llr, uint32_t *hb, uint32_t *pb) {
+    const lb::RsCrcFrame cf = lb::rs_crc_frame(rp, phdr1, hb, n_payload, implicit_len);
+    if (cf.L == 0u || cf.n_slots > lb::RS_CRC_MAX_SLOTS || cf.h + 2u * (cf.L + 2u) > cf.n_slots) return 0;
+    std::vector<uint8_t> nib(cf.n_slots), alt(cf.n_slots);
+    std::vector<float> gap(cf.n_slots);
+    for (uint32_t q = 0; q < cf.n_slots; q++) {
+        const lb::RsSoftPick r = lb::rs_crc_pick(cf, hllr, llr, q);
+        nib[q] = (uint8_t)r.s1; alt[q] = (uint8_t)r.s2; gap[q] = r.gap;
+    }
+    const uint32_t S0 = lb::rs_crc_syndrome(cf, nib.data());
+    if (S0 == 0u) return 0;
+    std::vector<unsigned long long> cand;
+    for (uint32_t q = 0; q < cf.n_slots; q++)
+        if (lb::rs_crc_candidate(cf, q)) cand.push_back(lb::rs_crc_key(gap[q], q));
+    std::sort(cand.begin(), cand.end());
+    const uint32_t n = std::min<uint32_t>(K, (uint32_t)cand.size());
+    uint32_t lq[lb::RS_CRC_MAX_LIST], delta[lb::RS_CRC_MAX_LIST];
+    float lgap[lb::RS_CRC_MAX_LIST];
+    for (uint32_t j = 0; j < n; j++) {
+        lq[j] = (uint32_t)cand[j];
+        lgap[j] = gap[lq[j]];
+        delta[j] = lb::rs_crc_delta(cf.L, lq[j] - cf.h, nib[lq[j]] ^ alt[lq[j]]);
+    }
+    unsigned long long best = ~0ull;
+    for (uint32_t mask = 1; mask < (1u << n); mask++) {
+        uint32_t syn = 0;
+        for (uint32_t j = 0; j < n; j++)
+            if (mask >> j & 1u) syn ^= delta[j];
+        if (syn == S0) best = std::min(best, lb::rs_crc_key(lb::rs_crc_cost(lgap, mask), mask));
+    }
+    if (best == ~0ull) return 0;
+    const uint32_t mask = (uint32_t)best;
+    for (uint32_t j = 0; j < n; j++)
+        if (mask >> j & 1u) nib[lq[j]] = alt[lq[j]];
+    for (uint32_t j = 0; j < n; j++) {
+        if (!(mask >> j & 1u)) continue;
+        uint32_t *out = lb::rs_crc_block_out(cf, lq[j], hb, pb);
+        for (uint32_t i = 0; i < lb::rs_crc_block_bins(cf, lq[j]); i++) out[i] = lb::rs_crc_block_bin(cf, nib.data(), lq[j], i);
+    }
+    return 1;
+}
+
 // the receive path of lb_emul_rx_receive_osr (m = 1) and lb_emul_rx_receive_antennas (m rows of n_items each, x[a * n_items
 // ..]); with several antennas chan[f * m ..] gets each synchronised frame's channel estimates h (may be NULL)
 uint32_t rs_host_receive(const float2 *x, size_t n_items, uint32_t m, const float2 *down, const float2 *up, const float2 *tw, uint32_t sf,
                          uint32_t osr, uint32_t cr, int implicit, int crc, int reduced_rate, uint32_t sync_word, uint32_t implicit_len,
                          uint32_t min_preamble, float sfo_ppm, double carrier_hz, int soft, long long *start, float *cfo_bins,
-                         float *snr_db, int32_t *status, float *sfo, uint8_t *payload, uint32_t *len, float2 *chan, uint32_t cap) {
+                         float *snr_db, int32_t *status, float *sfo, uint8_t *payload, uint32_t *len, float2 *chan, uint32_t cap,
+                         uint32_t crc_list = 0, uint8_t *crc_status = nullptr) {
     if (osr != 8u && osr != 2u) return 0;
     const uint32_t N = 1u << sf, sps = osr * N;
     const double bin_hz = 125e3 / N;
@@ -357,16 +403,17 @@ uint32_t rs_host_receive(const float2 *x, size_t n_items, uint32_t m, const floa
             od.x = y.data();
         }
         start[nf] = r.start; cfo_bins[nf] = r.cfo_bins; snr_db[nf] = r.snr_db; status[nf] = 2; len[nf] = 0;
+        if (crc_status) crc_status[nf] = LORA_CRC_NONE;
         if (sfo) sfo[nf] = r.sfo_ppm;
         // end of the window of data symbol n - 1
         auto data_end = [&](long long n) { return lb::rs_sym(r.start, lb::rs_data_j(n - 1), sps, r.sfo_ppm) + (long long)sps; };
         if (r.status == lb::RS_OK && data_end(8) <= (long long)n_items) {
             std::vector<uint32_t> hb, pb;
-            std::vector<float> llr;
+            std::vector<float> llr, hllr;
             if (soft) {
                 hb.resize(8);
-                rs_host_llrs(od, r, 0, 8, true, llr);
-                lb::rs_soft_header(lb::rs_code(rp, phdr1), llr.data(), hb.data(), nullptr);
+                rs_host_llrs(od, r, 0, 8, true, hllr);
+                lb::rs_soft_header(lb::rs_code(rp, phdr1), hllr.data(), hb.data(), nullptr);
             } else {
                 rs_host_bins(od, r, 0, 8, hb);
             }
@@ -374,19 +421,27 @@ uint32_t rs_host_receive(const float2 *x, size_t n_items, uint32_t m, const floa
             const int32_t np = lb::rs_header(&st, rp, phdr1, hb.data(), implicit_len);
             if (np < 0) status[nf] = 1;
             else if (data_end(8ll + np) <= (long long)n_items) {
+                int recovered = 0;
                 if (soft) {
                     pb.resize((size_t)np);
                     rs_host_llrs(od, r, 8, (uint32_t)np, reduced_rate != 0, llr);
                     lb::rs_soft_payload(rp, phdr1, hb.data(), np, implicit_len, llr.data(), pb.data());
+                    if (crc_list) recovered = rs_host_crc_list(rp, phdr1, implicit_len, crc_list, np, hllr.data(), llr.data(), hb.data(), pb.data());
                 } else {
                     rs_host_bins(od, r, 8, (uint32_t)np, pb);
                 }
                 lb::RxFrameRec fr;
                 lb::rs_frame(&st, rp, pb.data(), np, &fr, 0, nf, 1.0f);
                 const uint32_t nd = lb::decode_len_bytes(lb::decode_len_words(fr.n_cw, 0), fr.cr);
+                std::vector<uint8_t> bytes(fr.payload_length);
+                for (uint32_t i = 0; i < fr.payload_length; i++) bytes[i] = i < nd ? lb::decode_byte(fr.cw, fr.n_cw, 0, fr.cr, i) : 0;
                 len[nf] = std::min<uint32_t>(fr.payload_length, 256u);
-                for (uint32_t i = 0; i < len[nf]; i++) payload[(size_t)nf * 256 + i] = i < nd ? lb::decode_byte(fr.cw, fr.n_cw, 0, fr.cr, i) : 0;
+                std::copy(bytes.begin(), bytes.begin() + len[nf], payload + (size_t)nf * 256);
                 status[nf] = 0;
+                if (crc_status) {
+                    const uint32_t c = lb::lb_crc_check(bytes.data(), fr.payload_length, fr.cr, (fr.phdr[1] >> 4) & 1u);
+                    crc_status[nf] = (uint8_t)(c == LORA_CRC_OK && recovered ? LORA_CRC_RECOVERED : c);
+                }
             }
         }
         nf++;
@@ -427,6 +482,34 @@ uint32_t lb_emul_rx_receive_antennas(const float2 *x, size_t n_items, uint32_t m
     return rs_host_receive(x, n_items, m, down, up, tw, sf, osr, cr, implicit, crc, reduced_rate, sync_word, implicit_len, min_preamble,
                            sfo_ppm, carrier_hz, soft, start, cfo_bins, snr_db, status, sfo, payload, len, (float2 *)chan, cap);
 }
+
+// lb_emul_rx_receive_antennas with CRC-aided list decoding (crc_list = K as lora_b200_rx_params.crc_list; 0 = off, any K
+// needs soft) and each synchronised frame's payload CRC status in crc_status[f] (LORA_B200_CRC_*; NONE when not published).
+uint32_t lb_emul_rx_receive_crc(const float2 *x, size_t n_items, uint32_t m, const float2 *down, const float2 *up, const float2 *tw,
+                                uint32_t sf, uint32_t osr, uint32_t cr, int implicit, int crc, int reduced_rate, uint32_t sync_word,
+                                uint32_t implicit_len, uint32_t min_preamble, float sfo_ppm, double carrier_hz, int soft, uint32_t crc_list,
+                                long long *start, float *cfo_bins, float *snr_db, int32_t *status, float *sfo, uint8_t *payload,
+                                uint32_t *len, uint8_t *crc_status, uint32_t cap) {
+    if (m < 1 || m > (uint32_t)lb::RS_MAX_ANTENNAS || crc_list > lb::RS_CRC_MAX_LIST || (crc_list && !soft)) return 0;
+    return rs_host_receive(x, n_items, m, down, up, tw, sf, osr, cr, implicit, crc, reduced_rate, sync_word, implicit_len, min_preamble,
+                           sfo_ppm, carrier_hz, soft, start, cfo_bins, snr_db, status, sfo, payload, len, nullptr, cap, crc_list, crc_status);
+}
+
+// rs_crc_list_kernel on one frame's given LLRs (header block hllr[8][sf - 2], payload blocks llr[n_payload][ppm]) and corrected
+// bins (hbins[8], pbins[n_payload], as the soft decoder left them; corrected in place): 1 when the frame was recovered
+int lb_emul_rx_crc_list(uint32_t sf, uint32_t cr, int implicit, int crc, int reduced_rate, uint32_t implicit_len, uint32_t crc_list,
+                        int32_t n_payload, const float *hllr, const float *llr, uint32_t *hbins, uint32_t *pbins) {
+    lb::RxParams rp;
+    memset(&rp, 0, sizeof rp);
+    rp.sf = sf; rp.n_bins = 1u << sf; rp.n_bins_hdr = rp.n_bins / 4; rp.sps = 8u << sf; rp.decim = 8; rp.implicit = implicit;
+    rp.reduced_rate = reduced_rate;
+    const uint8_t phdr1 = (uint8_t)(((cr & 7u) << 5) | (crc ? 1u << 4 : 0u));
+    return rs_host_crc_list(rp, phdr1, implicit_len, std::min<uint32_t>(crc_list, lb::RS_CRC_MAX_LIST), n_payload, hllr, llr, hbins, pbins);
+}
+
+// the payload CRC status (LORA_B200_CRC_NONE / _OK / _BAD) of a published record (lora_crc.h)
+uint32_t lb_emul_crc_record_status(const uint8_t *rec, uint32_t len) { return lb::lb_crc_record_status(rec, len); }
+uint32_t lb_emul_crc16(const uint8_t *b, uint32_t n) { return lb::lb_crc16(b, n); }
 
 // lb_emul_rx_receive_osr at fs/bw = 8 (fs = 1 MHz)
 uint32_t lb_emul_rx_receive_soft(const float2 *x, size_t n_items, const float2 *down, const float2 *up, const float2 *tw, uint32_t sf,

@@ -131,6 +131,8 @@ struct lora_b200_decoder : A1Params {
     DeviceBuffer<float2> d_rs_stage, d_rs_win;
     DeviceBuffer<uint32_t> d_rs_bins[2], d_rs_hbins, d_rs_pbins, d_rs_ncand, d_rs_nframes, d_rs_tab;
     DeviceBuffer<float> d_rs_mags[2], d_rs_llr;
+    DeviceBuffer<float> d_rs_hllr;        // the header round's LLRs, kept for list decoding (rx_params.crc_list)
+    DeviceBuffer<uint8_t> d_rs_recovered; // per published frame: recovered by rs_crc_list_kernel
     DeviceBuffer<RsCand> d_rs_cands;
     DeviceBuffer<long long> d_rs_dropped;
     DeviceBuffer<unsigned long long> d_rs_hold;
@@ -144,6 +146,8 @@ struct lora_b200_decoder : A1Params {
     DeviceBuffer<float2> d_rs_chan;
     std::vector<float2> rs_chan;
     uint32_t rs_chan_m = 1;
+    // lora_b200_frames_crc_last: the frames of the last call that list decoding recovered (empty: none), and the statuses
+    std::vector<uint8_t> rs_recovered, crc_status;
 };
 
 namespace {
@@ -481,6 +485,7 @@ int rx_finish(lora_b200_decoder *d, uint32_t stream_base, uint32_t n_launch, siz
     d->h_sorted.resize(n_frames);
     d->rs_info.clear();                           // (lora_b200_rx_info_last describes lora_b200_receive calls only)
     d->rs_chan.clear();
+    d->rs_recovered.clear();
     for (uint32_t k = 0; k < n_frames; k++) {
         const RxFrameOut &f = d->h_frames[order[k]];
         d->h_sorted[k] = f;
@@ -931,6 +936,7 @@ int lora_b200_reset(lora_b200_decoder *d) {
     CU(cudaMemset(d->d_consumed, 0, sizeof(unsigned long long) * d->cfg.n_streams));
     if (d->d_trace_n) CU(cudaMemset(d->d_trace_n, 0, sizeof(uint32_t) * d->cfg.n_streams));
     d->h_sorted.clear();
+    d->rs_recovered.clear();
     for (auto &so : d->stdout_last) so.clear();
     return LORA_B200_OK;
 }
@@ -1201,6 +1207,8 @@ static int rs_receive(lora_b200_decoder *d, const void *iq, size_t n_items, size
     if (P.carrier_hz != 0.0 && !(std::isfinite(P.carrier_hz) && P.carrier_hz > d->samples_per_second))
         return fail(LORA_B200_EINVAL, "carrier_hz must be 0 or above the sample rate %g, got %g", d->samples_per_second, P.carrier_hz);
     if (P.soft > 1u) return fail(LORA_B200_EINVAL, "soft must be 0 or 1, got %u", (unsigned)P.soft);
+    if (P.crc_list > RS_CRC_MAX_LIST || (P.crc_list && !P.soft))
+        return fail(LORA_B200_EINVAL, "crc_list must be 0..%u and needs soft = 1, got %u", RS_CRC_MAX_LIST, (unsigned)P.crc_list);
     CU(cudaSetDevice(d->device));
     // rows: ns; receivers (groups of m antenna rows): ng.  m = 1 is lora_b200_receive, launch for launch.
     const uint32_t rows = d->cfg.n_streams, ns = rows / m, sps = d->sps, N = d->n_bins, cap = d->cfg.max_frames_per_call;
@@ -1218,6 +1226,7 @@ static int rs_receive(lora_b200_decoder *d, const void *iq, size_t n_items, size
     d->rs_hdr_drops = 0;
     d->rs_chan.clear();
     d->rs_chan_m = m;
+    d->rs_recovered.clear();
     const size_t guard = (size_t)(rp.min_preamble + 4u) * sps, none = ~(size_t)0;
     std::vector<size_t> end_pub(ns, 0), hold(ns, none);
     auto finish = [&]() {
@@ -1292,15 +1301,17 @@ static int rs_receive(lora_b200_decoder *d, const void *iq, size_t n_items, size
     CU(d->d_rs_win.reserve(win_cap * sps));
     CU(d->d_rs_hbins.reserve((size_t)n_sync * 8));
     // soft decisions: LLRs of ppm values per window (sf - 2 in the header round), corrected into the bins afterwards
+    // (with list decoding they go to a buffer of their own, which the payload round does not reuse)
     const uint32_t hppm = d->cfg.sf - 2u, pppm = d->cfg.reduced_rate ? hppm : d->cfg.sf;
-    if (soft) CU(d->d_rs_llr.reserve((size_t)n_sync * 8 * hppm));
+    DeviceBuffer<float> &hllr = P.crc_list ? d->d_rs_hllr : d->d_rs_llr;
+    if (soft) CU(hllr.reserve((size_t)n_sync * 8 * hppm));
     for (uint32_t f0 = 0; f0 < n_sync; f0 += (uint32_t)(win_cap / 8)) {
         const uint32_t nb = (uint32_t)std::min<size_t>(win_cap / 8, n_sync - f0);
         if (int rc = rs_assemble(d, x, stride, n_items, m, d->d_rs_frames + f0, m > 1 ? d->d_rs_chan + (size_t)f0 * 2 * RS_MAX_ANTENNAS : nullptr,
                                  nb, nullptr, 0, nullptr, 0, nullptr))
             return rc;
         if (soft) {
-            if (int rc = dispatch_llr(d, d->d_rs_win, (size_t)nb * 8, true, d->d_rs_llr + (size_t)f0 * 8 * hppm, nullptr, st)) return rc;
+            if (int rc = dispatch_llr(d, d->d_rs_win, (size_t)nb * 8, true, hllr + (size_t)f0 * 8 * hppm, nullptr, st)) return rc;
         } else if (int rc = dispatch_k1(d, d->k1s[0], d->d_rs_win, (size_t)nb * 8, d->d_rs_hbins + (size_t)f0 * 8, nullptr, st)) {
             return rc;
         }
@@ -1310,7 +1321,7 @@ static int rs_receive(lora_b200_decoder *d, const void *iq, size_t n_items, size
     rxp.sps = sps; rxp.n_bins = N; rxp.n_bins_hdr = d->n_bins_hdr; rxp.decim = d->decim; rxp.sf = d->cfg.sf;
     rxp.implicit = d->cfg.implicit; rxp.reduced_rate = d->cfg.reduced_rate;
     if (soft) {
-        rs_soft_header_kernel<<<(n_sync + 127) / 128, 128, 0, st>>>(n_sync, rxp, d->phdr1_init, d->d_rs_llr, d->d_rs_hbins);
+        rs_soft_header_kernel<<<(n_sync + 127) / 128, 128, 0, st>>>(n_sync, rxp, d->phdr1_init, hllr, d->d_rs_hbins);
         if (int rc = launched(d)) return rc;
     }
     rs_header_kernel<<<(n_sync + 127) / 128, 128, 0, st>>>(d->d_rs_frames, d->d_rs_nframes, fcap, rxp, d->phdr1_init, d->d_rs_hbins,
@@ -1387,6 +1398,13 @@ static int rs_receive(lora_b200_decoder *d, const void *iq, size_t n_items, size
                                                                   P.implicit_len, d->d_rs_llr, d->d_rs_pbins);
         if (int rc = launched(d)) return rc;
     }
+    if (P.crc_list) {
+        CU(d->d_rs_recovered.reserve(np));
+        rs_crc_list_kernel<<<(np + RS_CRC_WARPS - 1) / RS_CRC_WARPS, 32 * RS_CRC_WARPS, 0, st>>>(
+            d->d_rs_frames, t_pub, np, rxp, d->phdr1_init, P.crc_list, d->d_rs_hbins, t_off, P.implicit_len, d->d_rs_hllr, d->d_rs_llr,
+            d->d_rs_pbins, d->d_rs_recovered);
+        if (int rc = launched(d)) return rc;
+    }
     CU(d->d_rs_recs.reserve(np));
     CU(d->d_rs_out.reserve(np));
     rs_frame_kernel<<<(np + 127) / 128, 128, 0, st>>>(d->d_rs_frames, t_pub, t_seq, np, rxp, d->phdr1_init, d->d_rs_hbins, d->d_rs_pbins,
@@ -1404,6 +1422,10 @@ static int rs_receive(lora_b200_decoder *d, const void *iq, size_t n_items, size
     if (m > 1) {
         chan.resize((size_t)n_sync * 2 * RS_MAX_ANTENNAS);
         CU(cudaMemcpyAsync(chan.data(), d->d_rs_chan, sizeof(float2) * chan.size(), cudaMemcpyDeviceToHost, st));
+    }
+    if (P.crc_list) {
+        d->rs_recovered.resize(np);
+        CU(cudaMemcpyAsync(d->rs_recovered.data(), d->d_rs_recovered, np, cudaMemcpyDeviceToHost, st));
     }
     CU(cudaStreamSynchronize(st));
     d->rs_info.resize(np);
@@ -1454,6 +1476,7 @@ int lora_b200_demod_fft_antennas_dev(lora_b200_decoder *d, const void *iq, uint3
 }
 
 static_assert(sizeof(lora_b200_rx_info) == 32 && sizeof(lora_b200_rx_params) == 32 && offsetof(lora_b200_rx_params, soft) == 1 &&
+              offsetof(lora_b200_rx_params, crc_list) == 2 && offsetof(lora_b200_rx_params, implicit_len) == 4 &&
               offsetof(lora_b200_rx_params, sfo_ppm) == 16 &&
               offsetof(lora_b200_rx_params, carrier_hz) == 24 && offsetof(lora_b200_rx_info, sfo_ppm) == 28, "lora_b200_rx_* layout");
 
@@ -1532,6 +1555,20 @@ size_t lora_b200_frames_last(lora_b200_decoder *d, const lora_b200_frame **frame
     if (!d || !frames) { fail(LORA_B200_EINVAL, "null argument"); return 0; }
     *frames = reinterpret_cast<const lora_b200_frame *>(d->h_sorted.data());
     return d->h_sorted.size();
+}
+
+size_t lora_b200_frames_crc_last(lora_b200_decoder *d, const uint8_t **status) {
+    if (!d || !status) { fail(LORA_B200_EINVAL, "null argument"); return 0; }
+    const size_t n = d->h_sorted.size();
+    d->crc_status.resize(n);
+    for (size_t k = 0; k < n; k++) {
+        const RxFrameOut &f = d->h_sorted[k];
+        uint8_t s = (uint8_t)lb_crc_record_status(f.bytes, std::min<uint32_t>(f.len, (uint32_t)sizeof f.bytes));
+        if (s == LORA_CRC_OK && k < d->rs_recovered.size() && d->rs_recovered[k]) s = LORA_CRC_RECOVERED;
+        d->crc_status[k] = s;
+    }
+    *status = d->crc_status.data();
+    return n;
 }
 
 int lora_b200_set_cfo_estimate(lora_b200_decoder *d, int enable) {

@@ -21,6 +21,7 @@
 #include "int_chain.cuh"
 #include "k1_fft.cuh"
 #include "k1_llr.cuh"
+#include "lora_crc.h"
 #include "rx_stream.cuh"
 #include "tx_encode.cuh"
 
@@ -439,6 +440,119 @@ LB_HD void rs_soft_payload(const RxParams &p, uint8_t phdr1, const uint32_t *hdr
     for (uint32_t b = 0; b < (uint32_t)n_payload / spb; b++) rs_soft_block(c, b, llr + (size_t)b * spb * ppm, bins + (size_t)b * spb, nullptr);
 }
 
+// ---- CRC-aided list decoding (rx_params.crc_list) ---------------------------------------------------------------------------
+// A soft-decoded frame whose payload CRC (lora_crc.h) fails is given a second chance: of its code words that carry nibbles of
+// the CRC's message (rs_crc_candidate), the K least reliable (smallest gap between the best and the runner-up metric, ties to the lowest nibble index)
+// may each be replaced by its runner-up.  The CRC (initial value 0) and the whitening XOR are linear, so replacing nibble p's
+// s1 by s2 moves the syndrome by a fixed delta; of the 2^K subsets, those whose deltas sum to the syndrome satisfy the CRC,
+// and the one of least summed gap (the lowest subset mask on ties) is taken.  Its blocks are re-encoded into corrected bins,
+// so that decoding runs unchanged.  A frame whose real errors lie outside the list passes some subset with probability about
+// (2^K - 1) / 2^16: the price of the option, which is why K is at most RS_CRC_MAX_LIST and off by default.
+constexpr uint32_t RS_CRC_MAX_LIST = 12;
+constexpr uint32_t RS_CRC_MAX_SLOTS = 576;   // code words of one frame: sf - 2 in the header block, <= 2 (255 + 2) + sf in payload
+
+struct RsSoftPick {
+    uint32_t s1, s2;                   // the best nibble (rs_soft_nibble's) and the runner-up (the lowest on ties)
+    float gap;                         // their metric difference, >= 0
+};
+
+// rs_soft_nibble's candidates and metrics, keeping the runner-up as well
+template <class CW>
+LB_HD RsSoftPick rs_soft_pick(const CW &cw, const float *llr, uint32_t n_words, uint32_t ppm, uint32_t x) {
+    float m1 = 0.f, m2 = 0.f;
+    uint32_t s1 = 0, s2 = 0;
+    for (uint32_t s = 0; s < 16u; s++) {
+        const uint32_t c = cw(s);
+        float m = 0.f;
+        for (uint32_t i = 0; i < n_words; i++) {
+            const float l = llr[i * ppm + (x + 8u * ppm - i) % ppm];
+            m += (c >> i) & 1u ? -l : l;
+        }
+        if (s == 0u) { m1 = m; s1 = 0; }
+        else if (m > m1) { m2 = m1; s2 = s1; m1 = m; s1 = s; }
+        else if (s == 1u || m > m2) { m2 = m; s2 = s; }
+    }
+    return RsSoftPick{s1, s2, m1 - m2};
+}
+
+// one published frame as the list decoder sees it.  Its code words ("slots") q: the header block's sf - 2, then ppm per
+// payload block; slot q >= h carries payload nibble p = q - h (h = 5 header nibbles when explicit).
+struct RsCrcFrame {
+    TxCode c;                          // c.cr the frame's
+    uint32_t L;                        // payload bytes without the CRC; 0: no CRC to check
+    uint32_t hppm, ppm, spb, h, n_slots;
+};
+
+// the frame's header replayed from its corrected bins, as rs_frame_kernel does
+LB_HD RsCrcFrame rs_crc_frame(const RxParams &p, uint8_t phdr1, const uint32_t *hdr_bins, int32_t n_payload, uint32_t implicit_len) {
+    RxStreamState st;
+    rs_header(&st, p, phdr1, hdr_bins, implicit_len);
+    RsCrcFrame f;
+    f.c = rs_code(p, phdr1);
+    f.c.cr = st.phdr[1] >> 5;
+    f.L = ((st.phdr[1] >> 4) & 1u) && st.payload_length >= 4u ? st.payload_length - 2u : 0u;
+    f.hppm = p.sf - 2u; f.ppm = tx_ppm(f.c); f.spb = f.c.cr + 4u; f.h = f.c.explicit_hdr ? 5u : 0u;
+    f.n_slots = f.hppm + (uint32_t)(n_payload > 0 ? n_payload : 0) / f.spb * f.ppm;
+    return f;
+}
+
+// whether slot q is a list candidate: it carries a nibble of payload[0 .. L-2), the CRC's message.  The last two payload bytes
+// and the two CRC bytes are XORed into the check as they are, so an error of v in payload[L-1] and the same v in c0 (and in
+// payload[L-2] and c1) cancel: flipping one of them to "fix" an error in its partner satisfies the CRC and publishes a wrong
+// payload.  The interleaver makes such equal errors common (one bad symbol hits the same bit of neighbouring nibbles), so
+// these four bytes are never flipped: an error there leaves a syndrome that flips elsewhere only match by chance.
+LB_HD bool rs_crc_candidate(const RsCrcFrame &f, uint32_t q) { return q >= f.h && q - f.h < 2u * (f.L - 2u); }
+
+// slot q's pick from the header block's LLRs hllr[8][sf - 2] or the payload blocks' llr[][ppm]
+LB_HD RsSoftPick rs_crc_pick(const RsCrcFrame &f, const float *hllr, const float *llr, uint32_t q) {
+    if (q < f.hppm) return rs_soft_pick([&](uint32_t s) { return tx_header_cw(f.c, s, q); }, hllr, 8u, f.hppm, q);
+    const uint32_t b = (q - f.hppm) / f.ppm, x = (q - f.hppm) % f.ppm, p0 = tx_spare(f.c) + b * f.ppm;
+    return rs_soft_pick([&](uint32_t s) { return tx_payload_cw(f.c, s, p0 + x, f.spb); }, llr + (size_t)b * f.spb * f.ppm, f.spb, f.ppm, x);
+}
+
+// the syndrome of the published bytes that nibbles nib[q] (all slots) make: 0 iff the frame checks
+LB_HD uint32_t rs_crc_syndrome(const RsCrcFrame &f, const uint8_t *nib) {
+    auto byte = [&](uint32_t i) { return (uint32_t)nib[f.h + 2u * i] | ((uint32_t)nib[f.h + 2u * i + 1u] << 4); };
+    uint32_t crc = 0;
+    for (uint32_t i = 0; i + 2u < f.L; i++) crc = lb_crc16_byte(crc, byte(i));
+    return crc ^ byte(f.L - 1u) ^ (byte(f.L - 2u) << 8) ^ byte(f.L) ^ (byte(f.L + 1u) << 8) ^ lb_crc_whitening(f.c.cr, f.L);
+}
+
+// how the syndrome moves when payload nibble p (a candidate: in the CRC's message) is XORed with v: the CRC of e at byte p / 2
+// followed by the L - 3 - p / 2 bytes after it
+LB_HD uint32_t rs_crc_delta(uint32_t L, uint32_t p, uint32_t v) {
+    uint32_t c = lb_crc16_byte(0, v << (4u * (p & 1u)));
+    for (uint32_t k = (p >> 1) + 3u; k < L; k++) c = lb_crc16_byte(c, 0);
+    return c;
+}
+
+// the summed gap of subset `mask` of the list gap[0 .. K), in list order
+LB_HD float rs_crc_cost(const float *gap, uint32_t mask) {
+    float c = 0.f;
+    for (uint32_t j = 0; mask; j++, mask >>= 1)
+        if (mask & 1u) c += gap[j];
+    return c;
+}
+
+LB_HD unsigned long long rs_crc_key(float v, uint32_t idx) {      // (v >= 0, idx) ordered lexicographically, smallest first
+    union { float f; uint32_t u; } c;
+    c.f = v;
+    return ((unsigned long long)c.u << 32) | idx;
+}
+
+// number of bins of slot q's block, and bin i of it re-encoded from the frame's nibbles nib[q] (all slots); the header
+// block's bins are hdr[0 .. 8), payload block b's are pay[b spb ..]
+LB_HD uint32_t rs_crc_block_bins(const RsCrcFrame &f, uint32_t q) { return q < f.hppm ? 8u : f.spb; }
+LB_HD uint32_t *rs_crc_block_out(const RsCrcFrame &f, uint32_t q, uint32_t *hdr, uint32_t *pay) {
+    return q < f.hppm ? hdr : pay + (size_t)((q - f.hppm) / f.ppm) * f.spb;
+}
+LB_HD uint32_t rs_crc_block_bin(const RsCrcFrame &f, const uint8_t *nib, uint32_t q, uint32_t i) {
+    if (q < f.hppm) return tx_block_shift([&](uint32_t y) { return tx_header_cw(f.c, nib[y], y); }, i, f.hppm, true, 1u << f.c.sf);
+    const uint32_t b = (q - f.hppm) / f.ppm, q0 = f.hppm + b * f.ppm, p0 = tx_spare(f.c) + b * f.ppm;
+    return tx_block_shift([&](uint32_t y) { return tx_payload_cw(f.c, nib[q0 + y], p0 + y, f.spb); }, i, f.ppm, f.c.reduced_rate != 0u,
+                          1u << f.c.sf);
+}
+
 #ifdef __CUDACC__
 // ---- kernels ---------------------------------------------------------------------------------------------------------------
 // detect: one thread per stream.  The screen's windows of row s are the K1 results starting at s * stride / sps (stride a
@@ -791,6 +905,106 @@ __global__ void rs_soft_payload_kernel(const RsFrame *__restrict__ frames, const
     const uint32_t f = pub[k];
     rs_soft_payload(p, phdr1, hdr_bins + (size_t)f * 8, frames[f].n_payload, implicit_len,
                     llr + (size_t)offs[k] * tx_ppm(rs_code(p, phdr1)), bins + offs[k]);
+}
+
+// CRC-aided list decoding of the payload round: one warp per published frame (index list `pub`), after
+// rs_soft_payload_kernel.  hllr: the header round's LLRs (frame f at f * 8 * (sf - 2)), llr / bins / offs as
+// rs_soft_payload_kernel.  A recovered frame's changed blocks are re-encoded into hdr_bins and bins; recovered[k] = 1 then,
+// else 0.  Lane l picks slots l, l + 32, ...; the list is chosen in K rounds of a warp-wide minimum; the 2^K subsets are
+// split into 32 runs of consecutive Gray-code indices, one XOR per step.
+constexpr int RS_CRC_WARPS = 4;
+
+LB_D unsigned long long rs_warp_min(unsigned long long v) {
+    for (int o = 16; o > 0; o >>= 1) {
+        const unsigned long long w = __shfl_xor_sync(0xffffffffu, v, o);
+        v = w < v ? w : v;
+    }
+    return v;
+}
+
+__global__ void __launch_bounds__(32 * RS_CRC_WARPS)
+rs_crc_list_kernel(const RsFrame *__restrict__ frames, const uint32_t *__restrict__ pub, uint32_t n_pub, RxParams p, uint8_t phdr1,
+                   uint32_t K, uint32_t *__restrict__ hdr_bins, const uint32_t *__restrict__ offs, uint32_t implicit_len,
+                   const float *__restrict__ hllr, const float *__restrict__ llr, uint32_t *__restrict__ bins,
+                   uint8_t *__restrict__ recovered) {
+    __shared__ uint8_t s_nib[RS_CRC_WARPS][RS_CRC_MAX_SLOTS], s_alt[RS_CRC_WARPS][RS_CRC_MAX_SLOTS];
+    __shared__ float s_gap[RS_CRC_WARPS][RS_CRC_MAX_SLOTS];
+    __shared__ uint32_t s_q[RS_CRC_WARPS][RS_CRC_MAX_LIST], s_delta[RS_CRC_WARPS][RS_CRC_MAX_LIST];
+    __shared__ float s_lgap[RS_CRC_WARPS][RS_CRC_MAX_LIST];
+    const uint32_t w = threadIdx.x >> 5, lane = threadIdx.x & 31u, k = blockIdx.x * RS_CRC_WARPS + w;
+    if (k >= n_pub) return;                           // (whole warps)
+    const uint32_t f = pub[k];
+    const RsCrcFrame cf = rs_crc_frame(p, phdr1, hdr_bins + (size_t)f * 8, frames[f].n_payload, implicit_len);
+    uint8_t *nib = s_nib[w], *alt = s_alt[w];
+    float *gap = s_gap[w];
+    if (cf.L == 0u || cf.n_slots > RS_CRC_MAX_SLOTS || cf.h + 2u * (cf.L + 2u) > cf.n_slots) {
+        if (lane == 0) recovered[k] = 0;
+        return;
+    }
+    // metrics of every slot: the soft decoder's nibble, the runner-up, the gap
+    const float *hl = hllr + (size_t)f * 8 * cf.hppm, *pl = llr + (size_t)offs[k] * cf.ppm;
+    for (uint32_t q = lane; q < cf.n_slots; q += 32u) {
+        const RsSoftPick r = rs_crc_pick(cf, hl, pl, q);
+        nib[q] = (uint8_t)r.s1; alt[q] = (uint8_t)r.s2; gap[q] = r.gap;
+    }
+    __syncwarp();
+    const uint32_t S0 = rs_crc_syndrome(cf, nib);
+    if (S0 == 0u) {
+        if (lane == 0) recovered[k] = 0;
+        return;
+    }
+    // the list: the K candidates of least gap, the lowest slot (= nibble index) on ties
+    const uint32_t q0 = cf.h, q1 = cf.h + 2u * (cf.L - 2u);          // (rs_crc_candidate)
+    uint32_t n = 0;
+    for (; n < K; n++) {
+        unsigned long long key = ~0ull;
+        for (uint32_t q = q0 + lane; q < q1; q += 32u)
+            if (!(alt[q] & 0x80u)) { const unsigned long long c = rs_crc_key(gap[q], q); key = c < key ? c : key; }
+        key = rs_warp_min(key);
+        if (key == ~0ull) break;
+        const uint32_t q = (uint32_t)key;
+        if (lane == 0) { alt[q] |= 0x80u; s_q[w][n] = q; s_lgap[w][n] = gap[q]; }
+        __syncwarp();
+    }
+    if (lane < n) {
+        const uint32_t q = s_q[w][lane];
+        s_delta[w][lane] = rs_crc_delta(cf.L, q - cf.h, nib[q] ^ (alt[q] & 15u));
+    }
+    __syncwarp();
+    // the subsets: lane l walks Gray-code indices [l per, (l + 1) per)
+    const uint32_t total = 1u << n, per = total > 32u ? total >> 5 : 1u, g0 = lane * per;
+    unsigned long long best = ~0ull;
+    if (g0 < total) {
+        uint32_t mask = g0 ^ (g0 >> 1), syn = 0;
+        for (uint32_t j = 0; j < n; j++)
+            if (mask >> j & 1u) syn ^= s_delta[w][j];
+        for (uint32_t t = 0; t < per; t++) {
+            if (t) {
+                const uint32_t b = (uint32_t)(__ffs((int)(g0 + t)) - 1);
+                mask ^= 1u << b;
+                syn ^= s_delta[w][b];
+            }
+            if (syn == S0) {
+                const unsigned long long c = rs_crc_key(rs_crc_cost(s_lgap[w], mask), mask);
+                best = c < best ? c : best;
+            }
+        }
+    }
+    best = rs_warp_min(best);
+    if (best == ~0ull) {
+        if (lane == 0) recovered[k] = 0;
+        return;
+    }
+    const uint32_t mask = (uint32_t)best;
+    if (lane < n && (mask >> lane & 1u)) { const uint32_t q = s_q[w][lane]; nib[q] = alt[q] & 15u; }
+    __syncwarp();
+    uint32_t *hb = hdr_bins + (size_t)f * 8, *pb = bins + offs[k];
+    for (uint32_t j = 0; j < n; j++) {
+        if (!(mask >> j & 1u)) continue;
+        const uint32_t q = s_q[w][j];
+        if (lane < rs_crc_block_bins(cf, q)) rs_crc_block_out(cf, q, hb, pb)[lane] = rs_crc_block_bin(cf, nib, q, lane);
+    }
+    if (lane == 0) recovered[k] = 1;
 }
 #endif  // __CUDACC__
 

@@ -143,6 +143,13 @@ class decoder:
         buf = C.string_at(ptr.value, n * self.FRAME_DTYPE.itemsize)
         return np.frombuffer(buf, dtype=self.FRAME_DTYPE)
 
+    def frames_crc_last(self) -> np.ndarray:
+        """uint8 per frame of frames_last(): the payload CRC status (lora_b200_frames_crc_last) -- N.CRC_NONE (no CRC in the
+        header, or a payload under 2 bytes), CRC_OK, CRC_BAD or CRC_RECOVERED (OK after list decoding, receive(crc_list=K))."""
+        ptr = C.c_void_p(0)
+        n = int(self._L.lora_b200_frames_crc_last(self._h, C.byref(ptr)))
+        return np.frombuffer(C.string_at(ptr.value, n), dtype=np.uint8).copy() if n else np.zeros(0, np.uint8)
+
     def work_batch(self, iq, n_items=None, stride_items=None, host=None, sc16_scale=None, callbacks=True, sc8_scale=None):
         """All streams at once. ``iq``: host ndarray [n_streams, n_items] (complex64, or int16 / int8 [n_streams, n_items, 2]
         together with ``sc16_scale`` / ``sc8_scale``) or a device tensor/pointer.  ``sc16_scale`` / ``sc8_scale`` select the
@@ -181,7 +188,7 @@ class decoder:
                               ("sfo_ppm", "<f4")])       # struct lora_b200_rx_info
 
     def receive(self, iq, n_items=None, stride_items=None, host=None, sync_word=0x12, implicit_len=0, min_preamble=0,
-                max_cfo_hz=0.0, sfo_ppm=0.0, carrier_hz=0.0, soft=False, antennas=1):
+                max_cfo_hz=0.0, sfo_ppm=0.0, carrier_hz=0.0, soft=False, antennas=1, crc_list=0):
         """The dechirp-synchronised receiver (lora_b200_receive): decodes frames below the noise floor.  ``iq`` as for
         work_batch (host ndarray [n_streams, n_items] or a device tensor / pointer).  Returns (consumed, frames, info):
         consumed[s] = where stream s must be re-presented from, frames = FRAME_DTYPE records, info = RX_INFO_DTYPE records
@@ -193,7 +200,11 @@ class decoder:
         antennas = M (1..4, dividing n_streams): rows g M .. g M + M - 1 are the phase-coherent antennas of receiver g
         (lora_b200_receive_antennas): combined screen and synchronisation, maximum-ratio-combined data windows; consumed has
         one entry per receiver, frames and info carry stream = g and the combined SNR, and rx_channels_last() gives each
-        frame's channel estimates."""
+        frame's channel estimates.
+        crc_list = K (1..12, needs soft): a frame whose payload CRC fails gets its K least reliable code words tried at their
+        runner-up nibbles, and the cheapest combination that satisfies the CRC is published (frames_crc_last() reports it
+        RECOVERED).  A frame whose errors lie outside the list passes a wrong combination with probability about
+        (2^K - 1) / 2^16; 0 (the default) is off."""
         if isinstance(iq, np.ndarray):
             x = np.ascontiguousarray(iq, dtype=np.complex64)
             assert x.ndim == 2 and x.shape[0] == self.n_streams
@@ -206,7 +217,8 @@ class decoder:
             if stride_items is None:
                 stride_items = n_items
         p = N.RxParams(sync_word=int(sync_word) & 0xFF, implicit_len=int(implicit_len), min_preamble=int(min_preamble),
-                       max_cfo_hz=float(max_cfo_hz), sfo_ppm=float(sfo_ppm), carrier_hz=float(carrier_hz), soft=int(soft))
+                       max_cfo_hz=float(max_cfo_hz), sfo_ppm=float(sfo_ppm), carrier_hz=float(carrier_hz), soft=int(soft),
+                       crc_list=int(crc_list))
         m = int(antennas)
         consumed = np.zeros(max(self.n_streams // m, 1) if m > 0 else 1, dtype=np.uint64)
         cptr = consumed.ctypes.data_as(C.POINTER(C.c_size_t))

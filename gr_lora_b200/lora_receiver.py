@@ -6,6 +6,7 @@ from __future__ import annotations
 
 import numpy as np
 
+from . import _native as N
 from .decoder import decoder
 
 
@@ -19,7 +20,8 @@ class _DeviceRow:
 class lora_receiver:
     def __init__(self, samp_rate, center_freq, channel_list, bandwidth, sf, implicit, cr, crc, reduced_rate=False,
                  conj=False, decimation=1, disable_channelization=False, disable_drift_correction=False, cfo_feedback=False,
-                 sync="reference", sync_word=0x12, implicit_len=0, clock_from_carrier=False, soft=False, antennas=1, **decoder_kw):
+                 sync="reference", sync_word=0x12, implicit_len=0, clock_from_carrier=False, soft=False, antennas=1, crc_list=0,
+                 drop_bad_crc=False, **decoder_kw):
         self.samp_rate, self.center_freq, self.channel_list = samp_rate, center_freq, list(channel_list)
         self.bandwidth, self.sf, self.implicit, self.cr, self.crc = bandwidth, sf, implicit, cr, crc
         self.decimation, self.conj = decimation, conj
@@ -38,6 +40,11 @@ class lora_receiver:
         if soft and sync != "dechirp":
             raise ValueError("soft needs sync='dechirp' (the reference state machine makes hard decisions)")
         self.soft = bool(soft)
+        # crc_list = K: CRC-aided list decoding of the soft decisions (decoder.receive(..., crc_list=K)); drop_bad_crc: frames
+        # whose payload CRC fails are not published (off by default, so that the published stream is the reference's)
+        if (crc_list or drop_bad_crc) and sync != "dechirp":
+            raise ValueError("crc_list and drop_bad_crc need sync='dechirp'")
+        self.crc_list, self.drop_bad_crc = int(crc_list), bool(drop_bad_crc)
         # antennas = M: run() takes an (M, n) capture of M phase-coherent antennas (one LO, one sample clock) and the dechirp
         # receiver combines them (decoder.receive(..., antennas=M)); with the channelizer every antenna gets its own
         # channelizer, which filters and rotates it exactly as the others, so the combining weights stay meaningful
@@ -158,8 +165,11 @@ class lora_receiver:
                 part = src + 8 * pos
             c, frames, _ = self.decoder.receive(part, n_items=n, stride_items=n if stride is None else stride, host=0, sync_word=self.sync_word,
                                                 implicit_len=self.implicit_len, carrier_hz=carrier, soft=self.soft,
-                                                antennas=self.antennas)
-            for f in frames:
+                                                antennas=self.antennas, crc_list=self.crc_list)
+            crc = self.decoder.frames_crc_last() if self.drop_bad_crc else None
+            for k, f in enumerate(frames):
+                if crc is not None and crc[k] == N.CRC_BAD:
+                    continue
                 self.decoder._publish(int(f["stream"]), bytes(f["bytes"][: int(f["len"])]))
             c = int(c[0])
             at_end = pos + n >= n_out

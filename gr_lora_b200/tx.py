@@ -109,6 +109,43 @@ def header_bytes(length: int, cr: int, has_crc: int) -> bytes:
     return bytes([length & 0xFF, ((cr & 7) << 5) | ((has_crc & 1) << 4) | (chk >> 4), (chk & 0xF) << 4])
 
 
+def payload_crc(payload: bytes) -> int:
+    """Semtech's payload CRC of ``payload`` (L >= 2 bytes, without the CRC): CRC-16, polynomial 0x1021, initial value 0, no
+    reflection, no final XOR, over payload[0 .. L-2), XORed with payload[L-1] | payload[L-2] << 8.  de ad be ef -> 0xEC80."""
+    if len(payload) < 2:
+        raise ValueError("the payload CRC needs at least 2 payload bytes")
+    crc = 0
+    for b in payload[:-2]:
+        crc ^= b << 8
+        for _ in range(8):
+            crc = ((crc << 1) ^ 0x1021) & 0xFFFF if crc & 0x8000 else (crc << 1) & 0xFFFF
+    return crc ^ payload[-1] ^ (payload[-2] << 8)
+
+
+def _data_projection(w: int, cr: int) -> int:
+    """The nibble the decode chain makes of a dewhitened byte w: the nearest Hamming(8,4) code word's data (the lowest nibble
+    on ties) for CR 4/7 and 4/8, the data bits 1, 2, 3, 5 for CR 4/5 and 4/6 (lib/decoder_impl.cc:654-706)."""
+    if cr >= 3:
+        return min(range(16), key=lambda s: (bin(w ^ HAMMING84[s]).count("1"), s))
+    return ((w >> 1) & 1) | (((w >> 2) & 1) << 1) | (((w >> 3) & 1) << 2) | (((w >> 5) & 1) << 3)
+
+
+def crc_whitening(length: int, cr: int) -> int:
+    """W(L): what the decode chain, which dewhitens every payload nibble, makes of an unwhitened CRC of 0 after an L-byte
+    payload -- the data projection of whitening bytes 2L .. 2L+3, published low byte first.  L = 4: 0xE1F0."""
+    prng = whitening.payload_sequence(cr)
+    nib = [_data_projection(prng[i] if i < len(prng) else 0, cr) for i in range(2 * length, 2 * length + 4)]
+    return nib[0] | nib[1] << 4 | nib[2] << 8 | nib[3] << 12
+
+
+def crc_bytes(payload: bytes, cr: int) -> bytes:
+    """The two bytes to append to ``payload`` so that encode_frame(payload + crc_bytes(payload, cr), ...) is the frame a
+    radio sends: encode_frame whitens every byte it is given, the radio does not whiten its CRC, so the CRC goes in as
+    crc ^ W(L).  The decoder publishes these same two bytes, and the frame checks."""
+    v = payload_crc(payload) ^ crc_whitening(len(payload), cr)
+    return bytes([v & 0xFF, v >> 8])
+
+
 def payload_symbols_expected(payload_len: int, cr: int, sf: int, reduced_rate: bool) -> int:
     """Number of payload symbols the reference will read (lib/decoder_impl.cc:842-847),
     evaluated with the same fp32 expressions."""

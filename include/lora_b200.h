@@ -268,6 +268,18 @@ typedef struct lora_b200_frame {
     uint8_t  bytes[LORA_B200_MAX_FRAME_BYTES];
 } lora_b200_frame;
 size_t lora_b200_frames_last(lora_b200_decoder *d, const lora_b200_frame **frames);
+/* The payload CRC status of every frame of lora_b200_frames_last, parallel to it (valid after work, work_batch*, receive and
+ * receive_antennas, until the next call): LORA_B200_CRC_NONE when the frame's header (or the implicit configuration) carries
+ * no CRC or its payload is shorter than 2 bytes, _OK, _BAD, or _RECOVERED: OK only after CRC-aided list decoding
+ * (lora_b200_rx_params.crc_list).  Semtech's CRC: CRC-16, polynomial 0x1021, initial value 0, over payload[0 .. L-2), XORed
+ * with payload[L-1] | payload[L-2] << 8; the radio sends it low byte first, unwhitened, and the decode chain dewhitens it
+ * like every payload nibble, so the published CRC bytes are crc ^ W(L), a fixed XOR (DESIGN.md section 5).  Computed on the
+ * host from the published records: no launch, no copy, nothing published changes; frames that fail are still published. */
+#define LORA_B200_CRC_NONE 0
+#define LORA_B200_CRC_OK 1
+#define LORA_B200_CRC_BAD 2
+#define LORA_B200_CRC_RECOVERED 3
+size_t lora_b200_frames_crc_last(lora_b200_decoder *d, const uint8_t **status);
 /* ---- dechirp-synchronised receiver: frames below the noise floor (an opt-in path beside the reference state machine) ----
  * iq = [n_streams][n_items] cf32 (row stride stride_items; host_ptr != 0: host memory, copied inside; 0: device memory).
  * Every stream is screened by K1 (dechirp + FFT + argmax) on windows at hops of sps/2; runs of >= min_preamble windows whose
@@ -275,7 +287,7 @@ size_t lora_b200_frames_last(lora_b200_decoder *d, const lora_b200_frame **frame
  * SFD bins, fractional CFO from the preamble peak's phase advance, timing to the sample, then the two sync-word symbols are
  * checked.  Data windows are de-rotated by the frame's CFO and demodulated by the K1 batch kernels; the FFT demodulator's
  * (bin - 1) mod N mapping and the stream path's integer chain follow.  Explicit headers whose 5-bit checksum fails are dropped
- * (and counted); the payload CRC is not checked.  Implicit headers carry implicit_len payload bytes (0 with an implicit-header
+ * (and counted); frames whose payload CRC fails are published too (lora_b200_frames_crc_last reports it).  Implicit headers carry implicit_len payload bytes (0 with an implicit-header
  * decoder: LORA_B200_EINVAL).  Needs the FFT kernels (samp_rate / bandwidth == 8 or 2, SF7..SF12), else LORA_B200_EUNSUPPORTED;
  * at 2 (e.g. 500 kHz channels at 1 MS/s, or a channelizer's output at 2 samples per chip) timing is refined to +-1 sample.
  * Clock offset: a transmitter whose clock is off by delta = ppm * 1e-6 (delta > 0: fast against the receiver) sends TX symbol
@@ -298,11 +310,17 @@ size_t lora_b200_frames_last(lora_b200_decoder *d, const lora_b200_frame **frame
  * then by start), their synchronisation through lora_b200_rx_info_last.
  * Soft decisions (p->soft = 1; other values than 0 and 1: LORA_B200_EINVAL): the data windows go through the LLR
  * demodulator (lora_b200_demod_llr_dev) instead of K1, each code word is decoded to the nibble whose encoder code word best
- * matches its bits' LLRs, and the bins of the re-encoded code words replace the argmax bins before the integer chain. */
+ * matches its bits' LLRs, and the bins of the re-encoded code words replace the argmax bins before the integer chain.
+ * CRC-aided list decoding (p->crc_list = K, 1..12, needs soft = 1; other values: LORA_B200_EINVAL before any launch): a frame
+ * whose payload CRC fails gets its K least reliable payload / CRC code words (smallest metric gap to the runner-up nibble)
+ * tried at their runner-ups, and the cheapest combination (least summed gap) that satisfies the CRC is published, with status
+ * LORA_B200_CRC_RECOVERED.  The price: a frame whose errors lie outside the list passes a wrong combination with probability
+ * about (2^K - 1) / 2^16, which is why K is capped and the option is off by default.  0 changes nothing. */
 typedef struct lora_b200_rx_params {
     uint8_t  sync_word;          /* 0 = 0x12                                                    */
     uint8_t  soft;               /* 1: soft-decision decoding (per-bit LLRs, ML code words)      */
-    uint8_t  reserved0[2];
+    uint8_t  crc_list;           /* CRC-aided list decoding of K code words (0 = off), see above */
+    uint8_t  reserved0[1];
     uint32_t implicit_len;       /* payload bytes of implicit-header frames (incl. CRC bytes)  */
     uint32_t min_preamble;       /* windows of one phase (0 = 5)                                */
     float    max_cfo_hz;         /* 0 = BW / 4; larger values are clamped to BW / 4             */
