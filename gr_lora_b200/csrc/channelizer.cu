@@ -212,9 +212,7 @@ int lora_b200_channelizer_work_dev(lora_b200_channelizer *c, const void *in_dev,
     cudaStreamSynchronize(st);                       // dph is a stack vector
     const uint32_t seg = (CH_TN - 1) * c->decimation + c->ntaps;
     const size_t smem = sizeof(float2) * ((size_t)seg + (size_t)CH_CT * c->ntaps);
-    static lb::DeviceOnce once;
-    if (smem > 48 * 1024 &&
-        once(c->device, [] { return cudaFuncSetAttribute(chan_fir_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024); }) != cudaSuccess)
+    if (smem > 48 * 1024 && lb::opt_in_smem((const void *)chan_fir_kernel, c->device, 200 * 1024) != cudaSuccess)
         return cfail(c, LORA_B200_ECUDA, "channelizer_work: shared memory attribute");
     if (smem > 200 * 1024) return cfail(c, LORA_B200_EUNSUPPORTED, "channelizer_work: filter too long for one tile");
     dim3 grid((unsigned)((no + CH_TN - 1) / CH_TN), (c->n_channels + CH_CT - 1) / CH_CT);

@@ -3,6 +3,7 @@
 // on the host and compare them with the oracle, and drive the owning buffer type of
 // cuda_owned.h.  Not part of liblora_b200.so.
 #include "cuda_owned.h"
+#include "dispatch.h"
 #include "k1_fft.cuh"
 #include "k1_llr.cuh"
 #include "k1_warp.cuh"
@@ -19,41 +20,13 @@
 #include <cstring>
 #include <vector>
 
-template <int D>
-static int k1_emulate_d(int sf, const lb::K1Args &a, uint32_t *bins, float *mags) {
-    switch (sf) {
-    case 7: lb::k1_emulate<7, D>(a, bins, mags); break;
-    case 8: lb::k1_emulate<8, D>(a, bins, mags); break;
-    case 9: lb::k1_emulate<9, D>(a, bins, mags); break;
-    case 10: lb::k1_emulate<10, D>(a, bins, mags); break;
-    case 11: lb::k1_emulate<11, D>(a, bins, mags); break;
-    case 12: lb::k1_emulate<12, D>(a, bins, mags); break;
-    default: return -1;
-    }
-    return 0;
-}
-
-template <int D>
-static int k1_llr_emulate_d(int sf, const lb::K1Args &a, bool reduced, float *llrs, uint32_t *bins) {
-    switch (sf) {
-    case 7: lb::k1_llr_emulate<7, D>(a, reduced, llrs, bins); break;
-    case 8: lb::k1_llr_emulate<8, D>(a, reduced, llrs, bins); break;
-    case 9: lb::k1_llr_emulate<9, D>(a, reduced, llrs, bins); break;
-    case 10: lb::k1_llr_emulate<10, D>(a, reduced, llrs, bins); break;
-    case 11: lb::k1_llr_emulate<11, D>(a, reduced, llrs, bins); break;
-    case 12: lb::k1_llr_emulate<12, D>(a, reduced, llrs, bins); break;
-    default: return -1;
-    }
-    return 0;
-}
-
 extern "C" {
 
 // k1_fft_kernel<SF, D> on the host, D = osr = sps / N (8 or 2); -1 for another SF or D
 int lb_k1_emulate_osr(int sf, int osr, const float2 *x, size_t n_symbols, const float2 *chirp, const float2 *tw, uint32_t *bins,
                       float *mags) {
     const lb::K1Args a{x, chirp, tw, n_symbols};
-    return osr == 8 ? k1_emulate_d<8>(sf, a, bins, mags) : osr == 2 ? k1_emulate_d<2>(sf, a, bins, mags) : -1;
+    return lb::with_sf_osr(sf, osr, [] { return -1; }, [&](auto SF, auto D) { lb::k1_emulate<SF, D>(a, bins, mags); return 0; });
 }
 
 // k1_antennas_kernel<SF, D> on the host for one group: m rows of n_symbols windows, row_stride samples apart -> the argmax
@@ -61,23 +34,10 @@ int lb_k1_emulate_osr(int sf, int osr, const float2 *x, size_t n_symbols, const 
 int lb_k1_antennas_emulate_osr(int sf, int osr, const float2 *x, size_t row_stride, uint32_t m, size_t n_symbols, const float2 *chirp,
                                const float2 *tw, uint32_t *bins, float *mags) {
     const lb::K1Args a{x, chirp, tw, n_symbols};
-    if (osr != 8 && osr != 2) return -1;
-    switch (sf * 16 + osr) {
-    case 7 * 16 + 8: lb::k1_antennas_emulate<7, 8>(a, row_stride, m, bins, mags); break;
-    case 8 * 16 + 8: lb::k1_antennas_emulate<8, 8>(a, row_stride, m, bins, mags); break;
-    case 9 * 16 + 8: lb::k1_antennas_emulate<9, 8>(a, row_stride, m, bins, mags); break;
-    case 10 * 16 + 8: lb::k1_antennas_emulate<10, 8>(a, row_stride, m, bins, mags); break;
-    case 11 * 16 + 8: lb::k1_antennas_emulate<11, 8>(a, row_stride, m, bins, mags); break;
-    case 12 * 16 + 8: lb::k1_antennas_emulate<12, 8>(a, row_stride, m, bins, mags); break;
-    case 7 * 16 + 2: lb::k1_antennas_emulate<7, 2>(a, row_stride, m, bins, mags); break;
-    case 8 * 16 + 2: lb::k1_antennas_emulate<8, 2>(a, row_stride, m, bins, mags); break;
-    case 9 * 16 + 2: lb::k1_antennas_emulate<9, 2>(a, row_stride, m, bins, mags); break;
-    case 10 * 16 + 2: lb::k1_antennas_emulate<10, 2>(a, row_stride, m, bins, mags); break;
-    case 11 * 16 + 2: lb::k1_antennas_emulate<11, 2>(a, row_stride, m, bins, mags); break;
-    case 12 * 16 + 2: lb::k1_antennas_emulate<12, 2>(a, row_stride, m, bins, mags); break;
-    default: return -1;
-    }
-    return 0;
+    return lb::with_sf_osr(sf, osr, [] { return -1; }, [&](auto SF, auto D) {
+        lb::k1_antennas_emulate<SF, D>(a, row_stride, m, bins, mags);
+        return 0;
+    });
 }
 
 int lb_k1_emulate(int sf, const float2 *x, size_t n_symbols, const float2 *chirp, const float2 *tw,
@@ -89,7 +49,10 @@ int lb_k1_emulate(int sf, const float2 *x, size_t n_symbols, const float2 *chirp
 int lb_k1_llr_emulate_osr(int sf, int osr, const float2 *x, size_t n_symbols, const float2 *chirp, const float2 *tw, int reduced,
                           float *llrs, uint32_t *bins) {
     const lb::K1Args a{x, chirp, tw, n_symbols};
-    return osr == 8 ? k1_llr_emulate_d<8>(sf, a, reduced != 0, llrs, bins) : osr == 2 ? k1_llr_emulate_d<2>(sf, a, reduced != 0, llrs, bins) : -1;
+    return lb::with_sf_osr(sf, osr, [] { return -1; }, [&](auto SF, auto D) {
+        lb::k1_llr_emulate<SF, D>(a, reduced != 0, llrs, bins);
+        return 0;
+    });
 }
 
 // ... at fs/bw = 8

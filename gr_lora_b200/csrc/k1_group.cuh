@@ -278,11 +278,8 @@ k1_group_kernel(K1Args a, uint32_t *__restrict__ bins, float *__restrict__ mags)
 // instantiated in the translation unit that owns the SF's kernel: SF8 lora_b200.cu, SF9 k1_packed.cu
 template <int SF, int NGROUPS, int NSLOT>
 int k1_launch_group(const K1Launch &k) {
-    static DeviceOnce once;
     const size_t smem = sizeof(GSmem<SF, NGROUPS, NSLOT>);
-    K1_CU(once(k.device, [&] {
-        return cudaFuncSetAttribute(k1_group_kernel<SF, NGROUPS, NSLOT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    }));
+    K1_CU(opt_in_smem((const void *)k1_group_kernel<SF, NGROUPS, NSLOT>, k.device, smem));
     const int grid = (int)std::min((k.a.n_symbols + NGROUPS - 1) / NGROUPS, (size_t)k.n_sms);
     k1_group_kernel<SF, NGROUPS, NSLOT><<<grid, NGROUPS * GCfg<SF>::T, smem, k.st>>>(k.a, k.bins, k.mags);
     K1_CU(cudaGetLastError());

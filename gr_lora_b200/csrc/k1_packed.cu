@@ -9,11 +9,8 @@ namespace lb {
 
 int k1_launch_warp7(const K1Launch &k) {
     constexpr int NW = 12, NS = 2;
-    static DeviceOnce once;
     const size_t smem = sizeof(W7Smem<NW, NS>);
-    K1_CU(once(k.device, [&] {
-        return cudaFuncSetAttribute(k1_sf7_warp_kernel<NW, NS>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    }));
+    K1_CU(opt_in_smem((const void *)k1_sf7_warp_kernel<NW, NS>, k.device, smem));
     const int grid = (int)std::min((k.a.n_symbols + NW - 1) / NW, (size_t)k.n_sms);
     k1_sf7_warp_kernel<NW, NS><<<grid, NW * 32, smem, k.st>>>(k.a, k.bins, k.mags);
     K1_CU(cudaGetLastError());

@@ -34,9 +34,9 @@ int k1_launch_rows(const K1Launch &k) {
     using C = RCfg<SF>;
     static DeviceOnce once;
     const size_t smem = sizeof(RSmem<SF>);
-    K1_CU(once(k.device, [&] {      // the shared-memory and cluster opt-ins, and the per-q2 constants from the host table
-        cudaError_t e = cudaFuncSetAttribute(k1_rows_kernel<SF>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-        if (e == cudaSuccess && C::CL > 1) e = cudaFuncSetAttribute(k1_rows_kernel<SF>, cudaFuncAttributeNonPortableClusterSizeAllowed, 0);
+    K1_CU(opt_in_smem((const void *)k1_rows_kernel<SF>, k.device, smem));
+    K1_CU(once(k.device, [&] {      // the cluster opt-in, and the per-q2 constants from the host table
+        const cudaError_t e = C::CL > 1 ? cudaFuncSetAttribute(k1_rows_kernel<SF>, cudaFuncAttributeNonPortableClusterSizeAllowed, 0) : cudaSuccess;
         if (e != cudaSuccess) return e;
         RConsts rc;
         r_build_consts<SF>(k.tw_host, rc);

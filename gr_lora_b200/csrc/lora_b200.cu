@@ -8,6 +8,7 @@
 #include "k1_group.cuh"
 #include "k1_sf10.cuh"
 #include "k1_launch.h"
+#include "dispatch.h"
 #include "rx_stream.cuh"
 #include "rx_sync.cuh"
 #include "rx_warp.cuh"
@@ -82,8 +83,8 @@ struct lora_b200_decoder : A1Params {
     // derived, decoder_impl.cc:69-91 (A1Params and these)
     uint32_t n_bins_hdr, decim;
     double bits_per_second, bits_per_symbol;
-    bool k1_ok;                           // fs/bw == 8 and SF7..12: FFT kernels usable
-    bool k1_osr2;                         // fs/bw == 2 and SF7..12: the generic K1 and LLR kernels at D = 2 usable
+    int k1_osr;                           // the K1 kernels' D = fs/bw with SF7..12: 8 (every K1 kernel), 2 (the generic K1 and
+                                          // LLR kernels), or 0 (none)
     int device, n_sms;
     Tables toff;
     DeviceBuffer<uint8_t> d_tables;
@@ -226,13 +227,23 @@ const T *tab(const lora_b200_decoder *d, size_t off) { return (const T *)(d->d_t
 
 int launched(lora_b200_decoder *d) { d->launches++; CU(cudaGetLastError()); return LORA_B200_OK; }
 
+// LORA_B200_OK when the K1 kernels serve this decoder's configuration, else the error that `what` needs them
+int need_k1(const lora_b200_decoder *d, const char *what) {
+    if (d->k1_osr) return LORA_B200_OK;
+    return fail(LORA_B200_EUNSUPPORTED, "%s needs samp_rate/bandwidth == 8 or 2 and SF7..SF12", what);
+}
+
+// the `otherwise` of a dispatch on the decoder's SF
+auto unsupported_sf(const lora_b200_decoder *d) {
+    return [d] { return fail(LORA_B200_EUNSUPPORTED, "unsupported SF %u", d->cfg.sf); };
+}
+
 // ---- K1 launch -----------------------------------------------------------------------------
-template <int SF, int D = 8>
+template <int SF, int D>
 int k1_launch_generic(const K1Launch &k) {
     using C = K1Cfg<SF, D>;
-    static DeviceOnce once;
     const size_t smem = sizeof(float2) * C::SMEM_ELEMS;
-    K1_CU(once(k.device, [&] { return cudaFuncSetAttribute(k1_fft_kernel<SF, D>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem); }));
+    K1_CU(opt_in_smem((const void *)k1_fft_kernel<SF, D>, k.device, smem));
     const size_t n_work = ((k.a.n_symbols + C::G - 1) / C::G) * C::S;
     const int grid = (int)std::min<size_t>(n_work, (size_t)k.n_sms * 2);
     k1_fft_kernel<SF, D><<<grid, K1_THREADS, smem, k.st>>>(k.a, k.bins, k.mags, k.packed);
@@ -242,9 +253,8 @@ int k1_launch_generic(const K1Launch &k) {
 
 // SF10: one 256-thread group per symbol, two radix-32 passes (k1_sf10.cuh)
 int k1_launch_sf10(const K1Launch &k) {
-    static DeviceOnce once;
     const size_t smem = sizeof(S10Smem<2>);
-    K1_CU(once(k.device, [&] { return cudaFuncSetAttribute(k1_sf10_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem); }));
+    K1_CU(opt_in_smem((const void *)k1_sf10_kernel<2>, k.device, smem));
     const int grid = (int)std::min<size_t>(k.a.n_symbols, (size_t)k.n_sms);
     k1_sf10_kernel<2><<<grid, S10_T, smem, k.st>>>(k.a, k.bins, k.mags);
     K1_CU(cudaGetLastError());
@@ -266,49 +276,37 @@ bool k1_generic() {
     return v == 1;
 }
 
-K1Launcher k1_launcher(int sf, bool generic) {
-    switch (generic ? -sf : sf) {
+// fs/bw = 8: each SF's own kernel, each one a separate measured choice (DESIGN.md 5)
+K1Launcher k1_launcher(int sf) {
+    switch (sf) {
     case 7: return k1_launch_warp7;                  // k1_packed.cu
     case 8: return k1_launch_group<8, 6, 2>;         // a group of 2 warps per symbol (k1_group.cuh)
     case 9: return k1_launch_group9;                 // k1_packed.cu
     case 10: return k1_launch_sf10;
     case 11: return k1_launch_rows<11>;              // every sample stays inside one SM (k1_rows.cuh, k1_rows.cu)
     case 12: return k1_launch_rows<12>;              // a cluster of two CTAs per symbol
-    case -7: return k1_launch_generic<7>;
-    case -8: return k1_launch_generic<8>;
-    case -9: return k1_launch_generic<9>;
-    case -10: return k1_launch_generic<10>;
-    case -11: return k1_launch_generic<11>;
-    case -12: return k1_launch_generic<12>;
     }
     return nullptr;
 }
 
-// fs/bw = 2: the generic kernel at D = 2 for every SF (it splits a symbol at SF12 only)
-K1Launcher k1_launcher_osr2(int sf) {
+// the generic kernel k1_fft_kernel<SF, D>: every SF at fs/bw = 2 (where it splits a symbol at SF12 only), and at fs/bw = 8
+// when `generic` is set
+K1Launcher k1_launcher_generic(int sf, int osr) {
     static_assert(K1Cfg<11, 2>::S == 1 && K1Cfg<12, 2>::S == 2, "k1_fft_kernel<SF, 2> splits SF12 only");
-    switch (sf) {
-    case 7: return k1_launch_generic<7, 2>;
-    case 8: return k1_launch_generic<8, 2>;
-    case 9: return k1_launch_generic<9, 2>;
-    case 10: return k1_launch_generic<10, 2>;
-    case 11: return k1_launch_generic<11, 2>;
-    case 12: return k1_launch_generic<12, 2>;
-    }
-    return nullptr;
+    return with_sf_osr(sf, osr, [] { return K1Launcher(); }, [](auto SF, auto D) -> K1Launcher { return k1_launch_generic<SF, D>; });
 }
 
 int dispatch_k1_impl(lora_b200_decoder *d, K1Scratch &ks, const float2 *iq, size_t n, uint32_t *bins, float *mags, cudaStream_t st) {
-    if (!d->k1_ok && !d->k1_osr2) return fail(LORA_B200_EUNSUPPORTED, "FFT demodulator needs samp_rate/bandwidth == 8 or 2 and SF7..SF12");
+    if (int rc = need_k1(d, "FFT demodulator")) return rc;
     if (n == 0) return LORA_B200_OK;
     static const char *rows = getenv("LORA_B200_K1_ROWS");
     const int sf = (int)d->cfg.sf;
     const bool generic = k1_generic() || (sf >= 11 && rows && rows[0] == '0');
-    const K1Launcher launch = d->k1_osr2 ? k1_launcher_osr2(sf) : k1_launcher(sf, generic);
+    const K1Launcher launch = d->k1_osr == 8 && !generic ? k1_launcher(sf) : k1_launcher_generic(sf, d->k1_osr);
     if (!launch) return fail(LORA_B200_EUNSUPPORTED, "unsupported SF %u", d->cfg.sf);
     // the kernels that split a symbol (every SF12 kernel, the generic one at SF11 at fs/bw = 8) merge partial argmax keys in
     // ks.packed
-    const bool split = sf == 12 || (sf == 11 && generic && !d->k1_osr2);
+    const bool split = sf == 12 || (sf == 11 && generic && d->k1_osr == 8);
     if (split) {
         CU(ks.packed.reserve(n));
         CU(cudaMemsetAsync(ks.packed, 0, sizeof(unsigned long long) * n, st));
@@ -343,9 +341,8 @@ int dispatch_k1(lora_b200_decoder *d, K1Scratch &ks, const float2 *iq, size_t n,
 template <int SF, int D>
 int llr_launch(lora_b200_decoder *d, const float2 *iq, size_t n, bool reduced, float *llrs, uint32_t *bins, cudaStream_t st) {
     using C = K1Cfg<SF, D>;
-    static DeviceOnce once;
     const size_t smem = sizeof(float2) * C::SMEM_ELEMS;
-    CU(once(d->device, [&] { return cudaFuncSetAttribute(k1_llr_kernel<SF, D>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem); }));
+    CU(opt_in_smem((const void *)k1_llr_kernel<SF, D>, d->device, smem));
     const size_t n_batches = (n + C::G - 1) / C::G;
     const int grid = (int)std::min<size_t>(n_batches, (size_t)d->n_sms * 2);
     k1_llr_kernel<SF, D><<<grid, K1_THREADS, smem, st>>>(K1Args{iq, tab<float2>(d, d->toff.down), tab<float2>(d, d->toff.tw), n},
@@ -353,23 +350,11 @@ int llr_launch(lora_b200_decoder *d, const float2 *iq, size_t n, bool reduced, f
     return launched(d);
 }
 
-template <int D>
-int dispatch_llr_d(lora_b200_decoder *d, const float2 *iq, size_t n, bool reduced, float *llrs, uint32_t *bins, cudaStream_t st) {
-    switch (d->cfg.sf) {
-    case 7: return llr_launch<7, D>(d, iq, n, reduced, llrs, bins, st);
-    case 8: return llr_launch<8, D>(d, iq, n, reduced, llrs, bins, st);
-    case 9: return llr_launch<9, D>(d, iq, n, reduced, llrs, bins, st);
-    case 10: return llr_launch<10, D>(d, iq, n, reduced, llrs, bins, st);
-    case 11: return llr_launch<11, D>(d, iq, n, reduced, llrs, bins, st);
-    case 12: return llr_launch<12, D>(d, iq, n, reduced, llrs, bins, st);
-    }
-    return fail(LORA_B200_EUNSUPPORTED, "unsupported SF %u", d->cfg.sf);
-}
-
 int dispatch_llr(lora_b200_decoder *d, const float2 *iq, size_t n, bool reduced, float *llrs, uint32_t *bins, cudaStream_t st) {
-    if (!d->k1_ok && !d->k1_osr2) return fail(LORA_B200_EUNSUPPORTED, "the LLR demodulator needs samp_rate/bandwidth == 8 or 2 and SF7..SF12");
+    if (int rc = need_k1(d, "the LLR demodulator")) return rc;
     if (n == 0) return LORA_B200_OK;
-    return d->k1_osr2 ? dispatch_llr_d<2>(d, iq, n, reduced, llrs, bins, st) : dispatch_llr_d<8>(d, iq, n, reduced, llrs, bins, st);
+    return with_sf_osr(d->cfg.sf, d->k1_osr, unsupported_sf(d),
+                       [&](auto SF, auto D) { return llr_launch<SF, D>(d, iq, n, reduced, llrs, bins, st); });
 }
 
 // ---- stream-path launch -----------------------------------------------------------------------
@@ -378,8 +363,7 @@ int launch_rx_t(lora_b200_decoder *d, const RxParams &p, int grid, cudaStream_t 
     size_t smem = 0;
     if (FFT) {
         smem = sizeof(float2) * K1Cfg<SF>::SMEM_ELEMS;
-        static DeviceOnce once;
-        CU(once(d->device, [&] { return cudaFuncSetAttribute(rx_stream_kernel<SF, FFT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem); }));
+        CU(opt_in_smem((const void *)rx_stream_kernel<SF, FFT>, d->device, smem));
     }
     rx_stream_kernel<SF, FFT><<<grid, RX_THREADS, smem, st>>>(p);
     return launched(d);
@@ -390,9 +374,8 @@ bool rx_warp_path(const lora_b200_decoder *d) { return d->cfg.sf == 7 && d->sps 
 
 template <bool FFT>
 int launch_rx_warp(lora_b200_decoder *d, const RxParams &p, int n_streams, cudaStream_t st) {
-    static DeviceOnce once;
     const size_t smem = sizeof(RWSmem);
-    CU(once(d->device, [&] { return cudaFuncSetAttribute(rx_warp_kernel<FFT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem); }));
+    CU(opt_in_smem((const void *)rx_warp_kernel<FFT>, d->device, smem));
     rx_warp_kernel<FFT><<<(n_streams + RW_WARPS - 1) / RW_WARPS, RW_WARPS * 32, smem, st>>>(p);
     return launched(d);
 }
@@ -401,14 +384,8 @@ int launch_rx(lora_b200_decoder *d, const RxParams &p, int grid, cudaStream_t st
     const bool fft = d->cfg.demod == LORA_B200_DEMOD_FFT;
     if (rx_warp_path(d)) return fft ? launch_rx_warp<true>(d, p, grid, st) : launch_rx_warp<false>(d, p, grid, st);
     if (!fft) return launch_rx_t<7, false>(d, p, grid, st);       // SF is a run-time value on the gradient path
-    switch (d->cfg.sf) {                                          // (the FFT demodulator at SF7 always has sps = RW_SPS)
-    case 8: return launch_rx_t<8, true>(d, p, grid, st);
-    case 9: return launch_rx_t<9, true>(d, p, grid, st);
-    case 10: return launch_rx_t<10, true>(d, p, grid, st);
-    case 11: return launch_rx_t<11, true>(d, p, grid, st);
-    case 12: return launch_rx_t<12, true>(d, p, grid, st);
-    }
-    return fail(LORA_B200_EUNSUPPORTED, "unsupported SF %u", d->cfg.sf);
+    // the FFT demodulator at SF7 always has sps = RW_SPS, so rx_stream_kernel<7, true> is not built
+    return with_sf<8, 12>(d->cfg.sf, unsupported_sf(d), [&](auto SF) { return launch_rx_t<SF, true>(d, p, grid, st); });
 }
 
 void append_hex(std::string &s, const uint8_t *v, size_t n, bool endline, bool ascii) {   // print_vector_hex, utilities.h:351-368
@@ -610,9 +587,8 @@ lora_b200_decoder *lora_b200_create(const lora_b200_config *cfg) {
         fail(LORA_B200_EINVAL, "samp_rate %.1f too low for bandwidth %u", cfg->samp_rate, cfg->bandwidth);
         return nullptr;
     }
-    d->k1_ok = (d->sps == 8u * d->n_bins) && cfg->sf >= 7 && cfg->sf <= 12;
-    d->k1_osr2 = (d->sps == 2u * d->n_bins) && cfg->sf >= 7 && cfg->sf <= 12;
-    if (cfg->demod == LORA_B200_DEMOD_FFT && !d->k1_ok) {
+    d->k1_osr = (d->sps == 8u * d->n_bins || d->sps == 2u * d->n_bins) && cfg->sf >= 7 && cfg->sf <= 12 ? (int)d->decim : 0;
+    if (cfg->demod == LORA_B200_DEMOD_FFT && d->k1_osr != 8) {
         fail(LORA_B200_EUNSUPPORTED, "FFT demodulator needs samp_rate/bandwidth == 8 and SF7..SF12");
         return nullptr;
     }
@@ -725,7 +701,7 @@ int lora_b200_demod_fft_dev(lora_b200_decoder *d, const void *iq, size_t n_symbo
 
 int lora_b200_demod_llr_dev(lora_b200_decoder *d, const void *iq, size_t n_symbols, int reduced, float *llrs, uint32_t *bins, void *stream) {
     if (!d || (n_symbols && (!iq || !llrs))) return fail(LORA_B200_EINVAL, "null argument");
-    if (!d->k1_ok && !d->k1_osr2) return fail(LORA_B200_EUNSUPPORTED, "the LLR demodulator needs samp_rate/bandwidth == 8 or 2 and SF7..SF12");
+    if (int rc = need_k1(d, "the LLR demodulator")) return rc;
     if (((uintptr_t)iq & 15u) != 0) return fail(LORA_B200_EINVAL, "iq must be 16-byte aligned");
     if (reduced != 0 && reduced != 1) return fail(LORA_B200_EINVAL, "reduced must be 0 or 1, got %d", reduced);
     CU(cudaSetDevice(d->device));
@@ -736,7 +712,7 @@ int lora_b200_demod_llr_dev(lora_b200_decoder *d, const void *iq, size_t n_symbo
 // own keys / exchange scratch).  elem = 8: gr_complex; elem = 4: int16 I/Q, converted on the device right after the copy.
 static int demod_fft_host_any(lora_b200_decoder *d, const void *iq, size_t elem, float scale, size_t n_symbols, uint32_t *bins, float *mags) {
     if (!d || (!iq && n_symbols) || (!bins && n_symbols)) return fail(LORA_B200_EINVAL, "null argument");
-    if (!d->k1_ok && !d->k1_osr2) return fail(LORA_B200_EUNSUPPORTED, "FFT demodulator needs samp_rate/bandwidth == 8 or 2 and SF7..SF12");
+    if (int rc = need_k1(d, "FFT demodulator")) return rc;
     CU(cudaSetDevice(d->device));
     const size_t sym_bytes = sizeof(float2) * (size_t)d->sps, sym_in = elem * (size_t)d->sps;
     const bool sc16 = elem == 4;
@@ -1102,44 +1078,25 @@ static int rs_launch_sync(lora_b200_decoder *d, const float2 *x, size_t stride, 
     const size_t smem = sizeof(float2) * K1Cfg<SF, D>::SMEM_ELEMS;
     const uint32_t ng = d->cfg.n_streams / m;
     if (m == 1) {
-        static DeviceOnce once;
-        CU(once(d->device, [&] { return cudaFuncSetAttribute(rs_sync_kernel<SF, D, DRIFT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem); }));
+        CU(opt_in_smem((const void *)rs_sync_kernel<SF, D, DRIFT>, d->device, smem));
         rs_sync_kernel<SF, D, DRIFT><<<d->cfg.n_streams * cap, RX_THREADS, smem, d->rx_stream>>>(
             x, stride, n_items, tab<float2>(d, d->toff.down), tab<float2>(d, d->toff.up), tab<float2>(d, d->toff.tw), rp, d->d_rs_cands,
             d->d_rs_ncand, cap, d->d_rs_frames, d->d_rs_nframes, d->cfg.n_streams * cap, d->d_rs_hold);
         return launched(d);
     }
-    static DeviceOnce once_m;
-    CU(once_m(d->device, [&] {
-        return cudaFuncSetAttribute(rs_sync_antennas_kernel<SF, D, DRIFT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    }));
+    CU(opt_in_smem((const void *)rs_sync_antennas_kernel<SF, D, DRIFT>, d->device, smem));
     rs_sync_antennas_kernel<SF, D, DRIFT><<<ng * cap, RX_THREADS, smem, d->rx_stream>>>(
         x, stride, n_items, m, tab<float2>(d, d->toff.down), tab<float2>(d, d->toff.up), tab<float2>(d, d->toff.tw), rp, d->d_rs_cands,
         d->d_rs_ncand, cap, d->d_rs_frames, d->d_rs_nframes, ng * cap, d->d_rs_hold, d->d_rs_chan);
     return launched(d);
 }
 
-template <int D, bool DRIFT>
-static int rs_sync_sf(lora_b200_decoder *d, const float2 *x, size_t stride, size_t n_items, const RsParams &rp, uint32_t cap, uint32_t m) {
-    switch (d->cfg.sf) {
-    case 7: return rs_launch_sync<7, D, DRIFT>(d, x, stride, n_items, rp, cap, m);
-    case 8: return rs_launch_sync<8, D, DRIFT>(d, x, stride, n_items, rp, cap, m);
-    case 9: return rs_launch_sync<9, D, DRIFT>(d, x, stride, n_items, rp, cap, m);
-    case 10: return rs_launch_sync<10, D, DRIFT>(d, x, stride, n_items, rp, cap, m);
-    case 11: return rs_launch_sync<11, D, DRIFT>(d, x, stride, n_items, rp, cap, m);
-    case 12: return rs_launch_sync<12, D, DRIFT>(d, x, stride, n_items, rp, cap, m);
-    }
-    return fail(LORA_B200_EUNSUPPORTED, "unsupported SF %u", d->cfg.sf);
-}
-
 // without a clock offset the synchroniser runs its DRIFT = false instantiation, which does no drift arithmetic; D = sps / N
 // (8 or 2) selects the K1 phase functions of its argmax windows
-template <int D>
-static int rs_sync_d(lora_b200_decoder *d, const float2 *x, size_t stride, size_t n_items, const RsParams &rp, uint32_t cap, uint32_t m) {
-    return rs_drift(rp) ? rs_sync_sf<D, true>(d, x, stride, n_items, rp, cap, m) : rs_sync_sf<D, false>(d, x, stride, n_items, rp, cap, m);
-}
 static int rs_sync(lora_b200_decoder *d, const float2 *x, size_t stride, size_t n_items, const RsParams &rp, uint32_t cap, uint32_t m) {
-    return d->k1_osr2 ? rs_sync_d<2>(d, x, stride, n_items, rp, cap, m) : rs_sync_d<8>(d, x, stride, n_items, rp, cap, m);
+    return with_sf_osr(d->cfg.sf, d->k1_osr, unsupported_sf(d), [&](auto SF, auto D) {
+        return with_bool(rs_drift(rp), [&](auto DRIFT) { return rs_launch_sync<SF, D, DRIFT>(d, x, stride, n_items, rp, cap, m); });
+    });
 }
 
 // the combined screen of ng receivers with m antennas: k1_antennas_kernel over the n_win windows of each row (rows `stride`
@@ -1148,32 +1105,19 @@ template <int SF, int D>
 static int rs_screen_launch(lora_b200_decoder *d, const float2 *x, size_t n_win, size_t stride, uint32_t m, uint32_t ng, size_t out_stride,
                             uint32_t *bins, float *mags, cudaStream_t st) {
     using C = K1Cfg<SF, D>;
-    static DeviceOnce once;
     const size_t smem = sizeof(float2) * C::SMEM_ELEMS;
-    CU(once(d->device, [&] { return cudaFuncSetAttribute(k1_antennas_kernel<SF, D>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem); }));
+    CU(opt_in_smem((const void *)k1_antennas_kernel<SF, D>, d->device, smem));
     const size_t n_work = (n_win + C::G - 1) / C::G * ng;
     const int grid = (int)std::min<size_t>(n_work, (size_t)d->n_sms * 2);
     k1_antennas_kernel<SF, D><<<grid, K1_THREADS, smem, st>>>(K1Args{x, tab<float2>(d, d->toff.down), tab<float2>(d, d->toff.tw), n_win},
                                                              stride, m, ng, out_stride, bins, mags);
     return launched(d);
 }
-template <int D>
-static int rs_screen_d(lora_b200_decoder *d, const float2 *x, size_t n_win, size_t stride, uint32_t m, uint32_t ng, size_t out_stride,
-                       uint32_t *bins, float *mags, cudaStream_t st) {
-    switch (d->cfg.sf) {
-    case 7: return rs_screen_launch<7, D>(d, x, n_win, stride, m, ng, out_stride, bins, mags, st);
-    case 8: return rs_screen_launch<8, D>(d, x, n_win, stride, m, ng, out_stride, bins, mags, st);
-    case 9: return rs_screen_launch<9, D>(d, x, n_win, stride, m, ng, out_stride, bins, mags, st);
-    case 10: return rs_screen_launch<10, D>(d, x, n_win, stride, m, ng, out_stride, bins, mags, st);
-    case 11: return rs_screen_launch<11, D>(d, x, n_win, stride, m, ng, out_stride, bins, mags, st);
-    case 12: return rs_screen_launch<12, D>(d, x, n_win, stride, m, ng, out_stride, bins, mags, st);
-    }
-    return fail(LORA_B200_EUNSUPPORTED, "unsupported SF %u", d->cfg.sf);
-}
 static int rs_screen(lora_b200_decoder *d, const float2 *x, size_t n_win, size_t stride, uint32_t m, uint32_t ng, size_t out_stride,
                      uint32_t *bins, float *mags, cudaStream_t st) {
-    return d->k1_osr2 ? rs_screen_d<2>(d, x, n_win, stride, m, ng, out_stride, bins, mags, st)
-                      : rs_screen_d<8>(d, x, n_win, stride, m, ng, out_stride, bins, mags, st);
+    return with_sf_osr(d->cfg.sf, d->k1_osr, unsupported_sf(d), [&](auto SF, auto D) {
+        return rs_screen_launch<SF, D>(d, x, n_win, stride, m, ng, out_stride, bins, mags, st);
+    });
 }
 
 // the data windows of frames [slots], as rs_assemble_kernel (m = 1) or combined over m antennas
@@ -1195,7 +1139,7 @@ static int rs_receive(lora_b200_decoder *d, const void *iq, size_t n_items, size
                       const lora_b200_rx_params *prm, size_t *consumed) {
     if (!d || !consumed || (!iq && n_items)) return fail(LORA_B200_EINVAL, "null argument");
     if (stride_items < n_items) return fail(LORA_B200_EINVAL, "stride_items %zu < n_items %zu", stride_items, n_items);
-    if (!d->k1_ok && !d->k1_osr2) return fail(LORA_B200_EUNSUPPORTED, "the dechirp receiver needs samp_rate/bandwidth == 8 or 2 and SF7..SF12");
+    if (int rc = need_k1(d, "the dechirp receiver")) return rc;
     lora_b200_rx_params P;
     memset(&P, 0, sizeof P);
     if (prm) P = *prm;
@@ -1466,7 +1410,7 @@ size_t lora_b200_rx_channels_last(lora_b200_decoder *d, const float **h, uint32_
 int lora_b200_demod_fft_antennas_dev(lora_b200_decoder *d, const void *iq, uint32_t n_groups, uint32_t n_antennas, size_t n_symbols,
                                      size_t row_stride_items, uint32_t *bins, float *mags, void *cuda_stream) {
     if (!d || (n_symbols && n_groups && (!iq || !bins || !mags))) return fail(LORA_B200_EINVAL, "null argument");
-    if (!d->k1_ok && !d->k1_osr2) return fail(LORA_B200_EUNSUPPORTED, "the combined screen needs samp_rate/bandwidth == 8 or 2 and SF7..SF12");
+    if (int rc = need_k1(d, "the combined screen")) return rc;
     if (n_antennas < 1 || n_antennas > (uint32_t)RS_MAX_ANTENNAS) return fail(LORA_B200_EINVAL, "n_antennas must be 1..%d, got %u", RS_MAX_ANTENNAS, n_antennas);
     if (row_stride_items < n_symbols * d->sps || row_stride_items % 2 || ((uintptr_t)iq & 15u))
         return fail(LORA_B200_EINVAL, "rows must hold n_symbols windows, start 16-byte aligned and lie an even number of samples apart");
@@ -1496,7 +1440,7 @@ extern "C" {
 int lora_b200_rs_window_dev(lora_b200_decoder *d, const void *iq, size_t n_items, size_t n, const int64_t *pos, const float *cfo_bins,
                             const int32_t *up, const int32_t *bin, void *out, float *energy) {
     if (!d || (n && (!iq || !pos || !cfo_bins || !up || !bin || !out))) return fail(LORA_B200_EINVAL, "null argument");
-    if (!d->k1_ok && !d->k1_osr2) return fail(LORA_B200_EUNSUPPORTED, "the dechirp receiver needs samp_rate/bandwidth == 8 or 2 and SF7..SF12");
+    if (int rc = need_k1(d, "the dechirp receiver")) return rc;
     if (n > 0x7FFFFFFFu) return fail(LORA_B200_EINVAL, "too many windows: %zu", n);
     const long long sps = d->sps, N = d->n_bins;
     std::vector<RsWindowQuery> q(n);
@@ -1515,16 +1459,9 @@ int lora_b200_rs_window_dev(lora_b200_decoder *d, const void *iq, size_t n_items
     DeviceBuffer<RsWindowQuery> dq;
     CU(dq.reserve(n));
     CU(cudaMemcpyAsync(dq, q.data(), sizeof(RsWindowQuery) * n, cudaMemcpyHostToDevice, d->rx_stream));
-    const float2 *x = (const float2 *)iq;
-    int rc = LORA_B200_EUNSUPPORTED;
-    switch (d->cfg.sf) {
-    case 7: rc = rs_window_launch<7>(d, x, n_items, dq, n, (float2 *)out, energy); break;
-    case 8: rc = rs_window_launch<8>(d, x, n_items, dq, n, (float2 *)out, energy); break;
-    case 9: rc = rs_window_launch<9>(d, x, n_items, dq, n, (float2 *)out, energy); break;
-    case 10: rc = rs_window_launch<10>(d, x, n_items, dq, n, (float2 *)out, energy); break;
-    case 11: rc = rs_window_launch<11>(d, x, n_items, dq, n, (float2 *)out, energy); break;
-    case 12: rc = rs_window_launch<12>(d, x, n_items, dq, n, (float2 *)out, energy); break;
-    }
+    const int rc = with_sf<7, 12>(d->cfg.sf, unsupported_sf(d), [&](auto SF) {
+        return rs_window_launch<SF>(d, (const float2 *)iq, n_items, dq, n, (float2 *)out, energy);
+    });
     CU(cudaStreamSynchronize(d->rx_stream));     // (before dq is freed)
     return rc;
 }
