@@ -67,7 +67,8 @@ SIGNATURES = {
     "lora_b200_demod_fft_host": (_i, [_vp, _vp, _sz, _vp, _vp]),
     "lora_b200_demod_llr_dev": (_i, [_vp, _vp, _sz, _i, _vp, _vp, _vp]),
     "lora_b200_demod_fft_antennas_dev": (_i, [_vp, _vp, _u32, _u32, _sz, _sz, _vp, _vp, _vp]),
-    "lora_b200_rs_window_dev": (_i, [_vp, _vp, _sz, _sz, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "lora_b200_rs_window_dev": (_i, [_vp, _vp, _sz, _u32, _sz, _sz, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "lora_b200_rs_frame_dev": (_i, [_vp, _vp, _sz, _u32, _sz, _sz, _vp, _vp, _vp, _vp, _u32, _u32, _vp, _vp, _vp]),
     "lora_b200_demod_fft_host_sc16": (_i, [_vp, _vp, C.c_float, _sz, _vp, _vp]),
     "lora_b200_demod_gradient_dev": (_i, [_vp, _vp, _sz, _vp, _vp]),
     "lora_b200_ifreq_dev": (_i, [_vp, _vp, _sz, _u32, _vp, _vp]),

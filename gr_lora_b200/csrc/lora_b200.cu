@@ -1426,21 +1426,36 @@ static_assert(sizeof(lora_b200_rx_info) == 32 && sizeof(lora_b200_rx_params) == 
 
 }  // extern "C"
 
-template <int SF>
-static int rs_window_launch(lora_b200_decoder *d, const float2 *x, size_t n_items, const RsWindowQuery *q, size_t n, float2 *out,
-                            float *energy) {
-    rs_window_kernel<SF><<<(unsigned)n, RX_THREADS, 0, d->rx_stream>>>(x, (long long)n_items, tab<float2>(d, d->toff.down),
-                                                                       tab<float2>(d, d->toff.up), tab<float2>(d, d->toff.tw), d->sps, q,
-                                                                       out, energy);
+template <int SF, int D>
+static int rs_window_launch(lora_b200_decoder *d, const float2 *x, size_t stride, size_t n_items, uint32_t m, const RsWindowQuery *q,
+                            size_t n, float2 *out, float *energy, unsigned long long *key) {
+    const size_t smem = sizeof(float2) * K1Cfg<SF, D>::SMEM_ELEMS;   // (the synchronise kernels' dynamic shared memory)
+    CU(opt_in_smem((const void *)rs_window_kernel<SF, D>, d->device, smem));
+    rs_window_kernel<SF, D><<<(unsigned)n, RX_THREADS, smem, d->rx_stream>>>(x, stride, (long long)n_items, m, tab<float2>(d, d->toff.down),
+                                                                             tab<float2>(d, d->toff.up), tab<float2>(d, d->toff.tw), d->sps,
+                                                                             q, out, energy, key);
+    return launched(d);
+}
+
+template <int SF, int D, bool DRIFT>
+static int rs_channels_launch(lora_b200_decoder *d, const float2 *x, size_t stride, size_t n_items, uint32_t m, const RsParams &rp,
+                              const RsFrame *frames, size_t n, float2 *chan, float *snr_db) {
+    rs_channels_kernel<SF, D, DRIFT><<<(unsigned)n, RX_THREADS, 0, d->rx_stream>>>(x, stride, n_items, m, tab<float2>(d, d->toff.down),
+                                                                                  tab<float2>(d, d->toff.up), tab<float2>(d, d->toff.tw),
+                                                                                  rp, frames, chan, snr_db);
     return launched(d);
 }
 
 extern "C" {
 
-int lora_b200_rs_window_dev(lora_b200_decoder *d, const void *iq, size_t n_items, size_t n, const int64_t *pos, const float *cfo_bins,
-                            const int32_t *up, const int32_t *bin, void *out, float *energy) {
-    if (!d || (n && (!iq || !pos || !cfo_bins || !up || !bin || !out))) return fail(LORA_B200_EINVAL, "null argument");
+int lora_b200_rs_window_dev(lora_b200_decoder *d, const void *iq, size_t n_items, uint32_t m, size_t stride_items, size_t n,
+                            const int64_t *pos, const float *cfo_bins, const int32_t *up, const int32_t *bin, void *out, float *energy,
+                            uint32_t *argmax_bin, float *argmax_mag) {
+    if (!d || (n && (!iq || !pos || !cfo_bins || !up || !bin || !out)))
+        return fail(LORA_B200_EINVAL, "null argument");
     if (int rc = need_k1(d, "the dechirp receiver")) return rc;
+    if (m < 1 || m > (uint32_t)RS_MAX_ANTENNAS) return fail(LORA_B200_EINVAL, "m must be 1..%d, got %u", RS_MAX_ANTENNAS, m);
+    if (m > 1 && stride_items < n_items) return fail(LORA_B200_EINVAL, "stride_items %zu < n_items %zu", stride_items, n_items);
     if (n > 0x7FFFFFFFu) return fail(LORA_B200_EINVAL, "too many windows: %zu", n);
     const long long sps = d->sps, N = d->n_bins;
     std::vector<RsWindowQuery> q(n);
@@ -1457,12 +1472,76 @@ int lora_b200_rs_window_dev(lora_b200_decoder *d, const void *iq, size_t n_items
     CU(cudaSetDevice(d->device));
     if (n == 0) return LORA_B200_OK;
     DeviceBuffer<RsWindowQuery> dq;
+    DeviceBuffer<unsigned long long> dk;
     CU(dq.reserve(n));
+    CU(dk.reserve(n));
     CU(cudaMemcpyAsync(dq, q.data(), sizeof(RsWindowQuery) * n, cudaMemcpyHostToDevice, d->rx_stream));
-    const int rc = with_sf<7, 12>(d->cfg.sf, unsupported_sf(d), [&](auto SF) {
-        return rs_window_launch<SF>(d, (const float2 *)iq, n_items, dq, n, (float2 *)out, energy);
+    int rc = with_sf_osr(d->cfg.sf, d->k1_osr, unsupported_sf(d), [&](auto SF, auto D) {
+        return rs_window_launch<SF, D>(d, (const float2 *)iq, stride_items, n_items, m, dq, n, (float2 *)out, energy, dk);
     });
-    CU(cudaStreamSynchronize(d->rx_stream));     // (before dq is freed)
+    std::vector<unsigned long long> keys(n);
+    if (rc == LORA_B200_OK) CU(cudaMemcpyAsync(keys.data(), dk, sizeof(unsigned long long) * n, cudaMemcpyDeviceToHost, d->rx_stream));
+    CU(cudaStreamSynchronize(d->rx_stream));     // (before dq and dk are freed)
+    if (rc != LORA_B200_OK) return rc;
+    std::vector<uint32_t> kb(n);
+    std::vector<float> km(n);
+    for (size_t i = 0; i < n; i++) k1_store(kb.data(), km.data(), i, keys[i]);
+    if (argmax_bin) CU(cudaMemcpy(argmax_bin, kb.data(), sizeof(uint32_t) * n, cudaMemcpyHostToDevice));
+    if (argmax_mag) CU(cudaMemcpy(argmax_mag, km.data(), sizeof(float) * n, cudaMemcpyHostToDevice));
+    return LORA_B200_OK;
+}
+
+int lora_b200_rs_frame_dev(lora_b200_decoder *d, const void *iq, size_t n_items, uint32_t m, size_t stride_items, size_t n,
+                           const uint32_t *group, const int64_t *start, const float *cfo_bins, const float *sfo_ppm, uint32_t first,
+                           uint32_t cnt, void *chan, float *snr_db, void *windows) {
+    if (!d || (n && (!iq || !group || !start || !cfo_bins || !sfo_ppm || (cnt && !windows) || (m > 1 && (!chan || !snr_db)))))
+        return fail(LORA_B200_EINVAL, "null argument");
+    if (int rc = need_k1(d, "the dechirp receiver")) return rc;
+    if (m < 1 || m > (uint32_t)RS_MAX_ANTENNAS) return fail(LORA_B200_EINVAL, "m must be 1..%d, got %u", RS_MAX_ANTENNAS, m);
+    if (stride_items < n_items) return fail(LORA_B200_EINVAL, "stride_items %zu < n_items %zu", stride_items, n_items);
+    if (n > 0x7FFFFFFFu || (size_t)cnt * n > 0xFFFFFFFFu) return fail(LORA_B200_EINVAL, "too many frames or windows: %zu x %u", n, cnt);
+    const uint32_t sps = d->sps;
+    std::vector<RsFrame> fr(n);
+    bool drift = false;
+    for (size_t i = 0; i < n; i++) {
+        if (!std::isfinite(cfo_bins[i]) || std::fabs(cfo_bins[i]) > (float)d->n_bins || !std::isfinite(sfo_ppm[i]) || std::fabs(sfo_ppm[i]) > 1e4f)
+            return fail(LORA_B200_EINVAL, "frame %zu: cfo_bins %g or sfo_ppm %g out of range", i, (double)cfo_bins[i], (double)sfo_ppm[i]);
+        if (cnt && rs_sym(start[i], rs_data_j((long long)first), sps, sfo_ppm[i]) < 0)
+            return fail(LORA_B200_EINVAL, "frame %zu: data window %u starts before the row", i, first);
+        fr[i] = RsFrame{(long long)start[i], group[i], cfo_bins[i], 0.f, RS_OK, 0, sfo_ppm[i]};
+        drift = drift || sfo_ppm[i] != 0.f;
+    }
+    CU(cudaSetDevice(d->device));
+    if (n == 0) return LORA_B200_OK;
+    std::vector<uint32_t> tabh(2 * n);                // offs | cnts of the assemble kernels
+    for (size_t i = 0; i < n; i++) { tabh[i] = (uint32_t)(i * cnt); tabh[n + i] = cnt; }
+    DeviceBuffer<RsFrame> df;
+    DeviceBuffer<uint32_t> dt;
+    CU(df.reserve(n));
+    CU(dt.reserve(2 * n));
+    CU(cudaMemcpyAsync(df, fr.data(), sizeof(RsFrame) * n, cudaMemcpyHostToDevice, d->rx_stream));
+    CU(cudaMemcpyAsync(dt, tabh.data(), sizeof(uint32_t) * 2 * n, cudaMemcpyHostToDevice, d->rx_stream));
+    const float2 *x = (const float2 *)iq;
+    int rc = LORA_B200_OK;
+    if (m > 1) {
+        RsParams rp{sps, d->n_bins, d->decim, 0.f, 5u, {0u, 0u}, (float)d->n_bins / 4.0f, 0.f};   // (rs_channels reads sps, decim)
+        rc = with_sf_osr(d->cfg.sf, d->k1_osr, unsupported_sf(d), [&](auto SF, auto D) {
+            return with_bool(drift, [&](auto DRIFT) {
+                return rs_channels_launch<SF, D, DRIFT>(d, x, stride_items, n_items, m, rp, df, n, (float2 *)chan, snr_db);
+            });
+        });
+    }
+    if (rc == LORA_B200_OK && cnt) {
+        const int grid = std::min<int>((int)n, d->n_sms * 8);
+        if (m == 1)
+            rs_assemble_kernel<<<grid, 256, 0, d->rx_stream>>>(x, stride_items, (long long)n_items, df, (uint32_t)n, nullptr, first, dt, 0,
+                                                               dt + n, sps, (float2 *)windows);
+        else
+            rs_assemble_antennas_kernel<<<grid, 256, 0, d->rx_stream>>>(x, stride_items, (long long)n_items, m, df, (const float2 *)chan,
+                                                                        (uint32_t)n, nullptr, first, dt, 0, dt + n, sps, (float2 *)windows);
+        rc = launched(d);
+    }
+    CU(cudaStreamSynchronize(d->rx_stream));     // (before df and dt are freed)
     return rc;
 }
 

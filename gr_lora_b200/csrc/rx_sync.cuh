@@ -779,25 +779,64 @@ rs_sync_antennas_kernel(const float2 *__restrict__ iq, size_t stride, size_t n_i
 }
 
 // the synchroniser's window sums on their own (lora_b200_rs_window_dev), so that they can be held to a float64 reference:
-// one CTA per query, RsDevOps::binval and ::energy of the window at pos
+// one CTA per query on a group of m rows `stride` apart, with the Ops the synchronise kernels run -- RsDevOps (m = 1,
+// rs_sync_kernel) or RsAntOps (m >= 2, rs_sync_antennas_kernel): each antenna's binval and energy of the window at pos,
+// and the argmax key of the (combined) spectrum there, dechirped with the chirp of the query
 struct RsWindowQuery {
     long long pos;
     float cfo_bins;
     int32_t up, bin, pad;
 };
 
-template <int SF>
+template <int SF, int D>
 __global__ void __launch_bounds__(RX_THREADS)
-rs_window_kernel(const float2 *__restrict__ x, long long n_items, const float2 *down, const float2 *up, const float2 *tw, uint32_t sps,
-                 const RsWindowQuery *__restrict__ q, float2 *__restrict__ out, float *__restrict__ energy) {
+rs_window_kernel(const float2 *__restrict__ x, size_t stride, long long n_items, uint32_t m, const float2 *down, const float2 *up,
+                 const float2 *tw, uint32_t sps, const RsWindowQuery *__restrict__ q, float2 *__restrict__ out, float *__restrict__ energy,
+                 unsigned long long *__restrict__ key) {
+    extern __shared__ float2 rs_dyn_smem[];
     __shared__ RxShared sh;
-    RsDevOps<SF> ops{x, n_items, down, up, tw, sps, nullptr, &sh};   // (binval and energy use no dynamic shared memory)
     const RsWindowQuery w = q[blockIdx.x];
-    const float2 v = ops.binval(w.pos, w.cfo_bins, w.up != 0, w.bin);
-    const float e = ops.energy(w.pos);
+    float2 v[RS_MAX_ANTENNAS];
+    float e[RS_MAX_ANTENNAS];
+    unsigned long long k;
+    if (m == 1) {
+        RsDevOps<SF, D> ops{x, n_items, down, up, tw, sps, rs_dyn_smem, &sh};
+        ops.binvals(w.pos, w.cfo_bins, w.up != 0, w.bin, v);
+        e[0] = ops.energy(w.pos);
+        k = ops.argmax(w.pos, w.up != 0);
+    } else {
+        RsAntOps<SF, D> ops{{x, n_items, down, up, tw, sps, rs_dyn_smem, &sh}, stride, m};
+        ops.binvals(w.pos, w.cfo_bins, w.up != 0, w.bin, v);
+        ops.energies(w.pos, e);
+        k = ops.argmax(w.pos, w.up != 0);
+    }
     if (threadIdx.x == 0) {
-        out[blockIdx.x] = v;
-        if (energy) energy[blockIdx.x] = e;
+        for (uint32_t a = 0; a < m; a++) {
+            out[(size_t)blockIdx.x * m + a] = v[a];
+            if (energy) energy[(size_t)blockIdx.x * m + a] = e[a];
+        }
+        key[blockIdx.x] = k;
+    }
+}
+
+// the channel estimates and weights of given frames on their own (lora_b200_rs_frame_dev): one CTA per frame (group
+// frames[f].stream, rows stream * m + a), rs_channels over RsAntOps as rs_sync_antennas_kernel runs it after synchronising,
+// into chan[f][0..4) (h), chan[f][4..8) (w) and snr_db[f]
+template <int SF, int D, bool DRIFT>
+__global__ void __launch_bounds__(RX_THREADS)
+rs_channels_kernel(const float2 *__restrict__ iq, size_t stride, size_t n_items, uint32_t m, const float2 *down, const float2 *up,
+                   const float2 *tw, RsParams p, const RsFrame *__restrict__ frames, float2 *__restrict__ chan, float *__restrict__ snr_db) {
+    __shared__ RxShared sh;
+    const RsFrame r = frames[blockIdx.x];
+    RsAntOps<SF, D> ops{{iq + (size_t)r.stream * m * stride, (long long)n_items, down, up, tw, p.sps, nullptr, &sh}, stride, m};
+    float2 h[RS_MAX_ANTENNAS], w[RS_MAX_ANTENNAS];   // (rs_channels takes no argmax: no dynamic shared memory)
+    const float s = rs_channels<DRIFT>(ops, p, r, m, h, w);
+    if (threadIdx.x == 0) {
+        for (int a = 0; a < RS_MAX_ANTENNAS; a++) {
+            chan[(size_t)blockIdx.x * 2 * RS_MAX_ANTENNAS + a] = h[a];
+            chan[(size_t)blockIdx.x * 2 * RS_MAX_ANTENNAS + RS_MAX_ANTENNAS + a] = w[a];
+        }
+        snr_db[blockIdx.x] = s;
     }
 }
 

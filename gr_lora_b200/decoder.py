@@ -315,18 +315,39 @@ class decoder:
         N.check(self._L.lora_b200_demod_llr_dev(self._h, _dev_ptr(iq_dev), int(n_symbols), int(bool(reduced)), _dev_ptr(llrs_dev),
                                                _dev_ptr(bins_dev), int(cuda_stream)), "lora_b200_demod_llr_dev")
 
-    def rs_window(self, iq_dev, n_items, pos, cfo_bins, up, bins, out_dev, energy_dev=None):
-        """The dechirp receiver's window sums (lora_b200_rs_window_dev): out_dev[i] (complex64) = bin bins[i] of the window at
-        pos[i] of the row iq_dev, dechirped with the up-chirp (up[i]) or the down-chirp and de-rotated by cfo_bins[i] bins;
-        energy_dev[i] = its energy.  pos, cfo_bins, up, bins: host sequences of one length."""
+    def rs_window(self, iq_dev, n_items, pos, cfo_bins, up, bins, out_dev, energy_dev=None, argmax_bins_dev=None, argmax_mags_dev=None,
+                  antennas=1, stride=0):
+        """The dechirp receiver's window sums (lora_b200_rs_window_dev) on `antennas` rows of n_items samples, `stride` items
+        apart: out_dev[i * M + a] (complex64) = bin bins[i] of antenna a's window at pos[i], dechirped with the up-chirp (up[i])
+        or the down-chirp and de-rotated by cfo_bins[i] bins; energy_dev[i * M + a] = its energy; argmax_bins_dev[i] (int32)
+        / argmax_mags_dev[i] = the argmax bin and magnitude of the combined spectrum of the raw windows at pos[i] (each
+        output but out_dev optional).  pos, cfo_bins, up, bins: host sequences of one length."""
         p = np.ascontiguousarray(pos, dtype=np.int64)
         f = np.ascontiguousarray(cfo_bins, dtype=np.float32)
         u = np.ascontiguousarray(up, dtype=np.int32)
         b = np.ascontiguousarray(bins, dtype=np.int32)
         assert p.shape == f.shape == u.shape == b.shape and p.ndim == 1
-        N.check(self._L.lora_b200_rs_window_dev(self._h, _dev_ptr(iq_dev), int(n_items), p.size, p.ctypes.data, f.ctypes.data,
-                                               u.ctypes.data, b.ctypes.data, _dev_ptr(out_dev), _dev_ptr(energy_dev)),
+        N.check(self._L.lora_b200_rs_window_dev(self._h, _dev_ptr(iq_dev), int(n_items), int(antennas), int(stride), p.size,
+                                               p.ctypes.data, f.ctypes.data, u.ctypes.data, b.ctypes.data, _dev_ptr(out_dev),
+                                               _dev_ptr(energy_dev), _dev_ptr(argmax_bins_dev), _dev_ptr(argmax_mags_dev)),
                 "lora_b200_rs_window_dev")
+
+    def rs_frame(self, iq_dev, n_items, group, start, cfo_bins, sfo_ppm, first, cnt, windows_dev, chan_dev=None, snr_dev=None,
+                 antennas=1, stride=0):
+        """The channel estimates, weights and data windows of given frames (lora_b200_rs_frame_dev): frame i at start[i] with
+        cfo_bins[i] and sfo_ppm[i] on receiver group[i] (rows group[i] * M + a, `stride` items apart).  M >= 2: chan_dev[i]
+        (complex64[8]) = h[4] | w[4], snr_dev[i] = the combined SNR in dB.  windows_dev[(i * cnt + k) * sps ..] = its data
+        window first + k, combined over the antennas and de-rotated by its CFO.  group, start, cfo_bins, sfo_ppm: host
+        sequences of one length."""
+        g = np.ascontiguousarray(group, dtype=np.uint32)
+        s = np.ascontiguousarray(start, dtype=np.int64)
+        f = np.ascontiguousarray(cfo_bins, dtype=np.float32)
+        q = np.ascontiguousarray(sfo_ppm, dtype=np.float32)
+        assert g.shape == s.shape == f.shape == q.shape and g.ndim == 1
+        N.check(self._L.lora_b200_rs_frame_dev(self._h, _dev_ptr(iq_dev), int(n_items), int(antennas), int(stride or n_items), g.size,
+                                              g.ctypes.data, s.ctypes.data, f.ctypes.data, q.ctypes.data, int(first), int(cnt),
+                                              _dev_ptr(chan_dev), _dev_ptr(snr_dev), _dev_ptr(windows_dev)),
+                "lora_b200_rs_frame_dev")
 
     def demod_fft_host(self, iq_host, bins_out=None, mags_out=None):
         """K1 end to end from host memory (copies inside). iq_host: complex64 ndarray or (ptr, n_symbols)."""

@@ -134,13 +134,30 @@ int lora_b200_demod_fft_host(lora_b200_decoder *d, const void *iq, size_t n_symb
  * LORA_B200_EUNSUPPORTED unless samp_rate / bandwidth is 8 or 2 and SF7..SF12. */
 int lora_b200_demod_llr_dev(lora_b200_decoder *d, const void *iq, size_t n_symbols, int reduced, float *llrs, uint32_t *bins,
                             void *cuda_stream);
-/* The window sums the dechirp receiver's synchroniser (lora_b200_receive) measures, on their own, to check them against a
- * reference: for window i, out[i] = sum_n x[pos[i] + n] c[n] exp(-2 pi j (cfo_bins[i] (pos[i] + n) + bin[i] n) / sps),
- * n < sps, c the down-chirp table (up[i] = 0) or the up-chirp table (up[i] = 1), x the row iq of n_items samples; energy
- * (may be NULL) = sum |x|^2 over the window.  Every window inside the row, bin in -N/2..N/2-1, |cfo_bins| <= N.  iq, out
- * (float2[n]) and energy are device pointers, pos, cfo_bins, up and bin host arrays; returns when the results are written. */
-int lora_b200_rs_window_dev(lora_b200_decoder *d, const void *iq, size_t n_items, size_t n, const int64_t *pos, const float *cfo_bins,
-                            const int32_t *up, const int32_t *bin, void *out, float *energy);
+/* The window sums the dechirp receiver's synchroniser (lora_b200_receive, lora_b200_receive_antennas) measures, on their own,
+ * to check them against a reference.  One receiver of m (1..4) antennas, row a = iq + a * stride_items (n_items samples
+ * each; stride_items is ignored for m = 1).  For window i and antenna a, out[i * m + a] = sum_n x_a[pos[i] + n] c[n]
+ * exp(-2 pi j (cfo_bins[i] (pos[i] + n) + bin[i] n) / sps), n < sps, c the down-chirp table (up[i] = 0) or the up-chirp
+ * table (up[i] = 1); energy[i * m + a] = sum |x_a|^2 over the window; argmax_bin[i] / argmax_mag[i] = the first argmax of
+ * the combined spectrum P[k] = sum_a |tmp_a[k]|^2 of the raw windows at pos[i] dechirped with c (as
+ * lora_b200_demod_fft_antennas_dev, at any position) and sqrt(P[bin]).  m = 1 runs the one-row synchroniser's arithmetic,
+ * m >= 2 the antenna synchroniser's.  Every window inside the row, bin in -N/2..N/2-1, |cfo_bins| <= N.  iq, out
+ * (float2[n][m]), energy (float[n][m]), argmax_bin and argmax_mag are device pointers (energy, argmax_bin and argmax_mag
+ * may be NULL), pos, cfo_bins, up and bin host arrays; returns when the results are written.  Test entry point. */
+int lora_b200_rs_window_dev(lora_b200_decoder *d, const void *iq, size_t n_items, uint32_t m, size_t stride_items, size_t n,
+                            const int64_t *pos, const float *cfo_bins, const int32_t *up, const int32_t *bin, void *out, float *energy,
+                            uint32_t *argmax_bin, float *argmax_mag);
+/* The channel estimates, weights and data windows the dechirp receiver forms for given frames, on their own: frame i (start[i],
+ * its CFO cfo_bins[i] in bins, its clock offset sfo_ppm[i]) lies on receiver group[i], rows group[i] * m + a =
+ * iq + (group[i] * m + a) * stride_items, n_items samples each.  m >= 2: chan[i][0..4) = h, chan[i][4..8) = w (float2, 0 above
+ * m) and snr_db[i], as lora_b200_receive_antennas computes them after synchronising (rx_channels_last is h).  windows[(i cnt + k)
+ * sps ..] = data window first + k of frame i as the receiver demodulates it: sum_a w_a x_a (m = 1: x_0) from rs_sym(start[i],
+ * 12.25 + first + k) on, de-rotated by cfo_bins[i], 0 past n_items.  Data window `first` must start inside the row.  iq, chan
+ * (float2[n][8], m >= 2), snr_db (float[n], m >= 2) and windows (float2[n cnt sps]) are device pointers, group, start,
+ * cfo_bins and sfo_ppm host arrays; returns when the results are written.  Test entry point. */
+int lora_b200_rs_frame_dev(lora_b200_decoder *d, const void *iq, size_t n_items, uint32_t m, size_t stride_items, size_t n,
+                           const uint32_t *group, const int64_t *start, const float *cfo_bins, const float *sfo_ppm, uint32_t first,
+                           uint32_t cnt, void *chan, float *snr_db, void *windows);
 /* The combined screen of the dechirp receiver with several antennas (lora_b200_receive_antennas) on its own, so that it can be
  * held to a reference: n_groups groups of n_antennas (1..4) rows, row r = iq + r * row_stride_items, each holding n_symbols
  * aligned windows of sps samples.  For window i of group g, with tmp_a the kept bins of lora_b200_demod_fft_dev's spectrum of

@@ -95,8 +95,9 @@ def receive_emul(X, sf, osr, *, antennas=None, cr=4, rr=None, soft=False, sfo_pp
 
 def frame_rows(sf, osr, payload, cfo_hz, offset, gains, *, snr_db=None, seed=0, cr=4, rr=None, sfo_ppm=0.0, tail=3, noise_only=()):
     """One frame at sample `lead + offset` on len(gains) antennas: row a = gains[a] * frame (CFO in Hz, the transmitter's
-    clock off by sfo_ppm) + its own noise at snr_db in 125 kHz for a unit gain (None: no noise).  Rows in noise_only carry
-    noise at that level whatever snr_db is.  Returns (X [M, n] complex64, lead, frame length)."""
+    clock off by sfo_ppm) + its own noise at snr_db in 125 kHz for a unit gain (None: no noise; a sequence: one level per
+    antenna, None for a noiseless row).  Rows in noise_only carry noise at that level whatever snr_db is.  Returns (X [M, n]
+    complex64, lead, frame length)."""
     rr = sf > 10 if rr is None else rr
     fs, sps = osr * BW, osr << sf
     f = tx.modulate_frame(tx.encode_frame(payload, sf, cr, reduced_rate=rr), sf, fs=fs, sfo_ppm=sfo_ppm)
@@ -108,7 +109,8 @@ def frame_rows(sf, osr, payload, cfo_hz, offset, gains, *, snr_db=None, seed=0, 
     X = np.empty((len(gains), s.size), np.complex128)
     for a, g in enumerate(gains):
         X[a] = 0.0 if a in noise_only else g * s
-        level = snr_db if snr_db is not None else (10.0 if a in noise_only else None)
+        level = snr_db[a] if np.ndim(snr_db) else snr_db
+        level = level if level is not None else (10.0 if a in noise_only else None)
         if level is not None:
             X[a] += tx.awgn(s.size, level - 10 * np.log10(osr), rng)
     return X.astype(np.complex64), lead, f.size
@@ -133,14 +135,15 @@ def k1_batch(sf, osr, rng, n_clean=None):
 
 class CombinedReference:
     """The float64 combined spectrum P[k] = sum_a m64_a[k]^2 of M antennas' windows X [M, n, sps] (m64_a: tests/
-    k1_reference.py's |tmp| of antenna a, at fs/bw = osr), with the rounding band summed over the antennas:
+    k1_reference.py's |tmp| of antenna a, at fs/bw = osr; dechirped with the down-chirp, or with `chirp`), with the rounding
+    band summed over the antennas:
         tau_a[k] = u log2(sps) (m64_a[k] + ||y_a||),   tau_P[k] = sum_a (2 m64_a[k] + tau_a[k]) tau_a[k]."""
 
-    def __init__(self, X, sf, osr, antennas=None):
+    def __init__(self, X, sf, osr, antennas=None, chirp=None):
         X = np.asarray(X)
         m, n, sps = X.shape
         n_bins, h = 1 << sf, (1 << sf) // 2
-        c = tables(sf, osr)[0].astype(np.complex128)
+        c = (tables(sf, osr)[0] if chirp is None else np.asarray(chirp)).astype(np.complex128)
         self.P = np.zeros((n, n_bins))
         self.tauP = np.zeros((n, n_bins))
         step = max(1, CHUNK_BYTES // (16 * sps))

@@ -42,7 +42,7 @@ GROUP = {8: {7: 8, 8: 4, 9: 2, 10: 1, 11: 1, 12: 1}, 2: {7: 32, 8: 16, 9: 8, 10:
 @pytest.mark.parametrize("sf", range(7, 13))
 def test_combined_screen_against_float64(torch, sf, osr):
     """k1_antennas_kernel through lora_b200_demod_fft_antennas_dev: every bin clean (a spread at SF11/12), -3 dB, half-bin and
-    noise windows, each antenna its own symbols and gain, M = 2 and 4, two groups, in batches around the kernel's windows per
+    noise windows, each antenna its own symbols and gain, M = 2, 3 and 4, two groups, in batches around the kernel's windows per
     grid pass (more work items than CTAs): bins and magnitudes inside the band of the float64 sum_a |tmp_a|^2
     (antenna_common.CombinedReference), two runs bit-identical."""
     from antenna_common import CombinedReference, k1_batch
@@ -51,7 +51,7 @@ def test_combined_screen_against_float64(torch, sf, osr):
     per_pass = 2 * n_sms * GROUP[osr][sf]
     dec = make_dec(sf, osr)
     rng = np.random.default_rng(300 * sf + osr)
-    for m in (2, 4):
+    for m in (2, 3, 4):
         base = [k1_batch(sf, osr, np.random.default_rng(1000 * sf + 10 * osr + a), n_clean=24 if sf >= 11 else None)
                 for a in range(ng * m)]
         for n in sorted({min(b.shape[0] for b in base), per_pass // ng + 1}):
@@ -106,9 +106,9 @@ def test_one_antenna_is_byte_identical(torch, osr, soft):
 
 # ---- M = 2 against the host emulation ----------------------------------------------------------------------------------------------
 @pytest.mark.parametrize("osr", [8, 2])
-@pytest.mark.parametrize("sf,m", [(sf, 2) for sf in range(7, 13)] + [(7, 4), (9, 4), (12, 4)])
+@pytest.mark.parametrize("sf,m", [(sf, 2) for sf in range(7, 13)] + [(8, 3), (11, 3)] + [(7, 4), (9, 4), (12, 4)])
 def test_antennas_match_host_emulation(torch, sf, m, osr):
-    """M = 2 (every SF) and M = 4 (SF7, 9, 12) at +10 dB and at sensitivity - 1.5 dB per antenna, random relative phases and
+    """M = 2 (every SF), M = 3 (SF8, 11) and M = 4 (SF7, 9, 12) at +10 dB and at sensitivity - 1.5 dB per antenna, random relative phases and
     gains within +-3 dB: per receiver the device publishes the set of payloads the host emulation publishes (at +10 dB: the
     one sent), and frames both sides place within 2 samples of each other have the same start and payload and CFOs within 1e-3
     bin."""

@@ -10,6 +10,7 @@ from concurrent.futures import ThreadPoolExecutor
 import numpy as np
 import pytest
 
+from antenna_reference import ENERGY_TOL, window_energy, window_sum
 from test_gpu_rx_sync import SENSITIVITY, check_exact, frame_len, make_dec, sigma_for
 
 pytestmark = pytest.mark.gpu
@@ -187,7 +188,7 @@ def test_window_sums_against_float64(torch, sf):
     chirp tables: windows of frames and of noise anywhere in a row of 2^24 samples, both chirps, CFOs within +-N/4 bins
     and bins 0, +-1, the sync-word bins, -N/2, N/2 - 1 and random ones.  The error is within 2.5e-7 plus the float32 phase
     rounding of a CFO of F bins, 2 pi (|F| + 1) 2^-25, times the window's sum of |x c| (an H100 stays below 1/10 of that);
-    the energy within 1e-5."""
+    the energy within 1e-5 (antenna_reference.window_sum, which the several-antenna tests share)."""
     sps, N = 8 << sf, 1 << sf
     _, frames_row, _ = synth(torch, sf, 1, 2, 8, 10.0, seed=sf * 7 + 8)
     n = max(1 << 24, frames_row.shape[1])
@@ -208,20 +209,18 @@ def test_window_sums_against_float64(torch, sf):
     down_t, up_t, _ = dec_tables(dec)
     out = torch.zeros(m, dtype=torch.complex64, device="cuda")
     en = torch.zeros(m, dtype=torch.float32, device="cuda")
-    dec.rs_window(row, n, pos, cfo, up, bins, out, en)
+    kb = torch.zeros(m, dtype=torch.int32, device="cuda")
+    km = torch.zeros(m, dtype=torch.float32, device="cuda")
+    dec.rs_window(row, n, pos, cfo, up, bins, out, en, kb, km)
     got, got_e = out.cpu().numpy(), en.cpu().numpy()
-    k = np.arange(sps)
     worst = 0.0
     for i in range(m):
-        w = x[pos[i]: pos[i] + sps].astype(np.complex128)
-        c = (up_t if up[i] else down_t).astype(np.complex128)
-        X = np.sum(w * c * np.exp(-2j * np.pi * (float(cfo[i]) * (pos[i] + k) + float(bins[i]) * k) / sps))
-        l1 = np.sum(np.abs(w * c))
-        tol = (2.5e-7 + 2 * np.pi * (abs(float(cfo[i])) + 1) * 2.0 ** -25) * l1
+        w = x[pos[i]: pos[i] + sps]
+        X, tol = window_sum(w, up_t if up[i] else down_t, pos[i], cfo[i], bins[i])
         worst = max(worst, abs(got[i] - X) / tol)
         assert abs(got[i] - X) <= tol, (i, int(pos[i]), float(cfo[i]), int(bins[i]), int(up[i]), got[i], X, tol)
-        e = np.sum(np.abs(w) ** 2)
-        assert abs(got_e[i] - e) <= 1e-5 * e, (i, got_e[i], e)
+        e = window_energy(w)
+        assert abs(got_e[i] - e) <= ENERGY_TOL * e, (i, got_e[i], e)
     print(f"SF{sf}: window sums within {worst:.3f} of their tolerance")
     dec.close()
 

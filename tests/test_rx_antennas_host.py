@@ -52,12 +52,12 @@ def test_one_antenna_is_the_one_row_receiver(sf, osr):
 @pytest.mark.parametrize("osr", [8, 2])
 @pytest.mark.parametrize("sf", range(7, 13))
 def test_combined_screen_against_float64(sf, osr):
-    """Every bin clean (a spread at SF11/12), -3 dB, half-bin and noise windows on M = 2 and 4 antennas, each antenna its own
+    """Every bin clean (a spread at SF11/12), -3 dB, half-bin and noise windows on M = 2, 3 and 4 antennas (2 and 3 at SF11/12), each antenna its own
     symbols and gain: bin and magnitude inside the band of the float64 sum_a |tmp_a|^2; the criterion fails when any one
     antenna is left out of the reference's sum."""
     rng = np.random.default_rng(100 * sf + osr)
     sps = osr << sf
-    for m in ((2,) if sf >= 11 else (2, 4)):
+    for m in ((2, 3) if sf >= 11 else (2, 3, 4)):
         batches = [k1_batch(sf, osr, np.random.default_rng(1000 * sf + 10 * osr + a), n_clean=24 if sf >= 11 else None)
                    for a in range(m)]
         n = min(b.shape[0] for b in batches)
