@@ -31,7 +31,7 @@ class TxFrame(C.Structure):
 
 class RxParams(C.Structure):
     """struct lora_b200_rx_params (include/lora_b200.h)."""
-    _fields_ = [("sync_word", C.c_uint8), ("soft", C.c_uint8), ("crc_list", C.c_uint8), ("reserved0", C.c_uint8 * 1),
+    _fields_ = [("sync_word", C.c_uint8), ("soft", C.c_uint8), ("crc_list", C.c_uint8), ("wide_cfo", C.c_uint8),
                 ("implicit_len", C.c_uint32),
                 ("min_preamble", C.c_uint32),
                 ("max_cfo_hz", C.c_float), ("sfo_ppm", C.c_float), ("reserved1", C.c_uint32), ("carrier_hz", C.c_double)]

@@ -185,12 +185,17 @@ struct RsHostOps {
     long long n_items;
     const float2 *down, *up, *tw;
     uint32_t sps, sf, osr;
+    const float2 *shift;               // the shifted tables of hypotheses -hyp..hyp (rs_shift_tables)
+    int hyp;
     bool in_range(long long pos) const { return pos >= 0 && pos + (long long)sps <= n_items; }
     void binvals(long long pos, float F, bool use_up, int bin, float2 *v) { v[0] = binval(pos, F, use_up, bin); }
-    unsigned long long argmax(long long pos, bool use_up) {
+    const float2 *chirp(bool use_up, int c) const {
+        return c == 0 ? (use_up ? up : down) : shift + ((size_t)(c + hyp) * 2 + (use_up ? 1 : 0)) * sps;
+    }
+    unsigned long long argmax(long long pos, bool use_up, int c) {
         uint32_t b;
         float m;
-        lb_k1_emulate_osr((int)sf, (int)osr, x + pos, 1, use_up ? up : down, tw, &b, &m);
+        lb_k1_emulate_osr((int)sf, (int)osr, x + pos, 1, chirp(use_up, c), tw, &b, &m);
         return lb::pack_key(m * m, b);
     }
     float2 binval(long long pos, float F, bool use_up, int bin) {
@@ -218,10 +223,10 @@ struct RsHostAntOps {
     uint32_t m;
     bool in_range(long long pos) const { return one.in_range(pos); }
     RsHostOps row(uint32_t a) const { RsHostOps o = one; o.x = one.x + (size_t)a * one.n_items; return o; }
-    unsigned long long argmax(long long pos, bool use_up) {
+    unsigned long long argmax(long long pos, bool use_up, int c) {
         uint32_t b;
         float mg;
-        lb_k1_antennas_emulate_osr((int)one.sf, (int)one.osr, one.x + pos, (size_t)one.n_items, m, 1, use_up ? one.up : one.down, one.tw, &b, &mg);
+        lb_k1_antennas_emulate_osr((int)one.sf, (int)one.osr, one.x + pos, (size_t)one.n_items, m, 1, one.chirp(use_up, c), one.tw, &b, &mg);
         return lb::pack_key(mg * mg, b);
     }
     void binvals(long long pos, float F, bool use_up, int bin, float2 *v) {
@@ -314,35 +319,45 @@ int rs_host_crc_list(const lb::RxParams &rp, uint8_t phdr1, uint32_t implicit_le
 }
 
 // the receive path of lb_emul_rx_receive_osr (m = 1) and lb_emul_rx_receive_antennas (m rows of n_items each, x[a * n_items
-// ..]); with several antennas chan[f * m ..] gets each synchronised frame's channel estimates h (may be NULL)
+// ..]); with several antennas chan[f * m ..] gets each synchronised frame's channel estimates h (may be NULL).  max_cfo_bins
+// > 0: the coarse-offset search of rx_params.wide_cfo up to that CFO; else |CFO| <= N / 4 without it.
 uint32_t rs_host_receive(const float2 *x, size_t n_items, uint32_t m, const float2 *down, const float2 *up, const float2 *tw, uint32_t sf,
                          uint32_t osr, uint32_t cr, int implicit, int crc, int reduced_rate, uint32_t sync_word, uint32_t implicit_len,
                          uint32_t min_preamble, float sfo_ppm, double carrier_hz, int soft, long long *start, float *cfo_bins,
                          float *snr_db, int32_t *status, float *sfo, uint8_t *payload, uint32_t *len, float2 *chan, uint32_t cap,
-                         uint32_t crc_list = 0, uint8_t *crc_status = nullptr) {
+                         uint32_t crc_list = 0, uint8_t *crc_status = nullptr, float max_cfo_bins = 0.f) {
     if (osr != 8u && osr != 2u) return 0;
     const uint32_t N = 1u << sf, sps = osr * N;
     const double bin_hz = 125e3 / N;
     lb::RsParams p{sps, N, osr, sfo_ppm, min_preamble ? min_preamble : 5u, {((sync_word >> 4) & 15u) * 8u % N, (sync_word & 15u) * 8u % N},
-                   (float)N / 4.0f, carrier_hz > 0.0 ? (float)(1e6 * bin_hz / carrier_hz) : 0.0f};
-    RsHostOps o{x, (long long)n_items, down, up, tw, sps, sf, osr};
+                   max_cfo_bins > 0.f ? max_cfo_bins : (float)N / 4.0f, carrier_hz > 0.0 ? (float)(1e6 * bin_hz / carrier_hz) : 0.0f, 0};
+    p.hyp = lb::rs_hypotheses(p.max_cfo_bins, N);
+    if (p.hyp > lb::RS_MAX_HYP) return 0;
+    std::vector<float2> shift((size_t)(2 * p.hyp + 1) * 2 * sps);
+    lb::rs_shift_tables(down, up, sps, osr, p.hyp, shift.data());
+    RsHostOps o{x, (long long)n_items, down, up, tw, sps, sf, osr, shift.data(), p.hyp};
     RsHostAntOps oa{o, m};
-    // screen
-    std::vector<uint32_t> bins[2];
-    std::vector<float> mags[2];
+    // screen: both phases of every hypothesis, screen s = 2 (c + hyp) + ph (c = 0 with the plain down-chirp)
+    const int ns = 2 * (2 * p.hyp + 1);
+    std::vector<std::vector<uint32_t>> bins(ns);
+    std::vector<std::vector<float>> mags(ns);
+    std::vector<const uint32_t *> bp(ns);
+    std::vector<const float *> mp(ns);
     uint32_t n[2];
-    for (int ph = 0; ph < 2; ph++) {
-        n[ph] = n_items >= sps + ph * sps / 2 ? (uint32_t)((n_items - ph * sps / 2) / sps) : 0u;
-        bins[ph].resize(n[ph] + 1);
-        mags[ph].resize(n[ph] + 1);
-        if (n[ph] && m == 1) lb_k1_emulate_osr((int)sf, (int)osr, x + ph * sps / 2, n[ph], down, tw, bins[ph].data(), mags[ph].data());
-        else if (n[ph]) lb_k1_antennas_emulate_osr((int)sf, (int)osr, x + ph * sps / 2, n_items, m, n[ph], down, tw, bins[ph].data(), mags[ph].data());
+    for (int ph = 0; ph < 2; ph++) n[ph] = n_items >= sps + ph * sps / 2 ? (uint32_t)((n_items - ph * sps / 2) / sps) : 0u;
+    for (int s = 0; s < ns; s++) {
+        const int ph = s & 1;
+        const float2 *ch = o.chirp(false, s / 2 - p.hyp);
+        bins[s].resize(n[ph] + 1);
+        mags[s].resize(n[ph] + 1);
+        if (n[ph] && m == 1) lb_k1_emulate_osr((int)sf, (int)osr, x + ph * sps / 2, n[ph], ch, tw, bins[s].data(), mags[s].data());
+        else if (n[ph]) lb_k1_antennas_emulate_osr((int)sf, (int)osr, x + ph * sps / 2, n_items, m, n[ph], ch, tw, bins[s].data(), mags[s].data());
+        bp[s] = bins[s].data();
+        mp[s] = mags[s].data();
     }
-    const uint32_t *bp[2] = {bins[0].data(), bins[1].data()};
-    const float *mp[2] = {mags[0].data(), mags[1].data()};
     std::vector<lb::RsCand> cands(64);
     long long dropped;
-    const uint32_t nc = std::min<uint32_t>(lb::rs_detect_stream(bp, mp, n, p, cands.data(), 64, &dropped), 64u);
+    const uint32_t nc = std::min<uint32_t>(lb::rs_detect_stream<lb::RS_MAX_SCREENS>(bp.data(), mp.data(), n, p, cands.data(), 64, &dropped), 64u);
     lb::RxParams rp;
     memset(&rp, 0, sizeof rp);
     rp.sf = sf; rp.n_bins = N; rp.n_bins_hdr = N / 4; rp.sps = sps; rp.decim = osr; rp.implicit = implicit; rp.reduced_rate = reduced_rate;
@@ -473,6 +488,20 @@ int lb_emul_rx_crc_list(uint32_t sf, uint32_t cr, int implicit, int crc, int red
 // the payload CRC status (LORA_B200_CRC_NONE / _OK / _BAD) of a published record (lora_crc.h)
 uint32_t lb_emul_crc_record_status(const uint8_t *rec, uint32_t len) { return lb::lb_crc_record_status(rec, len); }
 uint32_t lb_emul_crc16(const uint8_t *b, uint32_t n) { return lb::lb_crc16(b, n); }
+
+// lb_emul_rx_receive_crc with the coarse-offset search of lora_b200_rx_params.wide_cfo: |CFO| up to max_cfo_bins bins (> 0,
+// at most (osr - 1) N / 2, the sampled band's limit; else 0 frames), as lora_b200_receive_antennas with wide_cfo = 1 and
+// max_cfo_hz = max_cfo_bins * BW / N
+uint32_t lb_emul_rx_receive_wide(const float2 *x, size_t n_items, uint32_t m, const float2 *down, const float2 *up, const float2 *tw,
+                                 uint32_t sf, uint32_t osr, uint32_t cr, int implicit, int crc, int reduced_rate, uint32_t sync_word,
+                                 uint32_t implicit_len, uint32_t min_preamble, float sfo_ppm, double carrier_hz, int soft, float max_cfo_bins,
+                                 long long *start, float *cfo_bins, float *snr_db, int32_t *status, float *sfo, uint8_t *payload,
+                                 uint32_t *len, uint32_t cap) {
+    if (m < 1 || m > (uint32_t)lb::RS_MAX_ANTENNAS || !(max_cfo_bins > 0.f) || max_cfo_bins > (float)((osr - 1u) << sf) / 2.0f) return 0;
+    return rs_host_receive(x, n_items, m, down, up, tw, sf, osr, cr, implicit, crc, reduced_rate, sync_word, implicit_len, min_preamble,
+                           sfo_ppm, carrier_hz, soft, start, cfo_bins, snr_db, status, sfo, payload, len, nullptr, cap, 0, nullptr,
+                           max_cfo_bins);
+}
 
 // lb_emul_rx_receive_osr at fs/bw = 8 (fs = 1 MHz)
 uint32_t lb_emul_rx_receive_soft(const float2 *x, size_t n_items, const float2 *down, const float2 *up, const float2 *tw, uint32_t sf,

@@ -149,6 +149,11 @@ struct lora_b200_decoder : A1Params {
     uint32_t rs_chan_m = 1;
     // lora_b200_frames_crc_last: the frames of the last call that list decoding recovered (empty: none), and the statuses
     std::vector<uint8_t> rs_recovered, crc_status;
+    // rx_params.wide_cfo: the shifted dechirp tables of hypotheses c = -rs_shift_hyp..rs_shift_hyp (rs_shift_tables), built
+    // once for the widest search asked so far
+    DeviceBuffer<float2> d_rs_shift;
+    std::vector<float2> h_rs_shift;
+    int rs_shift_hyp = 0;
 };
 
 namespace {
@@ -296,7 +301,8 @@ K1Launcher k1_launcher_generic(int sf, int osr) {
     return with_sf_osr(sf, osr, [] { return K1Launcher(); }, [](auto SF, auto D) -> K1Launcher { return k1_launch_generic<SF, D>; });
 }
 
-int dispatch_k1_impl(lora_b200_decoder *d, K1Scratch &ks, const float2 *iq, size_t n, uint32_t *bins, float *mags, cudaStream_t st) {
+int dispatch_k1_impl(lora_b200_decoder *d, K1Scratch &ks, const float2 *iq, size_t n, uint32_t *bins, float *mags, cudaStream_t st,
+                     const float2 *chirp) {
     if (int rc = need_k1(d, "FFT demodulator")) return rc;
     if (n == 0) return LORA_B200_OK;
     static const char *rows = getenv("LORA_B200_K1_ROWS");
@@ -312,7 +318,7 @@ int dispatch_k1_impl(lora_b200_decoder *d, K1Scratch &ks, const float2 *iq, size
         CU(cudaMemsetAsync(ks.packed, 0, sizeof(unsigned long long) * n, st));
     }
     char err[256] = {0};
-    const K1Launch k{K1Args{iq, tab<float2>(d, d->toff.down), tab<float2>(d, d->toff.tw), n},
+    const K1Launch k{K1Args{iq, chirp ? chirp : tab<float2>(d, d->toff.down), tab<float2>(d, d->toff.tw), n},
                      (const float2 *)(d->h_tables.data() + d->toff.tw), bins, mags, split ? ks.packed.get() : nullptr,
                      d->device, d->n_sms, st, err, sizeof err};
     if (launch(k)) return fail(LORA_B200_ECUDA, "K1: %s", err);
@@ -326,11 +332,12 @@ int dispatch_k1_impl(lora_b200_decoder *d, K1Scratch &ks, const float2 *iq, size
 
 // K1 on stream `st` with scratch `ks`: a launch that follows one on ANOTHER stream with the same scratch waits for it
 // (the memset of the keys / flags at the head of a launch must not run under the previous kernel; a wait on `done`
-// before its first record is a no-op)
-int dispatch_k1(lora_b200_decoder *d, K1Scratch &ks, const float2 *iq, size_t n, uint32_t *bins, float *mags, cudaStream_t st) {
+// before its first record is a no-op).  chirp: the dechirp table (NULL: the decoder's down-chirp).
+int dispatch_k1(lora_b200_decoder *d, K1Scratch &ks, const float2 *iq, size_t n, uint32_t *bins, float *mags, cudaStream_t st,
+                const float2 *chirp = nullptr) {
     CU(ks.done.ensure());
     if (ks.last != st) CU(cudaStreamWaitEvent(st, ks.done, 0));
-    const int rc = dispatch_k1_impl(d, ks, iq, n, bins, mags, st);
+    const int rc = dispatch_k1_impl(d, ks, iq, n, bins, mags, st, chirp);
     if (rc) return rc;
     CU(cudaEventRecord(ks.done, st));
     ks.last = st;
@@ -1074,49 +1081,50 @@ int lora_b200_tx_frames_sfo_dev(lora_b200_decoder *d, const void *up_table, cons
 // one receiver per stream (m = 1: rs_sync_kernel), or per group of m antenna rows (rs_sync_antennas_kernel)
 template <int SF, int D, bool DRIFT>
 static int rs_launch_sync(lora_b200_decoder *d, const float2 *x, size_t stride, size_t n_items, const RsParams &rp, uint32_t cap,
-                          uint32_t m) {
+                          uint32_t m, const float2 *shift) {
     const size_t smem = sizeof(float2) * K1Cfg<SF, D>::SMEM_ELEMS;
     const uint32_t ng = d->cfg.n_streams / m;
     if (m == 1) {
         CU(opt_in_smem((const void *)rs_sync_kernel<SF, D, DRIFT>, d->device, smem));
         rs_sync_kernel<SF, D, DRIFT><<<d->cfg.n_streams * cap, RX_THREADS, smem, d->rx_stream>>>(
-            x, stride, n_items, tab<float2>(d, d->toff.down), tab<float2>(d, d->toff.up), tab<float2>(d, d->toff.tw), rp, d->d_rs_cands,
-            d->d_rs_ncand, cap, d->d_rs_frames, d->d_rs_nframes, d->cfg.n_streams * cap, d->d_rs_hold);
+            x, stride, n_items, tab<float2>(d, d->toff.down), tab<float2>(d, d->toff.up), tab<float2>(d, d->toff.tw), shift, rp,
+            d->d_rs_cands, d->d_rs_ncand, cap, d->d_rs_frames, d->d_rs_nframes, d->cfg.n_streams * cap, d->d_rs_hold);
         return launched(d);
     }
     CU(opt_in_smem((const void *)rs_sync_antennas_kernel<SF, D, DRIFT>, d->device, smem));
     rs_sync_antennas_kernel<SF, D, DRIFT><<<ng * cap, RX_THREADS, smem, d->rx_stream>>>(
-        x, stride, n_items, m, tab<float2>(d, d->toff.down), tab<float2>(d, d->toff.up), tab<float2>(d, d->toff.tw), rp, d->d_rs_cands,
-        d->d_rs_ncand, cap, d->d_rs_frames, d->d_rs_nframes, ng * cap, d->d_rs_hold, d->d_rs_chan);
+        x, stride, n_items, m, tab<float2>(d, d->toff.down), tab<float2>(d, d->toff.up), tab<float2>(d, d->toff.tw), shift, rp,
+        d->d_rs_cands, d->d_rs_ncand, cap, d->d_rs_frames, d->d_rs_nframes, ng * cap, d->d_rs_hold, d->d_rs_chan);
     return launched(d);
 }
 
 // without a clock offset the synchroniser runs its DRIFT = false instantiation, which does no drift arithmetic; D = sps / N
-// (8 or 2) selects the K1 phase functions of its argmax windows
-static int rs_sync(lora_b200_decoder *d, const float2 *x, size_t stride, size_t n_items, const RsParams &rp, uint32_t cap, uint32_t m) {
+// (8 or 2) selects the K1 phase functions of its argmax windows; shift: the hypotheses' tables (NULL when rp.hyp = 0)
+static int rs_sync(lora_b200_decoder *d, const float2 *x, size_t stride, size_t n_items, const RsParams &rp, uint32_t cap, uint32_t m,
+                   const float2 *shift) {
     return with_sf_osr(d->cfg.sf, d->k1_osr, unsupported_sf(d), [&](auto SF, auto D) {
-        return with_bool(rs_drift(rp), [&](auto DRIFT) { return rs_launch_sync<SF, D, DRIFT>(d, x, stride, n_items, rp, cap, m); });
+        return with_bool(rs_drift(rp), [&](auto DRIFT) { return rs_launch_sync<SF, D, DRIFT>(d, x, stride, n_items, rp, cap, m, shift); });
     });
 }
 
 // the combined screen of ng receivers with m antennas: k1_antennas_kernel over the n_win windows of each row (rows `stride`
-// apart), receiver g's results at bins / mags[g * out_stride ..]
+// apart), receiver g's results at bins / mags[g * out_stride ..]; chirp: the dechirp table (NULL: the decoder's down-chirp)
 template <int SF, int D>
 static int rs_screen_launch(lora_b200_decoder *d, const float2 *x, size_t n_win, size_t stride, uint32_t m, uint32_t ng, size_t out_stride,
-                            uint32_t *bins, float *mags, cudaStream_t st) {
+                            uint32_t *bins, float *mags, cudaStream_t st, const float2 *chirp) {
     using C = K1Cfg<SF, D>;
     const size_t smem = sizeof(float2) * C::SMEM_ELEMS;
     CU(opt_in_smem((const void *)k1_antennas_kernel<SF, D>, d->device, smem));
     const size_t n_work = (n_win + C::G - 1) / C::G * ng;
     const int grid = (int)std::min<size_t>(n_work, (size_t)d->n_sms * 2);
-    k1_antennas_kernel<SF, D><<<grid, K1_THREADS, smem, st>>>(K1Args{x, tab<float2>(d, d->toff.down), tab<float2>(d, d->toff.tw), n_win},
+    k1_antennas_kernel<SF, D><<<grid, K1_THREADS, smem, st>>>(K1Args{x, chirp ? chirp : tab<float2>(d, d->toff.down), tab<float2>(d, d->toff.tw), n_win},
                                                              stride, m, ng, out_stride, bins, mags);
     return launched(d);
 }
 static int rs_screen(lora_b200_decoder *d, const float2 *x, size_t n_win, size_t stride, uint32_t m, uint32_t ng, size_t out_stride,
-                     uint32_t *bins, float *mags, cudaStream_t st) {
+                     uint32_t *bins, float *mags, cudaStream_t st, const float2 *chirp = nullptr) {
     return with_sf_osr(d->cfg.sf, d->k1_osr, unsupported_sf(d), [&](auto SF, auto D) {
-        return rs_screen_launch<SF, D>(d, x, n_win, stride, m, ng, out_stride, bins, mags, st);
+        return rs_screen_launch<SF, D>(d, x, n_win, stride, m, ng, out_stride, bins, mags, st, chirp);
     });
 }
 
@@ -1153,16 +1161,22 @@ static int rs_receive(lora_b200_decoder *d, const void *iq, size_t n_items, size
     if (P.soft > 1u) return fail(LORA_B200_EINVAL, "soft must be 0 or 1, got %u", (unsigned)P.soft);
     if (P.crc_list > RS_CRC_MAX_LIST || (P.crc_list && !P.soft))
         return fail(LORA_B200_EINVAL, "crc_list must be 0..%u and needs soft = 1, got %u", RS_CRC_MAX_LIST, (unsigned)P.crc_list);
+    if (P.wide_cfo > 1u) return fail(LORA_B200_EINVAL, "wide_cfo must be 0 or 1, got %u", (unsigned)P.wide_cfo);
+    const float band_max = (float)((d->samples_per_second - (double)d->cfg.bandwidth) / 2.0);    // (fs - BW) / 2
+    if (P.wide_cfo && !(std::isfinite(P.max_cfo_hz) && P.max_cfo_hz > 0.f && P.max_cfo_hz <= band_max))
+        return fail(LORA_B200_EINVAL, "wide_cfo needs max_cfo_hz in (0, %g], got %g", (double)band_max, (double)P.max_cfo_hz);
     CU(cudaSetDevice(d->device));
     // rows: ns; receivers (groups of m antenna rows): ng.  m = 1 is lora_b200_receive, launch for launch.
     const uint32_t rows = d->cfg.n_streams, ns = rows / m, sps = d->sps, N = d->n_bins, cap = d->cfg.max_frames_per_call;
     const bool soft = P.soft != 0;
     const uint8_t sw = P.sync_word ? P.sync_word : 0x12;
     const float fs = (float)d->samples_per_second, bin_hz = fs / (float)sps;
-    const float max_cfo = P.max_cfo_hz > 0.f && P.max_cfo_hz < d->cfg.bandwidth / 4.0f ? P.max_cfo_hz : d->cfg.bandwidth / 4.0f;
+    const float max_cfo = P.wide_cfo ? P.max_cfo_hz
+                          : P.max_cfo_hz > 0.f && P.max_cfo_hz < d->cfg.bandwidth / 4.0f ? P.max_cfo_hz : d->cfg.bandwidth / 4.0f;
     const float ppm_per_bin = P.carrier_hz > 0.0 ? (float)(1e6 * (double)bin_hz / P.carrier_hz) : 0.0f;
     RsParams rp{sps, N, d->decim, P.sfo_ppm, P.min_preamble ? P.min_preamble : 5u, {((sw >> 4) & 15u) * 8u % N, (sw & 15u) * 8u % N},
-                max_cfo / bin_hz, ppm_per_bin};
+                max_cfo / bin_hz, ppm_per_bin, 0};
+    rp.hyp = rs_hypotheses(rp.max_cfo_bins, N);
     // end of the window of data symbol n - 1 of a frame (its first n data symbols inside the row)
     auto data_end = [&](const RsFrame &r, long long n) { return rs_sym(r.start, rs_data_j(n - 1), sps, r.sfo_ppm) + (long long)sps; };
     d->rs_info.clear();
@@ -1193,24 +1207,46 @@ static int rs_receive(lora_b200_decoder *d, const void *iq, size_t n_items, size
                              host_ptr ? cudaMemcpyHostToDevice : cudaMemcpyDeviceToDevice, st));
         x = d->d_rs_stage;
     }
+    // wide_cfo: the shifted tables of hypotheses -hyp..hyp, at shift[((c + hyp) * 2 + up) * sps]
+    const float2 *shift = nullptr;
+    if (rp.hyp > 0) {
+        if (rp.hyp > d->rs_shift_hyp) {
+            const size_t n_tab = (size_t)(2 * rp.hyp + 1) * 2 * sps;
+            d->h_rs_shift.resize(n_tab);
+            rs_shift_tables((const float2 *)(d->h_tables.data() + d->toff.down), (const float2 *)(d->h_tables.data() + d->toff.up), sps,
+                            d->decim, rp.hyp, d->h_rs_shift.data());
+            CU(d->d_rs_shift.reserve(n_tab));
+            CU(cudaMemcpyAsync(d->d_rs_shift, d->h_rs_shift.data(), sizeof(float2) * n_tab, cudaMemcpyHostToDevice, st));
+            d->rs_shift_hyp = rp.hyp;
+        }
+        shift = d->d_rs_shift + (size_t)(d->rs_shift_hyp - rp.hyp) * 2 * sps;
+    }
+    // the screen of hypothesis h - hyp (h = 0 .. 2 hyp) at bins / mags[ph][h * hs ..]; hypothesis 0 dechirps with the
+    // decoder's own table
+    const size_t hs = (size_t)ns * (stride / sps) + 1, n_hyp = 2 * (size_t)rp.hyp + 1;
+    auto screen_chirp = [&](size_t h) { return (int)h == rp.hyp ? nullptr : shift + h * 2 * sps; };
+    for (int ph = 0; ph < 2; ph++) {
+        CU(d->d_rs_bins[ph].reserve(n_hyp * hs));
+        CU(d->d_rs_mags[ph].reserve(n_hyp * hs));
+    }
     if (m == 1) {
         const size_t span = (ns - 1) * stride + n_items, nw[2] = {span / sps, (span - sps / 2) / sps};
-        for (int ph = 0; ph < 2; ph++) {
-            CU(d->d_rs_bins[ph].reserve(nw[ph] + 1));
-            CU(d->d_rs_mags[ph].reserve(nw[ph] + 1));
-            if (int rc = dispatch_k1(d, d->k1s[0], x + ph * (sps / 2), nw[ph], d->d_rs_bins[ph], d->d_rs_mags[ph], st)) return rc;
-        }
+        for (size_t h = 0; h < n_hyp; h++)
+            for (int ph = 0; ph < 2; ph++)
+                if (int rc = dispatch_k1(d, d->k1s[0], x + ph * (sps / 2), nw[ph], d->d_rs_bins[ph] + h * hs, d->d_rs_mags[ph] + h * hs, st,
+                                         screen_chirp(h)))
+                    return rc;
     } else {
         // the combined screen: receiver g's window j of phase ph at bins[ph][g * stride / sps + j], as rs_detect_kernel reads
         // the screen of one row (only the windows it reads are computed)
         const size_t nw[2] = {n_items / sps, n_items >= sps + sps / 2 ? (n_items - sps / 2) / sps : 0};
-        for (int ph = 0; ph < 2; ph++) {
-            CU(d->d_rs_bins[ph].reserve((size_t)ns * (stride / sps) + 1));
-            CU(d->d_rs_mags[ph].reserve((size_t)ns * (stride / sps) + 1));
-            if (nw[ph] == 0) continue;
-            if (int rc = rs_screen(d, x + ph * (sps / 2), nw[ph], stride, m, ns, stride / sps, d->d_rs_bins[ph], d->d_rs_mags[ph], st))
-                return rc;
-        }
+        for (size_t h = 0; h < n_hyp; h++)
+            for (int ph = 0; ph < 2; ph++) {
+                if (nw[ph] == 0) continue;
+                if (int rc = rs_screen(d, x + ph * (sps / 2), nw[ph], stride, m, ns, stride / sps, d->d_rs_bins[ph] + h * hs,
+                                       d->d_rs_mags[ph] + h * hs, st, screen_chirp(h)))
+                    return rc;
+            }
         CU(d->d_rs_chan.reserve((size_t)ns * cap * 2 * RS_MAX_ANTENNAS));
     }
     // detect, synchronise
@@ -1223,10 +1259,15 @@ static int rs_receive(lora_b200_decoder *d, const void *iq, size_t n_items, size
     CU(d->d_rs_nframes.reserve(1));
     CU(cudaMemsetAsync(d->d_rs_hold, 0xFF, sizeof(unsigned long long) * ns, st));
     CU(cudaMemsetAsync(d->d_rs_nframes, 0, sizeof(uint32_t), st));
-    rs_detect_kernel<<<(ns + 127) / 128, 128, 0, st>>>(d->d_rs_bins[0], d->d_rs_mags[0], d->d_rs_bins[1], d->d_rs_mags[1], stride, n_items,
-                                                       ns, rp, d->d_rs_cands, cap, d->d_rs_ncand, d->d_rs_dropped);
+    if (rp.hyp == 0)
+        rs_detect_kernel<2><<<(ns + 127) / 128, 128, 0, st>>>(d->d_rs_bins[0], d->d_rs_mags[0], d->d_rs_bins[1], d->d_rs_mags[1], hs, stride,
+                                                              n_items, ns, rp, d->d_rs_cands, cap, d->d_rs_ncand, d->d_rs_dropped);
+    else
+        rs_detect_kernel<RS_MAX_SCREENS><<<(ns + 127) / 128, 128, 0, st>>>(d->d_rs_bins[0], d->d_rs_mags[0], d->d_rs_bins[1], d->d_rs_mags[1],
+                                                                           hs, stride, n_items, ns, rp, d->d_rs_cands, cap, d->d_rs_ncand,
+                                                                           d->d_rs_dropped);
     if (int rc = launched(d)) return rc;
-    if (int rc = rs_sync(d, x, stride, n_items, rp, cap, m)) return rc;
+    if (int rc = rs_sync(d, x, stride, n_items, rp, cap, m, shift)) return rc;
     uint32_t n_sync = 0;
     std::vector<long long> dropped(ns);
     std::vector<unsigned long long> shold(ns);
@@ -1420,7 +1461,8 @@ int lora_b200_demod_fft_antennas_dev(lora_b200_decoder *d, const void *iq, uint3
 }
 
 static_assert(sizeof(lora_b200_rx_info) == 32 && sizeof(lora_b200_rx_params) == 32 && offsetof(lora_b200_rx_params, soft) == 1 &&
-              offsetof(lora_b200_rx_params, crc_list) == 2 && offsetof(lora_b200_rx_params, implicit_len) == 4 &&
+              offsetof(lora_b200_rx_params, crc_list) == 2 && offsetof(lora_b200_rx_params, wide_cfo) == 3 &&
+              offsetof(lora_b200_rx_params, implicit_len) == 4 &&
               offsetof(lora_b200_rx_params, sfo_ppm) == 16 &&
               offsetof(lora_b200_rx_params, carrier_hz) == 24 && offsetof(lora_b200_rx_info, sfo_ppm) == 28, "lora_b200_rx_* layout");
 
@@ -1458,6 +1500,8 @@ int lora_b200_rs_window_dev(lora_b200_decoder *d, const void *iq, size_t n_items
     if (m > 1 && stride_items < n_items) return fail(LORA_B200_EINVAL, "stride_items %zu < n_items %zu", stride_items, n_items);
     if (n > 0x7FFFFFFFu) return fail(LORA_B200_EINVAL, "too many windows: %zu", n);
     const long long sps = d->sps, N = d->n_bins;
+    // the widest offset the synchroniser evaluates windows at: (fs - BW) / 2 = (D - 1) N / 2 bins (wide_cfo), at least N
+    const long long cfo_lim = std::max<long long>(N, ((long long)d->decim - 1) * N / 2);
     std::vector<RsWindowQuery> q(n);
     for (size_t i = 0; i < n; i++) {
         if (pos[i] < 0 || pos[i] + sps > (long long)n_items)
@@ -1465,8 +1509,8 @@ int lora_b200_rs_window_dev(lora_b200_decoder *d, const void *iq, size_t n_items
                         (long long)pos[i] + sps, n_items);
         if (up[i] != 0 && up[i] != 1) return fail(LORA_B200_EINVAL, "window %zu: up must be 0 or 1, got %d", i, up[i]);
         if (bin[i] < -N / 2 || bin[i] >= N / 2) return fail(LORA_B200_EINVAL, "window %zu: bin %d outside -N/2..N/2-1", i, bin[i]);
-        if (!std::isfinite(cfo_bins[i]) || std::fabs(cfo_bins[i]) > (float)N)
-            return fail(LORA_B200_EINVAL, "window %zu: cfo_bins %g is not finite within +-N", i, (double)cfo_bins[i]);
+        if (!std::isfinite(cfo_bins[i]) || std::fabs(cfo_bins[i]) > (float)cfo_lim)
+            return fail(LORA_B200_EINVAL, "window %zu: cfo_bins %g is not finite within +-%lld", i, (double)cfo_bins[i], cfo_lim);
         q[i] = RsWindowQuery{(long long)pos[i], cfo_bins[i], up[i], bin[i], 0};
     }
     CU(cudaSetDevice(d->device));

@@ -16,6 +16,10 @@
 // A window at p dechirped with the down-chirp sees an up-chirp that started tau samples before p at bin tau / decim + F, and
 // dechirped with the up-chirp sees a down-chirp at bin -tau / decim + F (F = CFO in bins, modulo N): the preamble bin A and
 // the SFD bin B give 2F = A + B and 2 tau / decim = A - B, the N/2 ambiguity resolved by |F| <= N/4.
+// Wider offsets (rx_params.wide_cfo) search hypotheses c = -C..C of a coarse offset c N/2 bins: the screen runs once per
+// hypothesis with the shifted tables down_c[n] = down[n] e^{-j pi c n / D} (rs_shift_tables), whose windows see the preamble at
+// tau / decim + F - c N/2, and the synchroniser resolves the ambiguity F = c N/2 + smod(A + B, N) / 2 + k N/2 by scoring the
+// branches k = -1, 0, 1 (rs_synchronise).  C = 0 (|F| <= N/4) is the procedure above.
 // Everything a kernel decides is in the __host__ __device__ functions below, which host_emul.cu runs on the CPU.
 #pragma once
 #include "int_chain.cuh"
@@ -25,6 +29,8 @@
 #include "rx_stream.cuh"
 #include "tx_encode.cuh"
 
+#include <cmath>
+
 namespace lb {
 
 struct RsParams {
@@ -32,16 +38,40 @@ struct RsParams {
     float sfo_ppm;                     // clock offset of every frame, in ppm (0: none)
     uint32_t min_preamble;             // windows of one phase
     uint32_t sw[2];                    // sync-word bins, ((sw >> 4) & 15) * 8 and (sw & 15) * 8 (tx.modulate_frame)
-    float max_cfo_bins;                // |CFO| accepted, in bins (<= N / 4)
+    float max_cfo_bins;                // |CFO| accepted, in bins (<= N / 4 unless wide_cfo)
     float ppm_per_bin;                 // clock offset per bin of CFO: 1e6 * bin_hz / carrier_hz (0: no carrier given)
+    int32_t hyp;                       // C: coarse-offset hypotheses c = -C..C (rs_hypotheses; 0: the one screen of c = 0)
 };
+
+// coarse-offset hypotheses: the largest |c| the screen needs so that every |F| <= max_cfo_bins lies within N/4 of some c N/2
+constexpr int RS_MAX_HYP = 7;          // (fs - BW) / 2 at fs / bw = 8: 3.5 N bins
+constexpr int RS_MAX_SCREENS = 2 * (2 * RS_MAX_HYP + 1);
+inline int rs_hypotheses(float max_cfo_bins, uint32_t N) {
+    const double c = std::ceil(((double)max_cfo_bins - 0.25 * N) / (0.5 * N));
+    return c > 0.0 ? (int)c : 0;
+}
+
+// the shifted dechirp tables of hypotheses c = -C..C, out[((c + C) * 2 + up) * sps + n] = table[n] e^{-j pi c n / D}, table the
+// down- (up = 0) or up-chirp (up = 1); the phase is reduced exactly, (c n) mod 2D, and the product is formed in double
+inline void rs_shift_tables(const float2 *down, const float2 *up, uint32_t sps, uint32_t D, int C, float2 *out) {
+    for (int c = -C; c <= C; c++)
+        for (int u = 0; u < 2; u++) {
+            const float2 *t = u ? up : down;
+            float2 *o = out + ((size_t)(c + C) * 2 + u) * sps;
+            for (uint32_t n = 0; n < sps; n++) {
+                const long long r = (((long long)c * n) % (2 * (long long)D) + 2 * (long long)D) % (2 * (long long)D);
+                const double a = -M_PI * (double)r / (double)D, cs = std::cos(a), sn = std::sin(a);
+                o[n] = make_float2((float)(t[n].x * cs - t[n].y * sn), (float)(t[n].x * sn + t[n].y * cs));
+            }
+        }
+}
 
 struct RsCand {                        // one preamble run of the screen
     long long p_last;                  // first sample of the run's last window
     uint32_t bin;                      // its bin
     uint32_t run;                      // windows in the run
     float mag;                         // mean peak magnitude of the run
-    uint32_t pad;
+    int32_t hyp;                       // the coarse-offset hypothesis c of its screen
 };
 
 enum RsStatus { RS_OK = 0, RS_INCOMPLETE = 1, RS_REJECT = 2 };
@@ -89,15 +119,19 @@ LB_HD int rs_smod(int v, int n) {      // v mod n in [-n/2, n/2)
 }
 
 // ---- detect: one stream's screen -> candidates --------------------------------------------------------------------------
-// bins/mags[ph] hold the windows of phase ph, window j at j * sps + ph * sps / 2, n[ph] of them.  Windows are visited in
-// order of position; a run of one phase grows while consecutive bins agree within +-1.  Runs of both phases that end within
-// two symbols of each other describe the same preamble: the one with the larger mean peak (the better aligned) is kept.
+// The screens are s = 0 .. 2 (2 C + 1) - 1 (C = p.hyp): phase ph = s % 2 of hypothesis c = s / 2 - C.  bins/mags[s] hold the
+// windows of screen s, window j at j * sps + ph * sps / 2, n[ph] of them.  Windows are visited in order of position; a run of
+// one screen grows while consecutive bins agree within +-1.  Runs of any screens that end within two symbols of each other
+// describe the same preamble: the one with the larger mean peak (the better aligned, in the better hypothesis) is kept.
 // Writes at most cap candidates, returns how many there were (more than cap: the caller holds back from the first extra).
-LB_HD uint32_t rs_detect_stream(const uint32_t *const bins[2], const float *const mags[2], const uint32_t n[2], const RsParams &p,
+// S_MAX bounds the screens (2: the one hypothesis c = 0).
+template <int S_MAX>
+LB_HD uint32_t rs_detect_stream(const uint32_t *const *bins, const float *const *mags, const uint32_t n[2], const RsParams &p,
                                 RsCand *out, uint32_t cap, long long *first_dropped) {
-    const int N = (int)p.n_bins;
-    uint32_t run[2] = {0, 0}, last[2] = {0, 0};
-    float msum[2] = {0.f, 0.f};
+    const int N = (int)p.n_bins, ns = 2 * (2 * p.hyp + 1) < S_MAX ? 2 * (2 * p.hyp + 1) : S_MAX;
+    uint32_t run[S_MAX], last[S_MAX];
+    float msum[S_MAX];
+    for (int s = 0; s < S_MAX; s++) { run[s] = 0; last[s] = 0; msum[s] = 0.f; }
     RsCand pend = {0, 0, 0, 0.f, 0};
     bool have = false;
     uint32_t cnt = 0;
@@ -107,11 +141,11 @@ LB_HD uint32_t rs_detect_stream(const uint32_t *const bins[2], const float *cons
         else if (cnt == cap) *first_dropped = c.p_last - (long long)c.run * p.sps;
         cnt++;
     };
-    auto close = [&](int ph, uint32_t j_end) {     // run of phase ph whose last window is j_end - 1
-        if (run[ph] >= p.min_preamble) {
+    auto close = [&](int s, uint32_t j_end) {      // run of screen s whose last window is j_end - 1
+        if (run[s] >= p.min_preamble) {
             RsCand c;
-            c.p_last = (long long)(j_end - 1) * p.sps + ph * (p.sps / 2);
-            c.bin = last[ph]; c.run = run[ph]; c.mag = msum[ph] / (float)run[ph]; c.pad = 0;
+            c.p_last = (long long)(j_end - 1) * p.sps + (s & 1) * (p.sps / 2);
+            c.bin = last[s]; c.run = run[s]; c.mag = msum[s] / (float)run[s]; c.hyp = s / 2 - p.hyp;
             if (have && c.p_last - pend.p_last < 2ll * p.sps && pend.p_last - c.p_last < 2ll * p.sps) {
                 if (c.mag > pend.mag) pend = c;
             } else {
@@ -120,21 +154,23 @@ LB_HD uint32_t rs_detect_stream(const uint32_t *const bins[2], const float *cons
                 have = true;
             }
         }
-        run[ph] = 0; msum[ph] = 0.f;
+        run[s] = 0; msum[s] = 0.f;
     };
     const uint32_t jmax = n[0] > n[1] ? n[0] : n[1];
     for (uint32_t j = 0; j < jmax; j++) {
-        for (int ph = 0; ph < 2; ph++) {
-            if (j >= n[ph]) continue;
-            const uint32_t b = bins[ph][j];
-            if (run[ph] && (rs_smod((int)b - (int)last[ph], N) < -1 || rs_smod((int)b - (int)last[ph], N) > 1)) close(ph, j);
-            run[ph]++;
-            msum[ph] += mags[ph][j];
-            last[ph] = b;
+#pragma unroll
+        for (int s = 0; s < S_MAX; s++) {
+            if (s >= ns || j >= n[s & 1]) continue;
+            const uint32_t b = bins[s][j];
+            if (run[s] && (rs_smod((int)b - (int)last[s], N) < -1 || rs_smod((int)b - (int)last[s], N) > 1)) close(s, j);
+            run[s]++;
+            msum[s] += mags[s][j];
+            last[s] = b;
         }
     }
-    close(0, n[0]);
-    close(1, n[1]);
+#pragma unroll
+    for (int s = 0; s < S_MAX; s++)
+        if (s < ns) close(s, n[s & 1]);
     if (have) emit(pend);
     return cnt;
 }
@@ -144,7 +180,8 @@ LB_HD uint32_t rs_detect_stream(const uint32_t *const bins[2], const float *cons
 // several antennas (rows) sharing one timing and CFO; Ops::M is how many values binvals writes (1 for one row; with
 // fewer antennas than M the rest are 0):
 //   bool in_range(long long pos)                       window [pos, pos + sps) inside the row
-//   unsigned long long argmax(long long pos, bool up)  K1 argmax key of the raw window, dechirped with the down (up) chirp;
+//   unsigned long long argmax(long long pos, bool up, int c)  K1 argmax key of the raw window, dechirped with the down (up)
+//                                                      chirp of hypothesis c (rs_shift_tables; c = 0: the plain tables);
 //                                                      over several antennas the key of the summed |tmp_a|^2
 //   void binvals(long long pos, float F, bool up, int bin, float2 *v)   v[a]: bin `bin` (signed, -N/2..N/2) of antenna a's
 //                                                      window de-rotated by F bins
@@ -179,6 +216,10 @@ LB_HD float rs_score(Ops &ops, const RsParams &p, long long t, int m, float F) {
 #ifdef __CUDACC__
 #pragma nv_exec_check_disable
 #endif
+// The candidate's hypothesis c: its windows saw the preamble at A = tau / decim + F - c N/2 and the SFD, dechirped with up_c, at
+// B = -tau / decim + F - c N/2 (mod N), so F = c N/2 + smod(A + B, N) / 2 + k N/2.  Each branch k (k = 0 only while
+// max_cfo_bins <= N/4, where |F| <= N/4 decides it) gets its own timing, which moves by sps/2 per k, and its own fractional
+// CFO, and all branches' hypotheses compete in one score.
 template <bool DRIFT, class Ops>
 LB_HD RsFrame rs_synchronise(Ops &ops, const RsCand &c, const RsParams &p, uint32_t stream) {
     const long long sps = p.sps;
@@ -187,48 +228,57 @@ LB_HD RsFrame rs_synchronise(Ops &ops, const RsCand &c, const RsParams &p, uint3
     RsFrame r;
     r.start = c.p_last - (long long)c.run * sps; r.stream = stream; r.cfo_bins = 0.f; r.snr_db = 0.f;
     r.status = RS_REJECT; r.n_payload = 0; r.sfo_ppm = 0.f;
-    // SFD: the window 2..6 symbols after the run's last one with the strongest up-chirp dechirp
+    // SFD: the window 2..6 symbols after the run's last one with the strongest up-chirp dechirp.  A preamble tone often
+    // shows as strongly in two neighbouring hypotheses while the SFD's tone lies outside one of their bands, so the SFD is
+    // taken over hypotheses c - 1 .. c + 1 (those searched), and its bin moved into c's: B_c = B_c' + (c' - c) N/2
     unsigned long long best = 0ull;
-    int kbest = -1;
+    int kbest = -1, cbest = c.hyp;
+    const int c0 = c.hyp > -p.hyp ? c.hyp - 1 : c.hyp, c1 = c.hyp < p.hyp ? c.hyp + 1 : c.hyp;
     for (int k = 2; k <= 6; k++) {
         const long long pos = c.p_last + k * sps;
         if (!ops.in_range(pos)) { r.status = RS_INCOMPLETE; return r; }
-        const unsigned long long key = ops.argmax(pos, true);
-        if (key > best) { best = key; kbest = k; }
-    }
-    const int A = (int)c.bin, B = (int)key_idx(best);
-    const float Fc = 0.5f * (float)rs_smod(A + B, N);
-    if (fabsf(Fc) > p.max_cfo_bins + 1.0f) return r;
-    float tau = fmodf((float)A - Fc, (float)N);
-    if (tau < 0.f) tau += (float)N;
-    // frame start if the SFD window (kbest symbols after the run's last window) lies in the first down-chirp, TX symbol
-    // position 10: the run's last window, whose bin gave tau, then lies in preamble symbol 10 - kbest
-    const float rc = rs_ppm_of<DRIFT>(p, Fc);
-    const long long t0 = DRIFT ? c.p_last - (long long)lrintf(tau * decim) - rs_pos<DRIFT>(0, 10 - kbest, p.sps, rc)
-                               : c.p_last + kbest * sps - (long long)lrintf(tau * decim) - 10 * sps;
-    // fractional CFO: phase advance of the preamble peak from symbol to symbol (its residual modulo one bin)
-    float2 z = make_float2(0.f, 0.f), prev[Ops::M];
-    for (int a = 0; a < Ops::M; a++) prev[a] = make_float2(0.f, 0.f);
-    for (int i = 1; i <= 6; i++) {
-        const long long pos = rs_pos<DRIFT>(t0, i, p.sps, rc);
-        if (pos < 0 || !ops.in_range(pos)) continue;
-        float2 x[Ops::M];
-        ops.binvals(pos, Fc, false, 0, x);
-        for (int a = 0; a < Ops::M; a++) {
-            if (i > 1) z = cadd(z, cmul(x[a], cconj(prev[a])));
-            prev[a] = x[a];
+        for (int h = c0; h <= c1; h++) {
+            const unsigned long long key = ops.argmax(pos, true, h);
+            if (key > best) { best = key; kbest = k; cbest = h; }
         }
     }
-    const float eps = rs_phase_rev(z);
+    const int A = (int)c.bin, B = (int)key_idx(best) + (cbest - c.hyp) * (N / 2);
+    const float Fh = (float)c.hyp * (float)(N / 2);
+    const int kmax = p.max_cfo_bins > 0.25f * (float)N ? 1 : 0;
     float best_s = -1.f, Fb = 0.f;
     long long tb = 0;
-    for (int j = -1; j <= 1; j++) {
-        const float F = Fc + eps + (float)j;
-        if (fabsf(F) > p.max_cfo_bins + 0.5f) continue;
-        const long long tj = t0 + (long long)lrintf((F - Fc) * decim);   // timing follows the CFO: tau = (A - F) decim
-        for (int m = -1; m <= 1; m++) {
-            const float s = DRIFT ? rs_score<DRIFT>(ops, p, tj, m, F) : rs_score<DRIFT>(ops, p, tj + m * sps, 0, F);
-            if (s > best_s) { best_s = s; Fb = F; tb = rs_pos<DRIFT>(tj, m, p.sps, rs_ppm_of<DRIFT>(p, F)); }
+    for (int kb = -kmax; kb <= kmax; kb++) {
+        const float Fr = 0.5f * (float)rs_smod(A + B, N) + (float)(kb * (N / 2)), Fc = Fh + Fr;
+        if (fabsf(Fc) > p.max_cfo_bins + 1.0f) continue;
+        float tau = fmodf((float)A - Fr, (float)N);
+        if (tau < 0.f) tau += (float)N;
+        // frame start if the SFD window (kbest symbols after the run's last window) lies in the first down-chirp, TX symbol
+        // position 10: the run's last window, whose bin gave tau, then lies in preamble symbol 10 - kbest
+        const float rc = rs_ppm_of<DRIFT>(p, Fc);
+        const long long t0 = DRIFT ? c.p_last - (long long)lrintf(tau * decim) - rs_pos<DRIFT>(0, 10 - kbest, p.sps, rc)
+                                   : c.p_last + kbest * sps - (long long)lrintf(tau * decim) - 10 * sps;
+        // fractional CFO: phase advance of the preamble peak from symbol to symbol (its residual modulo one bin)
+        float2 z = make_float2(0.f, 0.f), prev[Ops::M];
+        for (int a = 0; a < Ops::M; a++) prev[a] = make_float2(0.f, 0.f);
+        for (int i = 1; i <= 6; i++) {
+            const long long pos = rs_pos<DRIFT>(t0, i, p.sps, rc);
+            if (pos < 0 || !ops.in_range(pos)) continue;
+            float2 x[Ops::M];
+            ops.binvals(pos, Fc, false, 0, x);
+            for (int a = 0; a < Ops::M; a++) {
+                if (i > 1) z = cadd(z, cmul(x[a], cconj(prev[a])));
+                prev[a] = x[a];
+            }
+        }
+        const float eps = rs_phase_rev(z);
+        for (int j = -1; j <= 1; j++) {
+            const float F = Fc + eps + (float)j;
+            if (fabsf(F) > p.max_cfo_bins + 0.5f) continue;
+            const long long tj = t0 + (long long)lrintf((F - Fc) * decim);   // timing follows the CFO: tau = (A - F) decim
+            for (int m = -1; m <= 1; m++) {
+                const float s = DRIFT ? rs_score<DRIFT>(ops, p, tj, m, F) : rs_score<DRIFT>(ops, p, tj + m * sps, 0, F);
+                if (s > best_s) { best_s = s; Fb = F; tb = rs_pos<DRIFT>(tj, m, p.sps, rs_ppm_of<DRIFT>(p, F)); }
+            }
         }
     }
     if (best_s < 0.f) return r;
@@ -240,7 +290,7 @@ LB_HD RsFrame rs_synchronise(Ops &ops, const RsCand &c, const RsParams &p, uint3
         if (s > best_s) { best_s = s; tf = tb + d; }
     }
     // the residual CFO at the final timing
-    z = make_float2(0.f, 0.f);
+    float2 z = make_float2(0.f, 0.f), prev[Ops::M];
     float pk = 0.f, en = 0.f;
     int npk = 0;
     const float rb = rs_ppm_of<DRIFT>(p, Fb);
@@ -260,14 +310,17 @@ LB_HD RsFrame rs_synchronise(Ops &ops, const RsCand &c, const RsParams &p, uint3
         npk++;
     }
     const float F = Fb + rs_phase_rev(z);
-    // sync word: the argmax of both sync symbols (raw windows, so shifted by the CFO) within one bin of the expected one
+    // sync word: the argmax of both sync symbols (raw windows, so shifted by the CFO) within one bin of the expected one,
+    // dechirped with the hypothesis c' whose c' N/2 lies nearest F
     const int Fi = (int)lrintf(F);
+    int cs = (int)lrintf(F / (float)(N / 2));
+    cs = cs < -p.hyp ? -p.hyp : cs > p.hyp ? p.hyp : cs;
     const float rf = rs_ppm_of<DRIFT>(p, F);
     for (int i = 0; i < 2; i++) {
         const long long pos = rs_pos<DRIFT>(tf, 8 + i, p.sps, rf);
         if (pos < 0 || !ops.in_range(pos)) return r;
-        const int b = (int)key_idx(ops.argmax(pos, false));
-        const int dv = rs_smod(b - Fi - (int)p.sw[i], N);
+        const int b = (int)key_idx(ops.argmax(pos, false, cs));
+        const int dv = rs_smod(b - (Fi - cs * (N / 2)) - (int)p.sw[i], N);
         if (dv < -1 || dv > 1) return r;
     }
     if (fabsf(F) > p.max_cfo_bins) return r;
@@ -556,18 +609,26 @@ LB_HD uint32_t rs_crc_block_bin(const RsCrcFrame &f, const uint8_t *nib, uint32_
 #ifdef __CUDACC__
 // ---- kernels ---------------------------------------------------------------------------------------------------------------
 // detect: one thread per stream.  The screen's windows of row s are the K1 results starting at s * stride / sps (stride a
-// multiple of sps) in each phase array.
+// multiple of sps) in each phase array, those of hypothesis c at (c + hyp) * hyp_stride further.  S_MAX bounds the screens
+// (2 without wide_cfo, RS_MAX_SCREENS with it).
+template <int S_MAX>
 __global__ void rs_detect_kernel(const uint32_t *__restrict__ bins0, const float *__restrict__ mags0, const uint32_t *__restrict__ bins1,
-                                 const float *__restrict__ mags1, size_t stride, size_t n_items, uint32_t n_streams, RsParams p,
-                                 RsCand *__restrict__ cands, uint32_t cap, uint32_t *__restrict__ n_cands,
+                                 const float *__restrict__ mags1, size_t hyp_stride, size_t stride, size_t n_items, uint32_t n_streams,
+                                 RsParams p, RsCand *__restrict__ cands, uint32_t cap, uint32_t *__restrict__ n_cands,
                                  long long *__restrict__ dropped) {
     const uint32_t s = blockIdx.x * blockDim.x + threadIdx.x;
     if (s >= n_streams) return;
     const size_t base = s * (stride / p.sps);
-    const uint32_t *b[2] = {bins0 + base, bins1 + base};
-    const float *m[2] = {mags0 + base, mags1 + base};
+    const uint32_t *b[S_MAX];
+    const float *m[S_MAX];
+#pragma unroll
+    for (int k = 0; k < S_MAX; k++) {
+        const size_t o = base + (size_t)(k >> 1) * hyp_stride;
+        b[k] = (k & 1 ? bins1 : bins0) + o;
+        m[k] = (k & 1 ? mags1 : mags0) + o;
+    }
     const uint32_t n[2] = {(uint32_t)(n_items / p.sps), (uint32_t)(n_items >= p.sps + p.sps / 2 ? (n_items - p.sps / 2) / p.sps : 0)};
-    n_cands[s] = rs_detect_stream(b, m, n, p, cands + (size_t)s * cap, cap, dropped + s);
+    n_cands[s] = rs_detect_stream<S_MAX>(b, m, n, p, cands + (size_t)s * cap, cap, dropped + s);
 }
 
 // the windows of one candidate, block-collective (all threads call every member with the same arguments); D = sps / N is
@@ -581,11 +642,16 @@ struct RsDevOps {
     uint32_t sps;
     float2 *smem;
     RxShared *sh;
+    const float2 *shift;               // the shifted tables of hypotheses -hyp..hyp (rs_shift_tables; NULL when hyp = 0)
+    int hyp;
     LB_D bool in_range(long long pos) const { return pos >= 0 && pos + (long long)sps <= n_items; }
-    LB_D unsigned long long argmax(long long pos, bool use_up) {
+    LB_D const float2 *chirp(bool use_up, int c) const {
+        return c == 0 ? (use_up ? up : down) : shift + ((size_t)(c + hyp) * 2 + (use_up ? 1 : 0)) * sps;
+    }
+    LB_D unsigned long long argmax(long long pos, bool use_up, int c) {
         using C = K1Cfg<SF, D>;
         const int tid = threadIdx.x;
-        K1Args a{x + pos, use_up ? up : down, tw, 1};
+        K1Args a{x + pos, chirp(use_up, c), tw, 1};
         unsigned long long best = 0ull;
         float2 wtab[C::NP / C::TPS];
         k1_combine_twiddles<SF, D>(a, tid, wtab);
@@ -639,10 +705,10 @@ struct RsAntOps {
     uint32_t m;
     LB_D bool in_range(long long pos) const { return one.in_range(pos); }
     static_assert(M == 4, "binvals reduces 2 M sums as two block_sum<4>");
-    LB_D unsigned long long argmax(long long pos, bool use_up) {
+    LB_D unsigned long long argmax(long long pos, bool use_up, int c) {
         using C = K1Cfg<SF, D>;
         const int tid = threadIdx.x;
-        K1Args a{one.x + pos, use_up ? one.up : one.down, one.tw, 1};
+        K1Args a{one.x + pos, one.chirp(use_up, c), one.tw, 1};
         unsigned long long best = 0ull;
         float2 wtab[C::NP / C::TPS];
         k1_combine_twiddles<SF, D>(a, tid, wtab);
@@ -726,7 +792,7 @@ struct RsAntOps {
 template <int SF, int D, bool DRIFT>
 __global__ void __launch_bounds__(RX_THREADS)
 rs_sync_kernel(const float2 *__restrict__ iq, size_t stride, size_t n_items, const float2 *down, const float2 *up, const float2 *tw,
-               RsParams p, const RsCand *__restrict__ cands, const uint32_t *__restrict__ n_cands, uint32_t cap,
+               const float2 *shift, RsParams p, const RsCand *__restrict__ cands, const uint32_t *__restrict__ n_cands, uint32_t cap,
                RsFrame *__restrict__ frames, uint32_t *__restrict__ n_frames, uint32_t frame_cap,
                unsigned long long *__restrict__ hold) {
     extern __shared__ float2 rs_dyn_smem[];
@@ -734,7 +800,7 @@ rs_sync_kernel(const float2 *__restrict__ iq, size_t stride, size_t n_items, con
     const uint32_t s = blockIdx.x / cap, i = blockIdx.x % cap;
     const uint32_t nc = n_cands[s];
     if (i >= (nc < cap ? nc : cap)) return;
-    RsDevOps<SF, D> ops{iq + (size_t)s * stride, (long long)n_items, down, up, tw, p.sps, rs_dyn_smem, &sh};
+    RsDevOps<SF, D> ops{iq + (size_t)s * stride, (long long)n_items, down, up, tw, p.sps, rs_dyn_smem, &sh, shift, p.hyp};
     const RsFrame r = rs_synchronise<DRIFT>(ops, cands[(size_t)s * cap + i], p, s);
     if (threadIdx.x == 0) {
         if (r.status == RS_INCOMPLETE) atomicMin(hold + s, (unsigned long long)(r.start > 0 ? r.start : 0));
@@ -751,7 +817,7 @@ rs_sync_kernel(const float2 *__restrict__ iq, size_t stride, size_t n_items, con
 template <int SF, int D, bool DRIFT>
 __global__ void __launch_bounds__(RX_THREADS)
 rs_sync_antennas_kernel(const float2 *__restrict__ iq, size_t stride, size_t n_items, uint32_t m, const float2 *down, const float2 *up,
-                        const float2 *tw, RsParams p, const RsCand *__restrict__ cands, const uint32_t *__restrict__ n_cands, uint32_t cap,
+                        const float2 *tw, const float2 *shift, RsParams p, const RsCand *__restrict__ cands, const uint32_t *__restrict__ n_cands, uint32_t cap,
                         RsFrame *__restrict__ frames, uint32_t *__restrict__ n_frames, uint32_t frame_cap,
                         unsigned long long *__restrict__ hold, float2 *__restrict__ chan) {
     extern __shared__ float2 rs_dyn_smem[];
@@ -759,7 +825,7 @@ rs_sync_antennas_kernel(const float2 *__restrict__ iq, size_t stride, size_t n_i
     const uint32_t s = blockIdx.x / cap, i = blockIdx.x % cap;
     const uint32_t nc = n_cands[s];
     if (i >= (nc < cap ? nc : cap)) return;
-    RsAntOps<SF, D> ops{{iq + (size_t)s * m * stride, (long long)n_items, down, up, tw, p.sps, rs_dyn_smem, &sh}, stride, m};
+    RsAntOps<SF, D> ops{{iq + (size_t)s * m * stride, (long long)n_items, down, up, tw, p.sps, rs_dyn_smem, &sh, shift, p.hyp}, stride, m};
     RsFrame r = rs_synchronise<DRIFT>(ops, cands[(size_t)s * cap + i], p, s);
     float2 h[RS_MAX_ANTENNAS], w[RS_MAX_ANTENNAS];
     if (r.status == RS_OK) r.snr_db = rs_channels<DRIFT>(ops, p, r, m, h, w);
@@ -800,15 +866,15 @@ rs_window_kernel(const float2 *__restrict__ x, size_t stride, long long n_items,
     float e[RS_MAX_ANTENNAS];
     unsigned long long k;
     if (m == 1) {
-        RsDevOps<SF, D> ops{x, n_items, down, up, tw, sps, rs_dyn_smem, &sh};
+        RsDevOps<SF, D> ops{x, n_items, down, up, tw, sps, rs_dyn_smem, &sh, nullptr, 0};
         ops.binvals(w.pos, w.cfo_bins, w.up != 0, w.bin, v);
         e[0] = ops.energy(w.pos);
-        k = ops.argmax(w.pos, w.up != 0);
+        k = ops.argmax(w.pos, w.up != 0, 0);
     } else {
-        RsAntOps<SF, D> ops{{x, n_items, down, up, tw, sps, rs_dyn_smem, &sh}, stride, m};
+        RsAntOps<SF, D> ops{{x, n_items, down, up, tw, sps, rs_dyn_smem, &sh, nullptr, 0}, stride, m};
         ops.binvals(w.pos, w.cfo_bins, w.up != 0, w.bin, v);
         ops.energies(w.pos, e);
-        k = ops.argmax(w.pos, w.up != 0);
+        k = ops.argmax(w.pos, w.up != 0, 0);
     }
     if (threadIdx.x == 0) {
         for (uint32_t a = 0; a < m; a++) {
@@ -828,7 +894,7 @@ rs_channels_kernel(const float2 *__restrict__ iq, size_t stride, size_t n_items,
                    const float2 *tw, RsParams p, const RsFrame *__restrict__ frames, float2 *__restrict__ chan, float *__restrict__ snr_db) {
     __shared__ RxShared sh;
     const RsFrame r = frames[blockIdx.x];
-    RsAntOps<SF, D> ops{{iq + (size_t)r.stream * m * stride, (long long)n_items, down, up, tw, p.sps, nullptr, &sh}, stride, m};
+    RsAntOps<SF, D> ops{{iq + (size_t)r.stream * m * stride, (long long)n_items, down, up, tw, p.sps, nullptr, &sh, nullptr, 0}, stride, m};
     float2 h[RS_MAX_ANTENNAS], w[RS_MAX_ANTENNAS];   // (rs_channels takes no argmax: no dynamic shared memory)
     const float s = rs_channels<DRIFT>(ops, p, r, m, h, w);
     if (threadIdx.x == 0) {

@@ -188,7 +188,7 @@ class decoder:
                               ("sfo_ppm", "<f4")])       # struct lora_b200_rx_info
 
     def receive(self, iq, n_items=None, stride_items=None, host=None, sync_word=0x12, implicit_len=0, min_preamble=0,
-                max_cfo_hz=0.0, sfo_ppm=0.0, carrier_hz=0.0, soft=False, antennas=1, crc_list=0):
+                max_cfo_hz=0.0, sfo_ppm=0.0, carrier_hz=0.0, soft=False, antennas=1, crc_list=0, wide_cfo=False):
         """The dechirp-synchronised receiver (lora_b200_receive): decodes frames below the noise floor.  ``iq`` as for
         work_batch (host ndarray [n_streams, n_items] or a device tensor / pointer).  Returns (consumed, frames, info):
         consumed[s] = where stream s must be re-presented from, frames = FRAME_DTYPE records, info = RX_INFO_DTYPE records
@@ -204,7 +204,10 @@ class decoder:
         crc_list = K (1..12, needs soft): a frame whose payload CRC fails gets its K least reliable code words tried at their
         runner-up nibbles, and the cheapest combination that satisfies the CRC is published (frames_crc_last() reports it
         RECOVERED).  A frame whose errors lie outside the list passes a wrong combination with probability about
-        (2^K - 1) / 2^16; 0 (the default) is off."""
+        (2^K - 1) / 2^16; 0 (the default) is off.
+        wide_cfo: receive frames up to max_cfo_hz off carrier (finite, in (0, (fs - bw) / 2]: 3.5 bw at fs/bw = 8, bw / 2 at 2),
+        beyond the BW / 4 to which max_cfo_hz is clamped without it.  The screen then searches coarse offsets c * bw / 2,
+        c = -C..C, C = ceil((max_cfo_hz - bw / 4) / (bw / 2)), each costing about one more screen."""
         if isinstance(iq, np.ndarray):
             x = np.ascontiguousarray(iq, dtype=np.complex64)
             assert x.ndim == 2 and x.shape[0] == self.n_streams
@@ -218,7 +221,7 @@ class decoder:
                 stride_items = n_items
         p = N.RxParams(sync_word=int(sync_word) & 0xFF, implicit_len=int(implicit_len), min_preamble=int(min_preamble),
                        max_cfo_hz=float(max_cfo_hz), sfo_ppm=float(sfo_ppm), carrier_hz=float(carrier_hz), soft=int(soft),
-                       crc_list=int(crc_list))
+                       crc_list=int(crc_list), wide_cfo=int(wide_cfo))
         m = int(antennas)
         consumed = np.zeros(max(self.n_streams // m, 1) if m > 0 else 1, dtype=np.uint64)
         cptr = consumed.ctypes.data_as(C.POINTER(C.c_size_t))

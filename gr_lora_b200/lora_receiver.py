@@ -21,7 +21,7 @@ class lora_receiver:
     def __init__(self, samp_rate, center_freq, channel_list, bandwidth, sf, implicit, cr, crc, reduced_rate=False,
                  conj=False, decimation=1, disable_channelization=False, disable_drift_correction=False, cfo_feedback=False,
                  sync="reference", sync_word=0x12, implicit_len=0, clock_from_carrier=False, soft=False, antennas=1, crc_list=0,
-                 drop_bad_crc=False, **decoder_kw):
+                 drop_bad_crc=False, max_cfo_hz=0.0, wide_cfo=False, **decoder_kw):
         self.samp_rate, self.center_freq, self.channel_list = samp_rate, center_freq, list(channel_list)
         self.bandwidth, self.sf, self.implicit, self.cr, self.crc = bandwidth, sf, implicit, cr, crc
         self.decimation, self.conj = decimation, conj
@@ -45,6 +45,12 @@ class lora_receiver:
         if (crc_list or drop_bad_crc) and sync != "dechirp":
             raise ValueError("crc_list and drop_bad_crc need sync='dechirp'")
         self.crc_list, self.drop_bad_crc = int(crc_list), bool(drop_bad_crc)
+        # max_cfo_hz, wide_cfo: the carrier offsets the dechirp receiver searches (decoder.receive(..., max_cfo_hz, wide_cfo));
+        # wide_cfo takes max_cfo_hz beyond BW / 4, up to (fs - bw) / 2 of the decoder's rate.  With the channelizer in front,
+        # its filter (cutoff bw / 2 + 15 kHz) bounds the offset that reaches the decoder, whatever max_cfo_hz says.
+        if (max_cfo_hz or wide_cfo) and sync != "dechirp":
+            raise ValueError("max_cfo_hz and wide_cfo need sync='dechirp'")
+        self.max_cfo_hz, self.wide_cfo = float(max_cfo_hz), bool(wide_cfo)
         # antennas = M: run() takes an (M, n) capture of M phase-coherent antennas (one LO, one sample clock) and the dechirp
         # receiver combines them (decoder.receive(..., antennas=M)); with the channelizer every antenna gets its own
         # channelizer, which filters and rotates it exactly as the others, so the combining weights stay meaningful
@@ -165,7 +171,8 @@ class lora_receiver:
                 part = src + 8 * pos
             c, frames, _ = self.decoder.receive(part, n_items=n, stride_items=n if stride is None else stride, host=0, sync_word=self.sync_word,
                                                 implicit_len=self.implicit_len, carrier_hz=carrier, soft=self.soft,
-                                                antennas=self.antennas, crc_list=self.crc_list)
+                                                antennas=self.antennas, crc_list=self.crc_list, max_cfo_hz=self.max_cfo_hz,
+                                                wide_cfo=self.wide_cfo)
             crc = self.decoder.frames_crc_last() if self.drop_bad_crc else None
             for k, f in enumerate(frames):
                 if crc is not None and crc[k] == N.CRC_BAD:

@@ -141,7 +141,8 @@ int lora_b200_demod_llr_dev(lora_b200_decoder *d, const void *iq, size_t n_symbo
  * table (up[i] = 1); energy[i * m + a] = sum |x_a|^2 over the window; argmax_bin[i] / argmax_mag[i] = the first argmax of
  * the combined spectrum P[k] = sum_a |tmp_a[k]|^2 of the raw windows at pos[i] dechirped with c (as
  * lora_b200_demod_fft_antennas_dev, at any position) and sqrt(P[bin]).  m = 1 runs the one-row synchroniser's arithmetic,
- * m >= 2 the antenna synchroniser's.  Every window inside the row, bin in -N/2..N/2-1, |cfo_bins| <= N.  iq, out
+ * m >= 2 the antenna synchroniser's.  Every window inside the row, bin in -N/2..N/2-1, |cfo_bins| <= max(N, (D - 1) N / 2) (D = fs / bw:
+ * the widest offset of wide_cfo, 3.5 N at fs / bw = 8).  iq, out
  * (float2[n][m]), energy (float[n][m]), argmax_bin and argmax_mag are device pointers (energy, argmax_bin and argmax_mag
  * may be NULL), pos, cfo_bins, up and bin host arrays; returns when the results are written.  Test entry point. */
 int lora_b200_rs_window_dev(lora_b200_decoder *d, const void *iq, size_t n_items, uint32_t m, size_t stride_items, size_t n,
@@ -314,7 +315,14 @@ size_t lora_b200_frames_crc_last(lora_b200_decoder *d, const uint8_t **status);
  * (the RF frequency of the channel, 0 = none) each frame's clock offset follows from its own measured CFO.  Both 0: timing
  * fixed per frame, which holds while ppm x frame length stays below about a quarter chip.  sfo_ppm must be finite within
  * +-500 and carrier_hz 0 or finite and above the sample rate, else LORA_B200_EINVAL.
- * Limits: |CFO| <= max_cfo_hz <= BW / 4, no blind drift estimation (the clock offset is given or follows the CFO), data
+ * Carrier offsets beyond BW / 4 (p->wide_cfo = 1): the screen searches coarse offsets c * BW / 2, c = -C..C with
+ * C = max(0, ceil((max_cfo_hz - BW / 4) / (BW / 2))), each with its own shifted dechirp tables (one more screen per c, about
+ * 2 C + 1 times the screen's cost), and the synchroniser scores the three candidates of the N / 2 ambiguity; max_cfo_hz is
+ * taken as given and must be finite in (0, (fs - BW) / 2], the widest offset at which a frame still lies inside the sampled
+ * band (3.5 BW at fs / bw = 8, BW / 2 at 2).  wide_cfo other than 0 and 1, or an out-of-range max_cfo_hz with wide_cfo = 1:
+ * LORA_B200_EINVAL before any launch.  wide_cfo = 0 is the receiver without the search, max_cfo_hz clamped to BW / 4; with
+ * max_cfo_hz <= BW / 4 both give the same frames.
+ * Limits: |CFO| <= max_cfo_hz <= BW / 4 ((fs - BW) / 2 with wide_cfo), no blind drift estimation (the clock offset is given or follows the CFO), data
  * windows placed to the nearest sample, one frame at a time per stream, the decoder's SF only, several antennas per receiver
  * through lora_b200_receive_antennas (below).  The stream state machine's
  * per-stream state is not touched.
@@ -337,10 +345,11 @@ typedef struct lora_b200_rx_params {
     uint8_t  sync_word;          /* 0 = 0x12                                                    */
     uint8_t  soft;               /* 1: soft-decision decoding (per-bit LLRs, ML code words)      */
     uint8_t  crc_list;           /* CRC-aided list decoding of K code words (0 = off), see above */
-    uint8_t  reserved0[1];
+    uint8_t  wide_cfo;           /* 1: search carrier offsets up to max_cfo_hz beyond BW / 4      */
     uint32_t implicit_len;       /* payload bytes of implicit-header frames (incl. CRC bytes)  */
     uint32_t min_preamble;       /* windows of one phase (0 = 5)                                */
-    float    max_cfo_hz;         /* 0 = BW / 4; larger values are clamped to BW / 4             */
+    float    max_cfo_hz;         /* 0 = BW / 4; larger values are clamped to BW / 4 (wide_cfo = 0);
+                                    with wide_cfo = 1 taken as given, (0, (fs - BW) / 2]          */
     float    sfo_ppm;            /* clock offset of every frame in ppm (> 0: transmitter fast)  */
     uint32_t reserved1;
     double   carrier_hz;         /* RF carrier of the channel: each frame's clock offset also

@@ -15,7 +15,10 @@ part of assemble + K1).
 With --osr 2 the sensitivity curve is measured at fs/bw = 2 (250 kS/s, the generic K1 and LLR kernels at D = 2), and the
 real-time shape is decoded at fs/bw = 8 and at fs/bw = 2 (the same payloads, CFOs and layout, synthesised at each rate),
 alternating call by call; its results carry the suffix _osr8 / _osr2.
-Usage: python tools/bench_rx_sync.py [--quick] [--ppm P | --soft] [--osr 2]"""
+With --cfo-range LO HI every frame's CFO is uniform in +-[LO, HI] BW (a random sign), and every capture is decoded with the
+coarse-offset search (lora_b200_rx_params.wide_cfo, max_cfo_hz = --max-cfo, default HI, in BW) and without it, alternating;
+results carry the suffix _wide / _off.
+Usage: python tools/bench_rx_sync.py [--quick] [--ppm P | --soft | --cfo-range LO HI [--max-cfo M]] [--osr 2]"""
 from __future__ import annotations
 
 import argparse
@@ -51,6 +54,9 @@ def dec(sf, rr, **kw):
     return G.decoder(FS, BW, sf, False, 4, True, rr, quiet=True, **kw)
 
 
+CFO_RANGE = None                                     # (lo, hi) in BW: --cfo-range
+
+
 def capture(torch, sf, n_streams, per_stream, snr, seed, n_items=None, plen=10, ppm=0.0):
     import gr_lora_b200 as G
     from gr_lora_b200 import tx
@@ -62,6 +68,9 @@ def capture(torch, sf, n_streams, per_stream, snr, seed, n_items=None, plen=10, 
         n_items = per_stream * (flen + 5 * sps) + 8 * sps
     pays = [[bytes(rng.integers(0, 256, plen, dtype=np.uint8)) for _ in range(per_stream)] for _ in range(n_streams)]
     cfo = [[float(rng.uniform(-0.9, 0.9) * BW / 4) for _ in p] for p in pays]
+    if CFO_RANGE:
+        lo, hi = CFO_RANGE
+        cfo = [[float(rng.choice((-1.0, 1.0)) * rng.uniform(lo, hi) * BW) for _ in p] for p in pays]
     kw = {}
     if ppm:                                          # a crystal off by e ppm: CFO e * 868.1 Hz, clock off by e ppm
         sfo = [[float(rng.uniform(-ppm, ppm)) for _ in p] for p in pays]
@@ -137,8 +146,15 @@ def main():
                     "at two more SNRs 1.5 and 3 dB below each SF's lowest point")
     ap.add_argument("--osr", type=int, default=8, choices=(8, 2), help="fs/bw of the sensitivity curve; 2 also times the "
                     "real-time shape at fs/bw = 8 against fs/bw = 2")
+    ap.add_argument("--cfo-range", type=float, nargs=2, metavar=("LO", "HI"), help="CFO uniform in +-[LO, HI] BW; decode with "
+                    "and without wide_cfo, alternating")
+    ap.add_argument("--max-cfo", type=float, default=None, help="max_cfo_hz of the wide_cfo decodes, in BW (default: HI)")
     a = ap.parse_args()
     set_osr(a.osr)
+    global CFO_RANGE
+    CFO_RANGE = tuple(a.cfo_range) if a.cfo_range else None
+    if CFO_RANGE and (a.soft or a.ppm):
+        raise SystemExit("--cfo-range compares two modes of its own: give it without --soft and --ppm")
     if a.soft and a.ppm:
         raise SystemExit("--soft and --ppm each compare two modes: give one of them")
     if abs(a.ppm) * CARRIER * 1e-6 > BW / 4:
@@ -158,12 +174,15 @@ def main():
     # with --ppm, every measurement with the clock offset following the CFO ("tracked") and without ("fixed")
     # with --soft, every measurement with hard and with soft decisions
     modes = ({"tracked": dict(carrier_hz=CARRIER), "fixed": dict(carrier_hz=0.0)} if a.ppm else
-             {"hard": dict(soft=False), "soft": dict(soft=True)} if a.soft else {"": {}})
+             {"hard": dict(soft=False), "soft": dict(soft=True)} if a.soft else
+             {"wide": dict(wide_cfo=True, max_cfo_hz=(a.max_cfo or CFO_RANGE[1]) * BW), "off": {}} if CFO_RANGE else {"": {}})
+    if CFO_RANGE:
+        res["cfo_range_bw"], res["max_cfo_bw"] = list(CFO_RANGE), a.max_cfo or CFO_RANGE[1]
     res["soft"] = a.soft
     if a.osr != 8:
         res["osr"] = a.osr
     curve = {}
-    for sf, pts in POINTS.items():
+    for sf, pts in (POINTS.items() if a.runs > 0 else ()):
         rr = sf >= 11
         row = []
         if a.soft:
