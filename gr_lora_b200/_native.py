@@ -34,7 +34,8 @@ class RxParams(C.Structure):
     _fields_ = [("sync_word", C.c_uint8), ("soft", C.c_uint8), ("crc_list", C.c_uint8), ("wide_cfo", C.c_uint8),
                 ("implicit_len", C.c_uint32),
                 ("min_preamble", C.c_uint32),
-                ("max_cfo_hz", C.c_float), ("sfo_ppm", C.c_float), ("reserved1", C.c_uint32), ("carrier_hz", C.c_double)]
+                ("max_cfo_hz", C.c_float), ("sfo_ppm", C.c_float), ("fine_toa", C.c_uint8), ("reserved1", C.c_uint8 * 3),
+                ("carrier_hz", C.c_double)]
 
 
 FRAME_CB = C.CFUNCTYPE(None, C.c_void_p, C.c_uint32, C.POINTER(C.c_uint8), C.c_size_t)
@@ -69,6 +70,7 @@ SIGNATURES = {
     "lora_b200_demod_fft_antennas_dev": (_i, [_vp, _vp, _u32, _u32, _sz, _sz, _vp, _vp, _vp]),
     "lora_b200_rs_window_dev": (_i, [_vp, _vp, _sz, _u32, _sz, _sz, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     "lora_b200_rs_frame_dev": (_i, [_vp, _vp, _sz, _u32, _sz, _sz, _vp, _vp, _vp, _vp, _u32, _u32, _vp, _vp, _vp]),
+    "lora_b200_rs_toa_dev": (_i, [_vp, _vp, _sz, _u32, _sz, _sz, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     "lora_b200_demod_fft_host_sc16": (_i, [_vp, _vp, C.c_float, _sz, _vp, _vp]),
     "lora_b200_demod_gradient_dev": (_i, [_vp, _vp, _sz, _vp, _vp]),
     "lora_b200_ifreq_dev": (_i, [_vp, _vp, _sz, _u32, _vp, _vp]),
@@ -89,6 +91,7 @@ SIGNATURES = {
     "lora_b200_frames_crc_last": (_sz, [_vp, C.POINTER(_vp)]),
     "lora_b200_receive": (_i, [_vp, _vp, _sz, _sz, _i, C.POINTER(RxParams), C.POINTER(_sz)]),
     "lora_b200_rx_info_last": (_sz, [_vp, C.POINTER(_vp), C.POINTER(C.c_uint32)]),
+    "lora_b200_rx_toa_last": (_sz, [_vp, C.POINTER(_vp)]),
     "lora_b200_receive_antennas": (_i, [_vp, _vp, _sz, _sz, _i, _u32, C.POINTER(RxParams), C.POINTER(_sz)]),
     "lora_b200_rx_channels_last": (_sz, [_vp, C.POINTER(_vp), C.POINTER(C.c_uint32)]),
     "lora_b200_stream_state": (_i, [_vp, _u32]),

@@ -214,6 +214,21 @@ struct RsHostOps {
         for (uint32_t n = 0; n < sps; n++) e += (double)x[pos + n].x * x[pos + n].x + (double)x[pos + n].y * x[pos + n].y;
         return (float)e;
     }
+    // rs_toa's window powers: |binval(pos, f0 + k df, use_up, 0)|^2, each frequency formed in double, the phase counted from org
+    template <int K> void tones(long long pos, long long org, float f0, float df, bool use_up, float *p) {
+        const float2 *ch = use_up ? up : down;
+        for (int k = 0; k < K; k++) {
+            const double f = (double)f0 + (double)k * (double)df;
+            double re = 0.0, im = 0.0;
+            for (uint32_t n = 0; n < sps; n++) {
+                const double a = -2.0 * M_PI * f * (double)(pos - org + n) / sps;
+                const float2 v = lb::cmul(x[pos + n], ch[n]);
+                re += v.x * cos(a) - v.y * sin(a);
+                im += v.x * sin(a) + v.y * cos(a);
+            }
+            p[k] = (float)(re * re + im * im);
+        }
+    }
 };
 
 // ... of a receiver with m antennas, rows one.x + a * one.n_items: the combined K1 argmax through k1_antennas_emulate
@@ -240,6 +255,14 @@ struct RsHostAntOps {
         energies(pos, e);
         for (int a = 0; a < M; a++) s += e[a];
         return s;
+    }
+    template <int K> void tones(long long pos, long long org, float f0, float df, bool use_up, float *p) {
+        for (int k = 0; k < K; k++) p[k] = 0.f;
+        for (uint32_t a = 0; a < m; a++) {
+            float q[K];
+            row(a).tones<K>(pos, org, f0, df, use_up, q);
+            for (int k = 0; k < K; k++) p[k] += q[k];
+        }
     }
 };
 
@@ -325,7 +348,7 @@ uint32_t rs_host_receive(const float2 *x, size_t n_items, uint32_t m, const floa
                          uint32_t osr, uint32_t cr, int implicit, int crc, int reduced_rate, uint32_t sync_word, uint32_t implicit_len,
                          uint32_t min_preamble, float sfo_ppm, double carrier_hz, int soft, long long *start, float *cfo_bins,
                          float *snr_db, int32_t *status, float *sfo, uint8_t *payload, uint32_t *len, float2 *chan, uint32_t cap,
-                         uint32_t crc_list = 0, uint8_t *crc_status = nullptr, float max_cfo_bins = 0.f) {
+                         uint32_t crc_list = 0, uint8_t *crc_status = nullptr, float max_cfo_bins = 0.f, double *toa = nullptr) {
     if (osr != 8u && osr != 2u) return 0;
     const uint32_t N = 1u << sf, sps = osr * N;
     const double bin_hz = 125e3 / N;
@@ -381,6 +404,14 @@ uint32_t rs_host_receive(const float2 *x, size_t n_items, uint32_t m, const floa
             od.x = y.data();
         }
         start[nf] = r.start; cfo_bins[nf] = r.cfo_bins; snr_db[nf] = r.snr_db; status[nf] = 2; len[nf] = 0;
+        if (toa) {
+            toa[nf] = NAN;
+            if (r.status == lb::RS_OK) {
+                const lb::RsToa t = m == 1 ? (drift ? lb::rs_toa<true>(o, p, r) : lb::rs_toa<false>(o, p, r))
+                                           : (drift ? lb::rs_toa<true>(oa, p, r) : lb::rs_toa<false>(oa, p, r));
+                toa[nf] = t.toa;
+            }
+        }
         if (crc_status) crc_status[nf] = LORA_CRC_NONE;
         if (sfo) sfo[nf] = r.sfo_ppm;
         // end of the window of data symbol n - 1
@@ -501,6 +532,39 @@ uint32_t lb_emul_rx_receive_wide(const float2 *x, size_t n_items, uint32_t m, co
     return rs_host_receive(x, n_items, m, down, up, tw, sf, osr, cr, implicit, crc, reduced_rate, sync_word, implicit_len, min_preamble,
                            sfo_ppm, carrier_hz, soft, start, cfo_bins, snr_db, status, sfo, payload, len, nullptr, cap, 0, nullptr,
                            max_cfo_bins);
+}
+
+// lb_emul_rx_receive_wide (max_cfo_bins 0: |CFO| <= N / 4 without the search) with the fine time of arrival of
+// lora_b200_rx_params.fine_toa: toa[f] of every synchronised frame (rs_toa at its final synchronisation; NaN unless it
+// synchronised, status 0 or 1)
+uint32_t lb_emul_rx_receive_toa(const float2 *x, size_t n_items, uint32_t m, const float2 *down, const float2 *up, const float2 *tw,
+                                uint32_t sf, uint32_t osr, uint32_t cr, int implicit, int crc, int reduced_rate, uint32_t sync_word,
+                                uint32_t implicit_len, uint32_t min_preamble, float sfo_ppm, double carrier_hz, int soft, float max_cfo_bins,
+                                long long *start, float *cfo_bins, float *snr_db, int32_t *status, float *sfo, uint8_t *payload,
+                                uint32_t *len, double *toa, uint32_t cap) {
+    if (m < 1 || m > (uint32_t)lb::RS_MAX_ANTENNAS || max_cfo_bins < 0.f || max_cfo_bins > (float)((osr - 1u) << sf) / 2.0f) return 0;
+    return rs_host_receive(x, n_items, m, down, up, tw, sf, osr, cr, implicit, crc, reduced_rate, sync_word, implicit_len, min_preamble,
+                           sfo_ppm, carrier_hz, soft, start, cfo_bins, snr_db, status, sfo, payload, len, nullptr, cap, 0, nullptr,
+                           max_cfo_bins, toa);
+}
+
+// rs_toa on given frames (lora_b200_rs_toa_dev on the host): frame i at start[i] with cfo_bins[i] and sfo_ppm[i] on the m rows
+// x[a * n_items ..] (fs = osr x 125 kHz) -> nu_a[i], nu_b[i], toa[i]; -1 for another osr or m
+int lb_emul_rs_toa(const float2 *x, size_t n_items, uint32_t m, const float2 *down, const float2 *up, const float2 *tw, uint32_t sf,
+                   uint32_t osr, size_t n, const long long *start, const float *cfo_bins, const float *sfo_ppm, float *nu_a, float *nu_b,
+                   double *toa) {
+    if ((osr != 8u && osr != 2u) || m < 1 || m > (uint32_t)lb::RS_MAX_ANTENNAS) return -1;
+    const uint32_t N = 1u << sf, sps = osr * N;
+    lb::RsParams p{sps, N, osr, 0.f, 5u, {0u, 0u}, (float)N / 4.0f, 0.f, 0};
+    RsHostOps o{x, (long long)n_items, down, up, tw, sps, sf, osr, nullptr, 0};
+    RsHostAntOps oa{o, m};
+    for (size_t i = 0; i < n; i++) {
+        const lb::RsFrame r{start[i], 0u, cfo_bins[i], 0.f, lb::RS_OK, 0, sfo_ppm[i]};
+        const lb::RsToa t = m == 1 ? (sfo_ppm[i] != 0.f ? lb::rs_toa<true>(o, p, r) : lb::rs_toa<false>(o, p, r))
+                                   : (sfo_ppm[i] != 0.f ? lb::rs_toa<true>(oa, p, r) : lb::rs_toa<false>(oa, p, r));
+        nu_a[i] = t.nu_a; nu_b[i] = t.nu_b; toa[i] = t.toa;
+    }
+    return 0;
 }
 
 // lb_emul_rx_receive_osr at fs/bw = 8 (fs = 1 MHz)

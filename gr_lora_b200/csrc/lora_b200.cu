@@ -154,6 +154,9 @@ struct lora_b200_decoder : A1Params {
     DeviceBuffer<float2> d_rs_shift;
     std::vector<float2> h_rs_shift;
     int rs_shift_hyp = 0;
+    // rx_params.fine_toa: per published frame, its time of arrival (rs_toa_kernel), for lora_b200_rx_toa_last
+    DeviceBuffer<double> d_rs_toa;
+    std::vector<double> rs_toa;
 };
 
 namespace {
@@ -470,6 +473,7 @@ int rx_finish(lora_b200_decoder *d, uint32_t stream_base, uint32_t n_launch, siz
     d->rs_info.clear();                           // (lora_b200_rx_info_last describes lora_b200_receive calls only)
     d->rs_chan.clear();
     d->rs_recovered.clear();
+    d->rs_toa.clear();
     for (uint32_t k = 0; k < n_frames; k++) {
         const RxFrameOut &f = d->h_frames[order[k]];
         d->h_sorted[k] = f;
@@ -920,6 +924,7 @@ int lora_b200_reset(lora_b200_decoder *d) {
     if (d->d_trace_n) CU(cudaMemset(d->d_trace_n, 0, sizeof(uint32_t) * d->cfg.n_streams));
     d->h_sorted.clear();
     d->rs_recovered.clear();
+    d->rs_toa.clear();
     for (auto &so : d->stdout_last) so.clear();
     return LORA_B200_OK;
 }
@@ -1142,6 +1147,22 @@ static int rs_assemble(lora_b200_decoder *d, const float2 *x, size_t stride, siz
     return launched(d);
 }
 
+// the fine time of arrival of n frames (frames[pub[k]], pub NULL: frames[k]) into toa[k] and nu[k] (may be NULL); DRIFT as
+// the synchroniser's (rs_drift)
+template <int SF, int D, bool DRIFT>
+static int rs_toa_launch(lora_b200_decoder *d, const float2 *x, size_t stride, size_t n_items, uint32_t m, const RsParams &rp,
+                         const RsFrame *frames, const uint32_t *pub, uint32_t n, double *toa, float2 *nu) {
+    rs_toa_kernel<SF, D, DRIFT><<<n, RX_THREADS, 0, d->rx_stream>>>(x, stride, n_items, m, tab<float2>(d, d->toff.down), tab<float2>(d, d->toff.up),
+                                                                    tab<float2>(d, d->toff.tw), rp, frames, pub, toa, nu);
+    return launched(d);
+}
+static int rs_toa(lora_b200_decoder *d, const float2 *x, size_t stride, size_t n_items, uint32_t m, const RsParams &rp, const RsFrame *frames,
+                  const uint32_t *pub, uint32_t n, double *toa, float2 *nu) {
+    return with_sf_osr(d->cfg.sf, d->k1_osr, unsupported_sf(d), [&](auto SF, auto D) {
+        return with_bool(rs_drift(rp), [&](auto DRIFT) { return rs_toa_launch<SF, D, DRIFT>(d, x, stride, n_items, m, rp, frames, pub, n, toa, nu); });
+    });
+}
+
 // lora_b200_receive (m = 1) and lora_b200_receive_antennas: the receiver of group g reads rows g m .. g m + m - 1
 static int rs_receive(lora_b200_decoder *d, const void *iq, size_t n_items, size_t stride_items, int host_ptr, uint32_t m,
                       const lora_b200_rx_params *prm, size_t *consumed) {
@@ -1162,6 +1183,7 @@ static int rs_receive(lora_b200_decoder *d, const void *iq, size_t n_items, size
     if (P.crc_list > RS_CRC_MAX_LIST || (P.crc_list && !P.soft))
         return fail(LORA_B200_EINVAL, "crc_list must be 0..%u and needs soft = 1, got %u", RS_CRC_MAX_LIST, (unsigned)P.crc_list);
     if (P.wide_cfo > 1u) return fail(LORA_B200_EINVAL, "wide_cfo must be 0 or 1, got %u", (unsigned)P.wide_cfo);
+    if (P.fine_toa > 1u) return fail(LORA_B200_EINVAL, "fine_toa must be 0 or 1, got %u", (unsigned)P.fine_toa);
     const float band_max = (float)((d->samples_per_second - (double)d->cfg.bandwidth) / 2.0);    // (fs - BW) / 2
     if (P.wide_cfo && !(std::isfinite(P.max_cfo_hz) && P.max_cfo_hz > 0.f && P.max_cfo_hz <= band_max))
         return fail(LORA_B200_EINVAL, "wide_cfo needs max_cfo_hz in (0, %g], got %g", (double)band_max, (double)P.max_cfo_hz);
@@ -1185,6 +1207,7 @@ static int rs_receive(lora_b200_decoder *d, const void *iq, size_t n_items, size
     d->rs_chan.clear();
     d->rs_chan_m = m;
     d->rs_recovered.clear();
+    d->rs_toa.clear();
     const size_t guard = (size_t)(rp.min_preamble + 4u) * sps, none = ~(size_t)0;
     std::vector<size_t> end_pub(ns, 0), hold(ns, none);
     auto finish = [&]() {
@@ -1401,6 +1424,12 @@ static int rs_receive(lora_b200_decoder *d, const void *iq, size_t n_items, size
     CU(cudaMemsetAsync(d->d_rs_out, 0, sizeof(RxFrameOut) * np, st));
     k8_frames_kernel<<<(int)std::min<uint32_t>(np, (uint32_t)d->n_sms * 4u), 128, 0, st>>>(d->d_rs_recs, d->d_rs_nframes, np, d->d_rs_out);
     if (int rc = launched(d)) return rc;
+    if (P.fine_toa) {
+        CU(d->d_rs_toa.reserve(np));
+        if (int rc = rs_toa(d, x, stride, n_items, m, rp, d->d_rs_frames, t_pub, np, d->d_rs_toa, nullptr)) return rc;
+        d->rs_toa.resize(np);
+        CU(cudaMemcpyAsync(d->rs_toa.data(), d->d_rs_toa, sizeof(double) * np, cudaMemcpyDeviceToHost, st));
+    }
     d->h_sorted.resize(np);
     CU(cudaMemcpyAsync(d->h_sorted.data(), d->d_rs_out, sizeof(RxFrameOut) * np, cudaMemcpyDeviceToHost, st));
     std::vector<float2> chan;
@@ -1463,8 +1492,8 @@ int lora_b200_demod_fft_antennas_dev(lora_b200_decoder *d, const void *iq, uint3
 static_assert(sizeof(lora_b200_rx_info) == 32 && sizeof(lora_b200_rx_params) == 32 && offsetof(lora_b200_rx_params, soft) == 1 &&
               offsetof(lora_b200_rx_params, crc_list) == 2 && offsetof(lora_b200_rx_params, wide_cfo) == 3 &&
               offsetof(lora_b200_rx_params, implicit_len) == 4 &&
-              offsetof(lora_b200_rx_params, sfo_ppm) == 16 &&
-              offsetof(lora_b200_rx_params, carrier_hz) == 24 && offsetof(lora_b200_rx_info, sfo_ppm) == 28, "lora_b200_rx_* layout");
+              offsetof(lora_b200_rx_params, sfo_ppm) == 16 && offsetof(lora_b200_rx_params, fine_toa) == 20 &&
+              offsetof(lora_b200_rx_params, reserved1) == 21 && offsetof(lora_b200_rx_params, carrier_hz) == 24 && offsetof(lora_b200_rx_info, sfo_ppm) == 28, "lora_b200_rx_* layout");
 
 }  // extern "C"
 
@@ -1586,6 +1615,51 @@ int lora_b200_rs_frame_dev(lora_b200_decoder *d, const void *iq, size_t n_items,
         rc = launched(d);
     }
     CU(cudaStreamSynchronize(d->rx_stream));     // (before df and dt are freed)
+    return rc;
+}
+
+size_t lora_b200_rx_toa_last(lora_b200_decoder *d, const double **toa) {
+    if (!d || !toa) { fail(LORA_B200_EINVAL, "null argument"); return 0; }
+    *toa = d->rs_toa.data();
+    return d->rs_toa.size();
+}
+
+int lora_b200_rs_toa_dev(lora_b200_decoder *d, const void *iq, size_t n_items, uint32_t m, size_t stride_items, size_t n,
+                         const uint32_t *group, const int64_t *start, const float *cfo_bins, const float *sfo_ppm, float *nu_a,
+                         float *nu_b, double *toa) {
+    if (!d || (n && (!iq || !group || !start || !cfo_bins || !sfo_ppm || !nu_a || !nu_b || !toa))) return fail(LORA_B200_EINVAL, "null argument");
+    if (int rc = need_k1(d, "the dechirp receiver")) return rc;
+    if (m < 1 || m > (uint32_t)RS_MAX_ANTENNAS) return fail(LORA_B200_EINVAL, "m must be 1..%d, got %u", RS_MAX_ANTENNAS, m);
+    if (stride_items < n_items) return fail(LORA_B200_EINVAL, "stride_items %zu < n_items %zu", stride_items, n_items);
+    if (n > 0x7FFFFFFFu) return fail(LORA_B200_EINVAL, "too many frames: %zu", n);
+    const long long cfo_lim = std::max<long long>(d->n_bins, ((long long)d->decim - 1) * d->n_bins / 2);   // (as rs_window_dev)
+    std::vector<RsFrame> fr(n);
+    bool drift = false;
+    for (size_t i = 0; i < n; i++) {
+        if (!std::isfinite(cfo_bins[i]) || std::fabs(cfo_bins[i]) > (float)cfo_lim || !std::isfinite(sfo_ppm[i]) || std::fabs(sfo_ppm[i]) > 1e4f)
+            return fail(LORA_B200_EINVAL, "frame %zu: cfo_bins %g or sfo_ppm %g out of range", i, (double)cfo_bins[i], (double)sfo_ppm[i]);
+        fr[i] = RsFrame{(long long)start[i], group[i], cfo_bins[i], 0.f, RS_OK, 0, sfo_ppm[i]};
+        drift = drift || sfo_ppm[i] != 0.f;
+    }
+    CU(cudaSetDevice(d->device));
+    if (n == 0) return LORA_B200_OK;
+    DeviceBuffer<RsFrame> df;
+    DeviceBuffer<double> dt;
+    DeviceBuffer<float2> dn;
+    CU(df.reserve(n));
+    CU(dt.reserve(n));
+    CU(dn.reserve(n));
+    CU(cudaMemcpyAsync(df, fr.data(), sizeof(RsFrame) * n, cudaMemcpyHostToDevice, d->rx_stream));
+    // rs_toa reads sps, decim; DRIFT from any frame's clock offset (a frame with 0 gives the DRIFT = false result either way)
+    RsParams rp{d->sps, d->n_bins, d->decim, drift ? 1.f : 0.f, 5u, {0u, 0u}, (float)d->n_bins / 4.0f, 0.f, 0};
+    int rc = rs_toa(d, (const float2 *)iq, stride_items, n_items, m, rp, df, nullptr, (uint32_t)n, dt, dn);
+    std::vector<float2> nu(n);
+    if (rc == LORA_B200_OK) {
+        CU(cudaMemcpyAsync(toa, dt, sizeof(double) * n, cudaMemcpyDeviceToHost, d->rx_stream));
+        CU(cudaMemcpyAsync(nu.data(), dn, sizeof(float2) * n, cudaMemcpyDeviceToHost, d->rx_stream));
+    }
+    CU(cudaStreamSynchronize(d->rx_stream));     // (before df, dt and dn are freed)
+    for (size_t i = 0; rc == LORA_B200_OK && i < n; i++) { nu_a[i] = nu[i].x; nu_b[i] = nu[i].y; }
     return rc;
 }
 

@@ -388,6 +388,104 @@ LB_HD float rs_channels(Ops &ops, const RsParams &p, const RsFrame &r, uint32_t 
     return 10.0f * log10f(snr * (float)p.decim);
 }
 
+// ---- fine time of arrival (rx_params.fine_toa) --------------------------------------------------------------------------
+// A synchronised frame (start t, CFO F bins, clock offset delta = r.sfo_ppm 1e-6) whose transmitter time 0 lands at row position
+// t + eps.  Its window j lies at pos_j = rs_pos(t, j) = t + j sps / (1 + delta) + r_j (r_j: that window's own rounding), so the
+// symbol started tau_j = r_j - eps samples before it.  Dechirped, preamble window j (down-chirp) shows its tone at
+// F + tau_j / decim + delta N / 2 and SFD window j (up-chirp) at F - tau_j / decim - delta N / 2: the chirps are stretched by
+// the transmitter's clock, which moves the tone at a window's centre by +-delta N / 2.  Each window is evaluated at its own
+// frequency F + nu + r_j / decim (preamble) or F + nu - r_j / decim (SFD), so that all of them peak at one nu:
+//   P_up(nu) = sum_{j = 1..6} sum_a |binval_a(pos_j, F + nu + r_j / decim, down, 0)|^2   peaks at nu_A = -eps / decim + delta N / 2
+//   P_dn(nu) = sum_{j = 10, 11} sum_a |binval_a(pos_j, F + nu - r_j / decim, up, 0)|^2    peaks at nu_B = +eps / decim - delta N / 2
+// eps = decim (nu_B - nu_A) / 2 + delta sps / 2; F's own error moves both peaks alike and cancels.  Peak search, the same for
+// nu_A and nu_B: the grid of RS_TOA_GRID points over +-W, W = (decim / 2 + 1) / decim + 1/4 bins (the timing refinement's
+// residual of at most decim / 2 + 1 samples, and a quarter bin for F), step h = 2 W / (RS_TOA_GRID - 1) <= 1/4 bin (inside the
+// main lobe of the peak, whose first nulls lie +-1 bin out); the first maximum, moved to the vertex of the parabola through it
+// and its neighbours; then RS_TOA_ROUNDS times: h /= 4 and the vertex of the parabola through nu - h, nu, nu + h.  A vertex is
+// taken only where the three values are concave, and clamped to +-h.  Windows outside the row are left out; a frame without
+// a preamble or an SFD window inside the row gets toa = NaN.  Ops::tones<K>(pos, org, f0, df, up, p) gives
+// p[k] = sum_a |binval_a(pos, f0 + k df, up, 0)|^2 for k < K in one pass over the window, its de-rotation phase counted from
+// row position org = t instead of 0 (a phase common to the window, which |.|^2 drops): the same frame re-presented at another
+// row offset gives the same sums, bit for bit, from the same t, F and clock offset.
+constexpr int RS_TOA_GRID = 11;
+constexpr int RS_TOA_ROUNDS = 2;
+constexpr int RS_TOA_WINDOWS = 8;
+LB_HD int rs_toa_j(int i) { return i < 6 ? i + 1 : i + 4; }      // windows 1..6 (preamble), 10, 11 (SFD)
+
+struct RsToa {
+    float nu_a, nu_b;                  // the peaks of P_up and P_dn, in bins from F
+    double toa;                        // t + eps, in the row's samples
+};
+
+LB_HD float rs_toa_vertex(float ym, float y0, float yp, float h) {
+    const float den = ym - 2.0f * y0 + yp;
+    if (!(den < 0.0f)) return 0.0f;
+    const float d = 0.5f * h * (ym - yp) / den;
+    return d < -h ? -h : d > h ? h : d;
+}
+
+#ifdef __CUDACC__
+#pragma nv_exec_check_disable
+#endif
+template <bool DRIFT, class Ops>
+LB_HD RsToa rs_toa(Ops &ops, const RsParams &p, const RsFrame &r) {
+    const float decim = (float)p.decim, W = (0.5f * decim + 1.0f) / decim + 0.25f;
+    const double rate = 1.0 + 1e-6 * (double)r.sfo_ppm;
+    long long pos[RS_TOA_WINDOWS];
+    float off[RS_TOA_WINDOWS];         // the frequency window i is evaluated at, minus F + nu: +-r_j / decim
+    bool in[RS_TOA_WINDOWS], have_a = false, have_b = false;
+    for (int i = 0; i < RS_TOA_WINDOWS; i++) {
+        const int j = rs_toa_j(i);
+        pos[i] = rs_pos<DRIFT>(r.start, j, p.sps, r.sfo_ppm);
+        const double rj = DRIFT ? (double)(pos[i] - r.start) - (double)j * (double)p.sps / rate : 0.0;
+        off[i] = (float)(i < 6 ? rj / (double)p.decim : -rj / (double)p.decim);
+        in[i] = pos[i] >= 0 && ops.in_range(pos[i]);
+        if (in[i]) { if (i < 6) have_a = true; else have_b = true; }
+    }
+    RsToa out;
+    if (!have_a || !have_b) {
+        out.nu_a = out.nu_b = 0.0f;
+        out.toa = (double)NAN;
+        return out;
+    }
+    // the grid
+    float h = 2.0f * W / (float)(RS_TOA_GRID - 1);
+    float pa[RS_TOA_GRID], pb[RS_TOA_GRID];
+    for (int k = 0; k < RS_TOA_GRID; k++) { pa[k] = 0.0f; pb[k] = 0.0f; }
+    for (int i = 0; i < RS_TOA_WINDOWS; i++) {
+        if (!in[i]) continue;
+        float t[RS_TOA_GRID];
+        ops.template tones<RS_TOA_GRID>(pos[i], r.start, r.cfo_bins + off[i] - W, h, i >= 6, t);
+        for (int k = 0; k < RS_TOA_GRID; k++) { if (i < 6) pa[k] += t[k]; else pb[k] += t[k]; }
+    }
+    float nu[2];
+    for (int s = 0; s < 2; s++) {
+        const float *q = s ? pb : pa;
+        int kb = 0;
+        for (int k = 1; k < RS_TOA_GRID; k++) if (q[k] > q[kb]) kb = k;
+        nu[s] = -W + (float)kb * h;
+        if (kb > 0 && kb < RS_TOA_GRID - 1) nu[s] += rs_toa_vertex(q[kb - 1], q[kb], q[kb + 1], h);
+    }
+    // the refinements
+    for (int round = 0; round < RS_TOA_ROUNDS; round++) {
+        h *= 0.25f;
+        float qa[3] = {0.0f, 0.0f, 0.0f}, qb[3] = {0.0f, 0.0f, 0.0f};
+        for (int i = 0; i < RS_TOA_WINDOWS; i++) {
+            if (!in[i]) continue;
+            float t[3];
+            ops.template tones<3>(pos[i], r.start, r.cfo_bins + off[i] + nu[i >= 6] - h, h, i >= 6, t);
+            for (int k = 0; k < 3; k++) { if (i < 6) qa[k] += t[k]; else qb[k] += t[k]; }
+        }
+        nu[0] += rs_toa_vertex(qa[0], qa[1], qa[2], h);
+        nu[1] += rs_toa_vertex(qb[0], qb[1], qb[2], h);
+    }
+    out.nu_a = nu[0];
+    out.nu_b = nu[1];
+    const double delta = DRIFT ? 1e-6 * (double)r.sfo_ppm : 0.0;
+    out.toa = (double)r.start + 0.5 * (double)p.decim * ((double)nu[1] - (double)nu[0]) + 0.5 * delta * (double)p.sps;
+    return out;
+}
+
 // ---- the integer chain of one frame -------------------------------------------------------------------------------------
 // FFT demodulator's bin -> rx_symbol_commit (rx_stream.cuh) for the 8 header-block symbols.  Returns the payload symbols
 // to read, or -1 when the explicit header's checksum (or coding rate) is wrong.  implicit_len: payload bytes of an
@@ -631,6 +729,68 @@ __global__ void rs_detect_kernel(const uint32_t *__restrict__ bins0, const float
     n_cands[s] = rs_detect_stream<S_MAX>(b, m, n, p, cands + (size_t)s * cap, cap, dropped + s);
 }
 
+// sum of NV values over the CTA through red[RX_WARPS * NV] (shared), in a fixed order; result valid in every thread
+template <int NV>
+LB_D void rs_block_sums(float (&v)[NV], float *red) {
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+#pragma unroll
+    for (int k = 0; k < NV; k++) {
+        const float s = warp_sum(v[k]);
+        if (lane == 0) red[warp * NV + k] = s;
+    }
+    __syncthreads();
+#pragma unroll
+    for (int k = 0; k < NV; k++) {
+        float t = 0.f;
+        for (int w = 0; w < RX_WARPS; w++) t += red[w * NV + k];
+        v[k] = t;
+    }
+    __syncthreads();
+}
+
+// the window sums of rs_toa: sample n's chirp product, de-rotated by f0 (phase counted from org), is formed once and stepped through the K frequencies
+// f0 + k df by w = e^{-2 pi j df n / sps} (the phase e^{-2 pi j k df pos / sps} common to the window drops out of |.|^2); the
+// 2 K M sums of M rows reduce through red (RX_WARPS * 2 K M floats of shared memory)
+template <int K, int M>
+LB_D void rs_tones(const float2 *x, size_t stride, uint32_t m, long long pos, long long org, const float2 *ch, uint32_t sps, float f0,
+                   float df, float *red, float *pw) {
+    double base = (double)f0 * (double)(pos - org) / (double)sps;
+    base -= floor(base);
+    const float fb = (float)base, fr = f0 / (float)sps, fd = df / (float)sps;
+    float s[2 * K * M];
+#pragma unroll
+    for (int k = 0; k < 2 * K * M; k++) s[k] = 0.f;
+    for (uint32_t n = threadIdx.x; n < sps; n += RX_THREADS) {
+        float t = fmaf(fr, (float)n, fb);
+        t -= floorf(t);
+        float u = fd * (float)n;
+        u -= floorf(u);
+        float sn, cs, sw, cw;
+        sincospif(-2.0f * t, &sn, &cs);
+        sincospif(-2.0f * u, &sw, &cw);
+        const float2 q = cmul(__ldg(ch + n), make_float2(cs, sn)), w = make_float2(cw, sw);
+#pragma unroll
+        for (int a = 0; a < M; a++) {
+            if (a < (int)m) {
+                float2 y = cmul(x[(size_t)a * stride + pos + n], q);
+#pragma unroll
+                for (int k = 0; k < K; k++) {
+                    s[2 * (a * K + k)] += y.x; s[2 * (a * K + k) + 1] += y.y;
+                    y = cmul(y, w);
+                }
+            }
+        }
+    }
+    rs_block_sums<2 * K * M>(s, red);
+#pragma unroll
+    for (int k = 0; k < K; k++) {
+        float p = 0.f;
+#pragma unroll
+        for (int a = 0; a < M; a++) p += s[2 * (a * K + k)] * s[2 * (a * K + k)] + s[2 * (a * K + k) + 1] * s[2 * (a * K + k) + 1];
+        pw[k] = p;
+    }
+}
+
 // the windows of one candidate, block-collective (all threads call every member with the same arguments); D = sps / N is
 // argmax's only use of the sample rate (binval and energy take sps at run time)
 template <int SF, int D = 8>
@@ -687,6 +847,10 @@ struct RsDevOps {
         return make_float2(v[0], v[1]);
     }
     LB_D void binvals(long long pos, float F, bool use_up, int bin, float2 *v) { v[0] = binval(pos, F, use_up, bin); }
+    // (rs_toa: smem holds RX_WARPS * 2 K floats)
+    template <int K> LB_D void tones(long long pos, long long org, float f0, float df, bool use_up, float *p) {
+        rs_tones<K, 1>(x, 0, 1, pos, org, use_up ? up : down, sps, f0, df, (float *)smem, p);
+    }
     LB_D float energy(long long pos) {
         float v[1] = {0.f};
         for (uint32_t n = threadIdx.x; n < sps; n += RX_THREADS) { const float2 a = x[pos + n]; v[0] += a.x * a.x + a.y * a.y; }
@@ -786,7 +950,37 @@ struct RsAntOps {
         for (int a = 0; a < M; a++) s += e[a];
         return s;
     }
+    // (rs_toa: one.smem holds RX_WARPS * 2 K M floats)
+    template <int K> LB_D void tones(long long pos, long long org, float f0, float df, bool use_up, float *p) {
+        rs_tones<K, M>(one.x, stride, m, pos, org, use_up ? one.up : one.down, one.sps, f0, df, (float *)one.smem, p);
+    }
 };
+
+// fine time of arrival: one CTA per frame k, frames[pub[k]] (pub NULL: frames[k]) on receiver group frames[..].stream, rows
+// stream * m + a, `stride` apart (m = 1: RsDevOps, as rs_sync_kernel; m >= 2: RsAntOps, as rs_sync_antennas_kernel): rs_toa
+// into toa[k] and, when given, (nu_A, nu_B) into nu[k]
+template <int SF, int D, bool DRIFT>
+__global__ void __launch_bounds__(RX_THREADS)
+rs_toa_kernel(const float2 *__restrict__ iq, size_t stride, size_t n_items, uint32_t m, const float2 *down, const float2 *up,
+              const float2 *tw, RsParams p, const RsFrame *__restrict__ frames, const uint32_t *__restrict__ pub, double *__restrict__ toa,
+              float2 *__restrict__ nu) {
+    __shared__ float2 red[RX_WARPS * RS_TOA_GRID * RS_MAX_ANTENNAS];
+    __shared__ RxShared sh;
+    const RsFrame r = frames[pub ? pub[blockIdx.x] : blockIdx.x];
+    const float2 *x = iq + (size_t)r.stream * m * stride;
+    RsToa t;
+    if (m == 1) {
+        RsDevOps<SF, D> ops{x, (long long)n_items, down, up, tw, p.sps, red, &sh, nullptr, 0};
+        t = rs_toa<DRIFT>(ops, p, r);
+    } else {
+        RsAntOps<SF, D> ops{{x, (long long)n_items, down, up, tw, p.sps, red, &sh, nullptr, 0}, stride, m};
+        t = rs_toa<DRIFT>(ops, p, r);
+    }
+    if (threadIdx.x == 0) {
+        toa[blockIdx.x] = t.toa;
+        if (nu) nu[blockIdx.x] = make_float2(t.nu_a, t.nu_b);
+    }
+}
 
 // synchronise: one CTA per candidate slot (stream = slot / cap); synchronised frames are appended to `frames`
 template <int SF, int D, bool DRIFT>

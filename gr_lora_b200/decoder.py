@@ -188,7 +188,8 @@ class decoder:
                               ("sfo_ppm", "<f4")])       # struct lora_b200_rx_info
 
     def receive(self, iq, n_items=None, stride_items=None, host=None, sync_word=0x12, implicit_len=0, min_preamble=0,
-                max_cfo_hz=0.0, sfo_ppm=0.0, carrier_hz=0.0, soft=False, antennas=1, crc_list=0, wide_cfo=False):
+                max_cfo_hz=0.0, sfo_ppm=0.0, carrier_hz=0.0, soft=False, antennas=1, crc_list=0, wide_cfo=False,
+                fine_toa=False):
         """The dechirp-synchronised receiver (lora_b200_receive): decodes frames below the noise floor.  ``iq`` as for
         work_batch (host ndarray [n_streams, n_items] or a device tensor / pointer).  Returns (consumed, frames, info):
         consumed[s] = where stream s must be re-presented from, frames = FRAME_DTYPE records, info = RX_INFO_DTYPE records
@@ -207,7 +208,9 @@ class decoder:
         (2^K - 1) / 2^16; 0 (the default) is off.
         wide_cfo: receive frames up to max_cfo_hz off carrier (finite, in (0, (fs - bw) / 2]: 3.5 bw at fs/bw = 8, bw / 2 at 2),
         beyond the BW / 4 to which max_cfo_hz is clamped without it.  The screen then searches coarse offsets c * bw / 2,
-        c = -C..C, C = ceil((max_cfo_hz - bw / 4) / (bw / 2)), each costing about one more screen."""
+        c = -C..C, C = ceil((max_cfo_hz - bw / 4) / (bw / 2)), each costing about one more screen.
+        fine_toa: also time each published frame's arrival to a fraction of a sample from its dechirped preamble and SFD
+        windows, read with rx_toa_last() afterwards; nothing published changes."""
         if isinstance(iq, np.ndarray):
             x = np.ascontiguousarray(iq, dtype=np.complex64)
             assert x.ndim == 2 and x.shape[0] == self.n_streams
@@ -221,7 +224,7 @@ class decoder:
                 stride_items = n_items
         p = N.RxParams(sync_word=int(sync_word) & 0xFF, implicit_len=int(implicit_len), min_preamble=int(min_preamble),
                        max_cfo_hz=float(max_cfo_hz), sfo_ppm=float(sfo_ppm), carrier_hz=float(carrier_hz), soft=int(soft),
-                       crc_list=int(crc_list), wide_cfo=int(wide_cfo))
+                       crc_list=int(crc_list), wide_cfo=int(wide_cfo), fine_toa=int(fine_toa))
         m = int(antennas)
         consumed = np.zeros(max(self.n_streams // m, 1) if m > 0 else 1, dtype=np.uint64)
         cptr = consumed.ctypes.data_as(C.POINTER(C.c_size_t))
@@ -236,6 +239,33 @@ class decoder:
                 else np.zeros(0, self.RX_INFO_DTYPE))
         self.header_drops = int(drops.value)
         return consumed.astype(np.int64), self.frames_last(), info
+
+    def rx_toa_last(self) -> np.ndarray:
+        """float64 per frame of the last receive(..., fine_toa=True) call, parallel to its frames (lora_b200_rx_toa_last): the
+        row position, in that call's coordinates like info["start"], at which the frame's first preamble sample arrived, to a
+        fraction of a sample (NaN for a frame without a preamble or SFD window inside the row).  Empty after a call without
+        fine_toa and after work()."""
+        ptr = C.c_void_p(0)
+        n = int(self._L.lora_b200_rx_toa_last(self._h, C.byref(ptr)))
+        if n == 0:
+            return np.zeros(0, np.float64)
+        return np.frombuffer(C.string_at(ptr.value, n * 8), dtype=np.float64).copy()
+
+    def rs_toa(self, iq_dev, n_items, group, start, cfo_bins, sfo_ppm, antennas=1, stride=0):
+        """The fine time of arrival of given frames on its own (lora_b200_rs_toa_dev): frame i at start[i] with cfo_bins[i] and
+        sfo_ppm[i] on receiver group[i] (rows group[i] * M + a, `stride` items apart).  Returns (nu_a, nu_b, toa): the peaks
+        of the preamble and SFD window powers in bins from the CFO, and the time of arrival.  group, start, cfo_bins, sfo_ppm:
+        host sequences of one length."""
+        g = np.ascontiguousarray(group, dtype=np.uint32)
+        s = np.ascontiguousarray(start, dtype=np.int64)
+        f = np.ascontiguousarray(cfo_bins, dtype=np.float32)
+        q = np.ascontiguousarray(sfo_ppm, dtype=np.float32)
+        assert g.shape == s.shape == f.shape == q.shape and g.ndim == 1
+        nu_a, nu_b, toa = np.zeros(g.size, np.float32), np.zeros(g.size, np.float32), np.zeros(g.size, np.float64)
+        N.check(self._L.lora_b200_rs_toa_dev(self._h, _dev_ptr(iq_dev), int(n_items), int(antennas), int(stride or n_items), g.size,
+                                            g.ctypes.data, s.ctypes.data, f.ctypes.data, q.ctypes.data, nu_a.ctypes.data,
+                                            nu_b.ctypes.data, toa.ctypes.data), "lora_b200_rs_toa_dev")
+        return nu_a, nu_b, toa
 
     def rx_channels_last(self) -> np.ndarray:
         """[n_frames, M] complex64: each antenna's channel estimate for every frame of the last receive(..., antennas=M) call,

@@ -268,19 +268,23 @@ def drifted_length(n_samples: int, sfo_ppm: float) -> int:
 
 
 def modulate_frame(fs_syms: FrameSymbols, sf: int, *, bw: float = 125e3, fs: float = 1e6,
-                   n_preamble: int = 8, sync_word: int = 0x12, sfo_ppm: float = 0.0) -> np.ndarray:
+                   n_preamble: int = 8, sync_word: int = 0x12, sfo_ppm: float = 0.0, delay: float = 0.0) -> np.ndarray:
     """preamble | 2 sync symbols | 2.25 downchirps | data symbols (complex128, unit power).
 
     sfo_ppm: the transmitter's clock is off by delta = sfo_ppm * 1e-6 (> 0: fast against the receiver), so receiver sample n
     holds transmitter time u = n (1 + delta) samples; the frame is the base_upchirp phase law evaluated at those fractional
     times (cyclic shifts at fractional positions, the conjugate for the SFD), drifted_length() samples long.  0: exactly the
-    undrifted frame."""
+    undrifted frame.
+    delay >= 0: the frame starts `delay` samples (fractional) into the output: receiver sample n holds transmitter time
+    u = (n - delay) (1 + delta), 0 before the frame; its time of arrival is `delay`.  0 with sfo_ppm = 0: the undrifted frame."""
     up = base_upchirp(sf, bw, fs)
     sps = up.size
     down = np.conj(up)
     n_bins = 1 << sf
     sync = [((sync_word >> 4) & 0xF) * 8 % n_bins, (sync_word & 0xF) * 8 % n_bins]
-    if sfo_ppm == 0:
+    if not delay >= 0.0:
+        raise ValueError(f"delay must be >= 0, got {delay}")
+    if sfo_ppm == 0 and delay == 0:
         parts = [np.tile(up, n_preamble), modulate_shifts(sync, sf, bw, fs), down, down, down[: sps // 4],
                  modulate_shifts(fs_syms.shifts, sf, bw, fs)]
         return np.concatenate(parts)
@@ -289,7 +293,13 @@ def modulate_frame(fs_syms: FrameSymbols, sf: int, *, bw: float = 125e3, fs: flo
     data0 = (n_sfd + 2) * sps + sps // 4
     length = data0 + len(fs_syms.shifts) * sps
     rate = 1.0 + 1e-6 * float(np.float32(sfo_ppm))
-    u = np.arange(drifted_length(length, sfo_ppm), dtype=np.float64) * rate
+    if delay == 0:
+        u = np.arange(drifted_length(length, sfo_ppm), dtype=np.float64) * rate
+    else:
+        u = (np.arange(int(math.ceil(delay)) + drifted_length(length, sfo_ppm), dtype=np.float64) - delay) * rate
+        u = u[u < length]
+    before = u < 0
+    u = np.where(before, 0.0, u)
     q = np.floor(u / sps)
     m = u - q * sps                                      # position in the chirp, before any cyclic shift
     shift = np.zeros(u.size, np.int64)
@@ -306,6 +316,7 @@ def modulate_frame(fs_syms: FrameSymbols, sf: int, *, bw: float = 125e3, fs: flo
     x = np.exp(1j * phase)
     sfd = (q >= n_sfd) & ~data
     x[sfd] = np.conj(x[sfd])
+    x[before] = 0.0
     return x
 
 

@@ -159,6 +159,14 @@ int lora_b200_rs_window_dev(lora_b200_decoder *d, const void *iq, size_t n_items
 int lora_b200_rs_frame_dev(lora_b200_decoder *d, const void *iq, size_t n_items, uint32_t m, size_t stride_items, size_t n,
                            const uint32_t *group, const int64_t *start, const float *cfo_bins, const float *sfo_ppm, uint32_t first,
                            uint32_t cnt, void *chan, float *snr_db, void *windows);
+/* The fine time of arrival of given frames on its own (the procedure of lora_b200_rx_params.fine_toa): frame i (start[i], CFO
+ * cfo_bins[i] in bins, clock offset sfo_ppm[i]) on receiver group[i], rows iq + (group[i] * m + a) * stride_items of n_items
+ * samples, m = 1..4.  nu_a[i] / nu_b[i] = the peaks of the summed preamble / SFD window powers in bins from the CFO, toa[i]
+ * the time of arrival (lora_b200_rx_toa_last).  iq is a device pointer, the rest host arrays; returns when the results are
+ * written.  Test entry point. */
+int lora_b200_rs_toa_dev(lora_b200_decoder *d, const void *iq, size_t n_items, uint32_t m, size_t stride_items, size_t n,
+                         const uint32_t *group, const int64_t *start, const float *cfo_bins, const float *sfo_ppm, float *nu_a,
+                         float *nu_b, double *toa);
 /* The combined screen of the dechirp receiver with several antennas (lora_b200_receive_antennas) on its own, so that it can be
  * held to a reference: n_groups groups of n_antennas (1..4) rows, row r = iq + r * row_stride_items, each holding n_symbols
  * aligned windows of sps samples.  For window i of group g, with tmp_a the kept bins of lora_b200_demod_fft_dev's spectrum of
@@ -340,7 +348,10 @@ size_t lora_b200_frames_crc_last(lora_b200_decoder *d, const uint8_t **status);
  * whose payload CRC fails gets its K least reliable payload / CRC code words (smallest metric gap to the runner-up nibble)
  * tried at their runner-ups, and the cheapest combination (least summed gap) that satisfies the CRC is published, with status
  * LORA_B200_CRC_RECOVERED.  The price: a frame whose errors lie outside the list passes a wrong combination with probability
- * about (2^K - 1) / 2^16, which is why K is capped and the option is off by default.  0 changes nothing. */
+ * about (2^K - 1) / 2^16, which is why K is capped and the option is off by default.  0 changes nothing.
+ * Fine time of arrival (p->fine_toa = 1; other values than 0 and 1: LORA_B200_EINVAL before any launch): each published
+ * frame's arrival to a fraction of a sample, from the dechirped preamble and SFD windows (lora_b200_rx_toa_last).  Reported
+ * only: nothing published changes, and 0 launches nothing more. */
 typedef struct lora_b200_rx_params {
     uint8_t  sync_word;          /* 0 = 0x12                                                    */
     uint8_t  soft;               /* 1: soft-decision decoding (per-bit LLRs, ML code words)      */
@@ -351,7 +362,9 @@ typedef struct lora_b200_rx_params {
     float    max_cfo_hz;         /* 0 = BW / 4; larger values are clamped to BW / 4 (wide_cfo = 0);
                                     with wide_cfo = 1 taken as given, (0, (fs - BW) / 2]          */
     float    sfo_ppm;            /* clock offset of every frame in ppm (> 0: transmitter fast)  */
-    uint32_t reserved1;
+    uint8_t  fine_toa;           /* 1: each published frame's time of arrival to a fraction of a
+                                    sample, lora_b200_rx_toa_last (0 = off)                      */
+    uint8_t  reserved1[3];
     double   carrier_hz;         /* RF carrier of the channel: each frame's clock offset also
                                     follows its CFO, cfo_hz / carrier_hz (0 = not given)        */
 } lora_b200_rx_params;
@@ -368,6 +381,13 @@ int lora_b200_receive(lora_b200_decoder *d, const void *iq, size_t n_items, size
 /* per published frame of the last lora_b200_receive call, parallel to lora_b200_frames_last; *hdr_drops (may be NULL) =
  * synchronised explicit-header frames dropped for a failed header checksum */
 size_t lora_b200_rx_info_last(lora_b200_decoder *d, const lora_b200_rx_info **info, uint32_t *hdr_drops);
+/* Per published frame of the last lora_b200_receive / lora_b200_receive_antennas call with p->fine_toa = 1, parallel to
+ * lora_b200_frames_last: *toa[k] = the row position, in the call's row coordinates like rx_info.start, at which the frame's
+ * first preamble sample (transmitter time 0) arrived, to a fraction of a sample: start + eps, eps from the peaks of the
+ * dechirped preamble windows 1..6 and SFD windows 10, 11 (DESIGN.md section 5).  NaN for a frame without a preamble or
+ * SFD window inside the row.  Returns 0 (no values) after a call without fine_toa and after the work entry points, which
+ * replace lora_b200_frames_last's records. */
+size_t lora_b200_rx_toa_last(lora_b200_decoder *d, const double **toa);
 /* The dechirp receiver on several phase-coherent antennas per receiver (one LO and one sample clock, e.g. both RX channels of
  * a B210): rows g * n_antennas .. g * n_antennas + n_antennas - 1 of iq ([n_streams][n_items], as lora_b200_receive) are
  * the antennas of receiver g.  Timing and CFO are common to a receiver's antennas: the screen takes the argmax of the
