@@ -14,10 +14,14 @@ auto with_sf(int sf, Otherwise otherwise, F f) {
     else return sf == LO ? f(std::integral_constant<int, LO>{}) : with_sf<LO + 1, HI>(sf, otherwise, f);
 }
 
-// f(D) for the K1 oversampling osr = sps / N: 8 or 2
+// f(D) for the K1 oversampling osr = sps / N: 8, 2, 16 or 32 (fs/bw = 4 has no kernels)
 template <class Otherwise, class F>
 auto with_osr(int osr, Otherwise otherwise, F f) {
-    return osr == 8 ? f(std::integral_constant<int, 8>{}) : osr == 2 ? f(std::integral_constant<int, 2>{}) : otherwise();
+    return osr == 8    ? f(std::integral_constant<int, 8>{})
+           : osr == 2  ? f(std::integral_constant<int, 2>{})
+           : osr == 16 ? f(std::integral_constant<int, 16>{})
+           : osr == 32 ? f(std::integral_constant<int, 32>{})
+                       : otherwise();
 }
 
 // f(B) for a bool
@@ -26,7 +30,7 @@ auto with_bool(bool b, F f) {
     return b ? f(std::true_type{}) : f(std::false_type{});
 }
 
-// f(SF, D) over the K1 configurations: sf in 7..12 and osr 8 or 2
+// f(SF, D) over the K1 configurations: sf in 7..12 and osr 8, 2, 16 or 32
 template <class Otherwise, class F>
 auto with_sf_osr(int sf, int osr, Otherwise otherwise, F f) {
     return with_osr(osr, otherwise, [&](auto D) { return with_sf<7, 12>(sf, otherwise, [&](auto SF) { return f(SF, D); }); });

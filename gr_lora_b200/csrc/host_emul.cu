@@ -22,7 +22,7 @@
 
 extern "C" {
 
-// k1_fft_kernel<SF, D> on the host, D = osr = sps / N (8 or 2); -1 for another SF or D
+// k1_fft_kernel<SF, D> on the host, D = osr = sps / N (8, 2, 16 or 32); -1 for another SF or D
 int lb_k1_emulate_osr(int sf, int osr, const float2 *x, size_t n_symbols, const float2 *chirp, const float2 *tw, uint32_t *bins,
                       float *mags) {
     const lb::K1Args a{x, chirp, tw, n_symbols};
@@ -341,6 +341,11 @@ int rs_host_crc_list(const lb::RxParams &rp, uint8_t phdr1, uint32_t implicit_le
     return 1;
 }
 
+// the rates the receiver runs at: those of the K1 kernels
+bool rs_host_osr(uint32_t osr) {
+    return lb::with_osr((int)osr, [] { return false; }, [](auto) { return true; });
+}
+
 // the receive path of lb_emul_rx_receive_osr (m = 1) and lb_emul_rx_receive_antennas (m rows of n_items each, x[a * n_items
 // ..]); with several antennas chan[f * m ..] gets each synchronised frame's channel estimates h (may be NULL).  max_cfo_bins
 // > 0: the coarse-offset search of rx_params.wide_cfo up to that CFO; else |CFO| <= N / 4 without it.
@@ -349,13 +354,13 @@ uint32_t rs_host_receive(const float2 *x, size_t n_items, uint32_t m, const floa
                          uint32_t min_preamble, float sfo_ppm, double carrier_hz, int soft, long long *start, float *cfo_bins,
                          float *snr_db, int32_t *status, float *sfo, uint8_t *payload, uint32_t *len, float2 *chan, uint32_t cap,
                          uint32_t crc_list = 0, uint8_t *crc_status = nullptr, float max_cfo_bins = 0.f, double *toa = nullptr) {
-    if (osr != 8u && osr != 2u) return 0;
+    if (!rs_host_osr(osr)) return 0;
     const uint32_t N = 1u << sf, sps = osr * N;
     const double bin_hz = 125e3 / N;
     lb::RsParams p{sps, N, osr, sfo_ppm, min_preamble ? min_preamble : 5u, {((sync_word >> 4) & 15u) * 8u % N, (sync_word & 15u) * 8u % N},
                    max_cfo_bins > 0.f ? max_cfo_bins : (float)N / 4.0f, carrier_hz > 0.0 ? (float)(1e6 * bin_hz / carrier_hz) : 0.0f, 0};
     p.hyp = lb::rs_hypotheses(p.max_cfo_bins, N);
-    if (p.hyp > lb::RS_MAX_HYP) return 0;
+    if (p.hyp > lb::rs_max_hyp((int)osr)) return 0;
     std::vector<float2> shift((size_t)(2 * p.hyp + 1) * 2 * sps);
     lb::rs_shift_tables(down, up, sps, osr, p.hyp, shift.data());
     RsHostOps o{x, (long long)n_items, down, up, tw, sps, sf, osr, shift.data(), p.hyp};
@@ -380,7 +385,7 @@ uint32_t rs_host_receive(const float2 *x, size_t n_items, uint32_t m, const floa
     }
     std::vector<lb::RsCand> cands(64);
     long long dropped;
-    const uint32_t nc = std::min<uint32_t>(lb::rs_detect_stream<lb::RS_MAX_SCREENS>(bp.data(), mp.data(), n, p, cands.data(), 64, &dropped), 64u);
+    const uint32_t nc = std::min<uint32_t>(lb::rs_detect_stream<lb::rs_max_screens(32)>(bp.data(), mp.data(), n, p, cands.data(), 64, &dropped), 64u);
     lb::RxParams rp;
     memset(&rp, 0, sizeof rp);
     rp.sf = sf; rp.n_bins = N; rp.n_bins_hdr = N / 4; rp.sps = sps; rp.decim = osr; rp.implicit = implicit; rp.reduced_rate = reduced_rate;
@@ -463,7 +468,7 @@ uint32_t rs_host_receive(const float2 *x, size_t n_items, uint32_t m, const floa
 extern "C" {
 
 // The whole dechirp-synchronised receive path (rx_sync.cuh) of one row on the host (BW = 125 kHz, fs = osr x BW with
-// osr = 8 or 2, the decoder's sps / N; other values return 0 frames): screen,
+// osr = 8, 2, 16 or 32, the decoder's sps / N; other values return 0 frames): screen,
 // detect, synchronise, header and payload rounds, integer chain.  sfo_ppm and carrier_hz as in lora_b200_rx_params.  Per
 // synchronised frame f (at most cap): start[f], cfo_bins[f], snr_db[f], status[f] (0 published, 1 header checksum failed,
 // 2 incomplete), the clock offset its windows were placed with sfo[f] (may be NULL) and, when published, its payload in
@@ -553,7 +558,7 @@ uint32_t lb_emul_rx_receive_toa(const float2 *x, size_t n_items, uint32_t m, con
 int lb_emul_rs_toa(const float2 *x, size_t n_items, uint32_t m, const float2 *down, const float2 *up, const float2 *tw, uint32_t sf,
                    uint32_t osr, size_t n, const long long *start, const float *cfo_bins, const float *sfo_ppm, float *nu_a, float *nu_b,
                    double *toa) {
-    if ((osr != 8u && osr != 2u) || m < 1 || m > (uint32_t)lb::RS_MAX_ANTENNAS) return -1;
+    if (!rs_host_osr(osr) || m < 1 || m > (uint32_t)lb::RS_MAX_ANTENNAS) return -1;
     const uint32_t N = 1u << sf, sps = osr * N;
     lb::RsParams p{sps, N, osr, 0.f, 5u, {0u, 0u}, (float)N / 4.0f, 0.f, 0};
     RsHostOps o{x, (long long)n_items, down, up, tw, sps, sf, osr, nullptr, 0};
@@ -632,4 +637,56 @@ void lb_emul_buffer_reserve(const size_t *bytes, size_t n, int *rc, void **ptr, 
     for (size_t i = 0; i < n; i++) { rc[i] = (int)b.reserve(bytes[i]); ptr[i] = b.get(); cap[i] = b.capacity(); }
 }
 
+}
+
+namespace {
+// The shared-memory indices (float2 units) of k1_fft_kernel<SF, D>'s phases over one batch, as k1_pass0, k1_pass and
+// k1_combine form them from the thread index: instruction after instruction, the index of each of the K1_THREADS threads
+// (-1: idle), and the phase (0 pass-0 stores, 1 and 2 the k1_pass loads -- its stores touch the same indices --, 3 the
+// combine loads).
+template <int SF, int D>
+void k1_smem_indices(std::vector<int32_t> &idx, std::vector<int32_t> &phase) {
+    using C = lb::K1Cfg<SF, D>;
+    constexpr int T = lb::K1_THREADS, HB_LOG = lb::k1_log2(C::HB);
+    auto instr = [&](int ph, auto at) {
+        for (int t = 0; t < T; t++) idx.push_back(at(t));
+        phase.push_back(ph);
+    };
+    for (int kc = 0; kc < 16; kc++)                   // thread (g, m, b): row kc of branches 2b, 2b + 1 of column m
+        for (int br = 0; br < 2; br++)
+            instr(0, [&](int tid) {
+                const int g = tid / (C::HB * C::M0), rem = tid % (C::HB * C::M0), m = rem >> HB_LOG, b = rem & (C::HB - 1);
+                return g * C::SYM_STRIDE + (2 * b + br) * C::SB + lb::k1_pad(kc * C::M0 + m);
+            });
+    auto pass = [&](int ph, int R, int SIG) {
+        const int per = C::NP / R, items = C::G * D * per;
+        for (int it0 = 0; it0 < items; it0 += T)
+            for (int c = 0; c < R; c++)
+                instr(ph, [&](int tid) {
+                    const int it = it0 + tid;
+                    if (it >= items) return -1;
+                    const int j = it % per, gr = it / per, lo = j % SIG;
+                    return gr * C::SB + lb::k1_pad((j / SIG) * (R * SIG) + lo + SIG * c);
+                });
+    };
+    pass(1, C::R1, C::SIG1);
+    if (C::R2 > 1) pass(2, C::R2, 1);
+    for (int i = 0; i < C::NP / C::TPS; i++)
+        for (int r = 0; r < D; r++)
+            instr(3, [&](int tid) { return (tid / C::TPS) * C::SYM_STRIDE + r * C::SB + lb::k1_pad(tid % C::TPS + C::TPS * i); });
+}
+}  // namespace
+
+extern "C" {
+// k1_smem_indices of k1_fft_kernel<sf, osr>: returns the number of indices n (a multiple of K1_THREADS; -1 for another SF or
+// osr) and, when cap >= n, writes them to idx[n] and the phase of each instruction to phase[n / K1_THREADS]
+long lb_k1_smem_replay(int sf, int osr, int32_t *idx, int32_t *phase, long cap) {
+    std::vector<int32_t> v, ph;
+    if (lb::with_sf_osr(sf, osr, [] { return -1; }, [&](auto SF, auto D) { k1_smem_indices<SF, D>(v, ph); return 0; })) return -1;
+    if (idx && phase && cap >= (long)v.size()) {
+        std::copy(v.begin(), v.end(), idx);
+        std::copy(ph.begin(), ph.end(), phase);
+    }
+    return (long)v.size();
+}
 }

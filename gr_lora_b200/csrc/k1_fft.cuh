@@ -9,18 +9,19 @@
 // without ever forming the 7N unused bins:  with n = 8*n1 + r (sps = 8N at fs/bw = 8)
 //     F[k'] = sum_r W_sps^{k' r} G_r[k' mod N],   G_r = N-point DFT over n1 of m[8 n1 + r]
 // i.e. 8 N-point FFTs (one per polyphase branch) and one 8-term twiddled sum per kept bin.  The phase functions take the
-// oversampling factor D = sps / N as a template argument (default 8); at fs/bw = 2 the same sum has D = 2 branches
-// (n = 2 n1 + r) and the split below starts at SF12 (sub-problems of up to 2048 bins).
-// For SF11/12 (N > 1024) a radix-S decimation-in-frequency step (S = 2, 4) is folded into
+// oversampling factor D = sps / N as a template argument (default 8); at fs/bw = 2, 16 and 32 the same sum has D branches
+// (n = D n1 + r) and the split below starts at SF12 (D = 2: sub-problems of up to 2048 bins), SF10 (D = 16: 512) or SF9
+// (D = 32: 256).  fs/bw = 4 has no kernels.
+// For N > NP_MAX (SF11/12 at D = 8) a radix-S decimation-in-frequency step (S = 2 .. 16) is folded into
 // the load:  F[S q + s] = DFT_{sps/S}( y_s )[q],  y_s[n] = W_sps^{s n} sum_j W_S^{s j} m[n + j sps/S],
-// giving S independent sub-problems of N' = N/S = 1024 bins whose partial argmaxes are
+// giving S independent sub-problems of N' = N/S = NP_MAX bins whose partial argmaxes are
 // merged with a 64-bit atomicMax.
 //
-// Data flow per CTA (256 threads) and batch of G = 1024/N' symbols:
+// Data flow per CTA (256 threads) and batch of G = 8192/(D N') symbols:
 //   pass 0  coalesced float4 loads straight into registers (each thread: 16 rows x 2 branches),
 //           dechirp, radix-16 DIF in registers, inter-pass twiddle, store to shared memory
 //   pass i  in-place radix-8/16/4 passes in shared memory (padded, conflict-free layout)
-//   combine Horner evaluation of the 8-branch twiddled sum, |.|^2, argmax
+//   combine Horner evaluation of the D-branch twiddled sum, |.|^2, argmax
 // The phase functions are __host__ __device__ so tests/test_k1_emulation.py can run the
 // very same index arithmetic on the CPU.
 #pragma once
@@ -32,23 +33,28 @@ constexpr int K1_THREADS = 256;
 
 LB_HD constexpr int k1_log2(int v) { return v > 1 ? 1 + k1_log2(v >> 1) : 0; }
 
-// D = sps / N, the oversampling factor: D polyphase branches (8 at fs/bw = 8, 2 at fs/bw = 2).  Every CTA batch holds
-// G * D * NP = 8192 samples whatever D is, so a symbol's share of the threads and of shared memory scales with D * NP.
+// D = sps / N, the oversampling factor: D polyphase branches (8 at fs/bw = 8; 2, 16 and 32 at those rates).  Every CTA
+// batch holds G * D * NP = 8192 samples whatever D is, so a symbol's share of the threads and of shared memory scales with
+// D * NP, and a symbol is split into sub-problems of NP_MAX = min(2048, 8192 / D) bins.
 template <int SF, int D = 8>
 struct K1Cfg {
     static constexpr int N = 1 << SF;                 // bins
     static constexpr int SPS = D * N;                 // samples per symbol
-    static constexpr int NP_MAX = D == 8 ? 1024 : 2048;   // the passes below cover sub-problems of up to 2048 bins
+    static constexpr int NP_MAX = 8192 / D < 2048 ? 8192 / D : 2048;   // the passes below cover sub-problems of up to 2048 bins
     static constexpr int S = N <= NP_MAX ? 1 : N / NP_MAX;   // DIF split factor
-    static constexpr int NP = N / S;                  // bins per sub-problem (128..1024 at D = 8, 128..2048 at D = 2)
+    static constexpr int NP = N / S;                  // bins per sub-problem (128..1024 at D = 8, ..2048 at 2, ..512 at 16, ..256 at 32)
     static constexpr int SPS_SUB = D * NP;
     static constexpr int HB = D / 2;                  // float4 loads (2 adjacent branches each) per row in pass 0
     static constexpr int G = 8192 / (D * NP);         // symbols per CTA batch
     static constexpr int M0 = NP / 16;                // columns after the radix-16 pass 0
     static constexpr int SB0 = NP + NP / 16;
-    // branch stride, == 2 (mod 16) at D = 8; == 4 (mod 16) at D = 2, where a half-warp can span two symbols (M0 = 8) and
-    // their strides must then fall 8 float2 apart
-    static constexpr int SB = SB0 + (((D == 8 ? 2 : 4) - SB0 % 16) + 16) % 16;
+    // branch stride: == 2 (mod 16) at D = 8; == 4 (mod 16) at D = 2, where a half-warp can span two symbols (M0 = 8) and
+    // their strides must then fall 8 float2 apart; == 1 (mod 8) at D = 16 and 32, where a pass-0 half-warp stores 8 branch
+    // pairs x 2 columns (D = 16: distinct banks) or 16 branch pairs of one column (D = 32: offsets 2 b SB, all of one parity,
+    // so 2-way whatever SB is).  tests/test_rx_osr_high_host.py replays every phase's shared-memory indices.
+    static constexpr int SB_MOD = D == 8 ? 2 : D == 2 ? 4 : 1;
+    static constexpr int SB_M = D == 8 || D == 2 ? 16 : 8;
+    static constexpr int SB = SB0 + ((SB_MOD - SB0 % SB_M) + SB_M) % SB_M;
     static constexpr int SYM_STRIDE = D * SB;
     static constexpr int SMEM_ELEMS = G * SYM_STRIDE; // float2 elements
     static constexpr int TPS = K1_THREADS / G;        // threads per symbol in the combine phase
@@ -58,8 +64,16 @@ struct K1Cfg {
     static constexpr int SIG1 = M0 / R1;              // 1, 1, 4, 8 (16 for NP = 2048)
     static constexpr int R2 = SIG1;                   // 1 (none), 1, 4, 8 (16)
     static_assert(SF >= 7 && SF <= 12, "K1 supports SF7..SF12");
-    static_assert(D == 8 || D == 2, "K1 runs at fs/bw = 8 or 2");
+    static_assert(D == 2 || D == 8 || D == 16 || D == 32, "K1 runs at fs/bw = 2, 8, 16 or 32");
     static_assert(G * TPS == K1_THREADS && G * M0 * HB == K1_THREADS, "one thread per pass-0 column pair and combine slot");
+    // the D = 2 and D = 8 configurations as they were before D = 16 and 32 were added (their kernels must not change)
+    static_assert(D != 8 || (NP == (N < 1024 ? N : 1024) && S == N / NP && G == 1024 / NP && SB % 16 == 2 && TPS == 256 / G &&
+                             W == (TPS < 32 ? TPS : 32)), "fs/bw = 8 layout");
+    static_assert(D != 2 || (NP == (N < 2048 ? N : 2048) && S == N / NP && G == 4096 / NP && SB % 16 == 4 && TPS == 256 / G &&
+                             W == (TPS < 32 ? TPS : 32)), "fs/bw = 2 layout");
+    static_assert((D != 8 && D != 2) || (SB >= SB0 && SB < SB0 + 16), "fs/bw = 8 and 2: the least such branch stride");
+    static_assert(D != 16 || (NP == (N < 512 ? N : 512) && S == N / NP && G == 512 / NP && SB == SB0 + 1), "fs/bw = 16 layout");
+    static_assert(D != 32 || (NP == (N < 256 ? N : 256) && S == N / NP && G == 256 / NP && SB == SB0 + 1), "fs/bw = 32 layout");
 };
 
 LB_HD int k1_pad(int i) { return i + (i >> 4); }

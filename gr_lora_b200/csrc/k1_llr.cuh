@@ -9,9 +9,9 @@
 // maximum-likelihood decision over these LLRs needs no SNR scale.
 //
 // The phases are K1's own (k1_pass0, k1_pass, k1_combine_twiddles, the horner<D> / plus_quirk sum per kept bin, D = sps / N
-// = 8 or 2), so the
+// = 2, 8, 16 or 32), so the
 // argmax key -- and the bin reported beside the LLRs -- is k1_fft_kernel's bit for bit.  The epilogue keeps 2 SF running
-// maxima of |X|^2 per thread and takes square roots only at the end.  At SF11/SF12 a CTA loops over the S sub-problems
+// maxima of |X|^2 per thread and takes square roots only at the end.  Where K1Cfg splits a symbol (S > 1) a CTA loops over the S sub-problems
 // of its symbol (as RsDevOps::argmax does): each warp's maxima are kept in shared memory between them, and no merge pass
 // over global memory follows.
 #pragma once

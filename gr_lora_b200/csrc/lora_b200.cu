@@ -83,8 +83,8 @@ struct lora_b200_decoder : A1Params {
     // derived, decoder_impl.cc:69-91 (A1Params and these)
     uint32_t n_bins_hdr, decim;
     double bits_per_second, bits_per_symbol;
-    int k1_osr;                           // the K1 kernels' D = fs/bw with SF7..12: 8 (every K1 kernel), 2 (the generic K1 and
-                                          // LLR kernels), or 0 (none)
+    int k1_osr;                           // the K1 kernels' D = fs/bw with SF7..12: 8 (every K1 kernel), 2, 16 or 32 (the
+                                          // generic K1 and LLR kernels), or 0 (none)
     int device, n_sms;
     Tables toff;
     DeviceBuffer<uint8_t> d_tables;
@@ -238,7 +238,7 @@ int launched(lora_b200_decoder *d) { d->launches++; CU(cudaGetLastError()); retu
 // LORA_B200_OK when the K1 kernels serve this decoder's configuration, else the error that `what` needs them
 int need_k1(const lora_b200_decoder *d, const char *what) {
     if (d->k1_osr) return LORA_B200_OK;
-    return fail(LORA_B200_EUNSUPPORTED, "%s needs samp_rate/bandwidth == 8 or 2 and SF7..SF12", what);
+    return fail(LORA_B200_EUNSUPPORTED, "%s needs samp_rate/bandwidth == 8, 2, 16 or 32 and SF7..SF12", what);
 }
 
 // the `otherwise` of a dispatch on the decoder's SF
@@ -297,11 +297,18 @@ K1Launcher k1_launcher(int sf) {
     return nullptr;
 }
 
-// the generic kernel k1_fft_kernel<SF, D>: every SF at fs/bw = 2 (where it splits a symbol at SF12 only), and at fs/bw = 8
-// when `generic` is set
+// the generic kernel k1_fft_kernel<SF, D>: every SF at fs/bw = 2, 16 and 32 (where it splits a symbol from SF12, SF10 and SF9
+// on), and at fs/bw = 8 when `generic` is set
 K1Launcher k1_launcher_generic(int sf, int osr) {
     static_assert(K1Cfg<11, 2>::S == 1 && K1Cfg<12, 2>::S == 2, "k1_fft_kernel<SF, 2> splits SF12 only");
+    static_assert(K1Cfg<9, 16>::S == 1 && K1Cfg<10, 16>::S == 2 && K1Cfg<12, 16>::S == 8, "k1_fft_kernel<SF, 16> splits SF10..12");
+    static_assert(K1Cfg<8, 32>::S == 1 && K1Cfg<9, 32>::S == 2 && K1Cfg<12, 32>::S == 16, "k1_fft_kernel<SF, 32> splits SF9..12");
     return with_sf_osr(sf, osr, [] { return K1Launcher(); }, [](auto SF, auto D) -> K1Launcher { return k1_launch_generic<SF, D>; });
+}
+
+// whether k1_fft_kernel<sf, osr> splits a symbol into sub-problems (K1Cfg::S > 1)
+bool k1_generic_splits(int sf, int osr) {
+    return with_sf_osr(sf, osr, [] { return false; }, [](auto SF, auto D) { return K1Cfg<SF, D>::S > 1; });
 }
 
 int dispatch_k1_impl(lora_b200_decoder *d, K1Scratch &ks, const float2 *iq, size_t n, uint32_t *bins, float *mags, cudaStream_t st,
@@ -311,11 +318,12 @@ int dispatch_k1_impl(lora_b200_decoder *d, K1Scratch &ks, const float2 *iq, size
     static const char *rows = getenv("LORA_B200_K1_ROWS");
     const int sf = (int)d->cfg.sf;
     const bool generic = k1_generic() || (sf >= 11 && rows && rows[0] == '0');
-    const K1Launcher launch = d->k1_osr == 8 && !generic ? k1_launcher(sf) : k1_launcher_generic(sf, d->k1_osr);
+    const bool tuned = d->k1_osr == 8 && !generic;
+    const K1Launcher launch = tuned ? k1_launcher(sf) : k1_launcher_generic(sf, d->k1_osr);
     if (!launch) return fail(LORA_B200_EUNSUPPORTED, "unsupported SF %u", d->cfg.sf);
-    // the kernels that split a symbol (every SF12 kernel, the generic one at SF11 at fs/bw = 8) merge partial argmax keys in
-    // ks.packed
-    const bool split = sf == 12 || (sf == 11 && generic && d->k1_osr == 8);
+    // the kernels that split a symbol merge partial argmax keys in ks.packed: of the fs/bw = 8 kernels the SF12 one (a cluster
+    // of two CTAs per symbol), of the generic ones those whose K1Cfg has S > 1
+    const bool split = tuned ? sf == 12 : k1_generic_splits(sf, d->k1_osr);
     if (split) {
         CU(ks.packed.reserve(n));
         CU(cudaMemsetAsync(ks.packed, 0, sizeof(unsigned long long) * n, st));
@@ -598,7 +606,10 @@ lora_b200_decoder *lora_b200_create(const lora_b200_config *cfg) {
         fail(LORA_B200_EINVAL, "samp_rate %.1f too low for bandwidth %u", cfg->samp_rate, cfg->bandwidth);
         return nullptr;
     }
-    d->k1_osr = (d->sps == 8u * d->n_bins || d->sps == 2u * d->n_bins) && cfg->sf >= 7 && cfg->sf <= 12 ? (int)d->decim : 0;
+    d->k1_osr = d->sps % d->n_bins == 0 && with_osr((int)d->decim, [] { return false; }, [](auto) { return true; }) && cfg->sf >= 7 &&
+                        cfg->sf <= 12
+                    ? (int)d->decim
+                    : 0;
     if (cfg->demod == LORA_B200_DEMOD_FFT && d->k1_osr != 8) {
         fail(LORA_B200_EUNSUPPORTED, "FFT demodulator needs samp_rate/bandwidth == 8 and SF7..SF12");
         return nullptr;
@@ -1104,7 +1115,7 @@ static int rs_launch_sync(lora_b200_decoder *d, const float2 *x, size_t stride, 
 }
 
 // without a clock offset the synchroniser runs its DRIFT = false instantiation, which does no drift arithmetic; D = sps / N
-// (8 or 2) selects the K1 phase functions of its argmax windows; shift: the hypotheses' tables (NULL when rp.hyp = 0)
+// (8, 2, 16 or 32) selects the K1 phase functions of its argmax windows; shift: the hypotheses' tables (NULL when rp.hyp = 0)
 static int rs_sync(lora_b200_decoder *d, const float2 *x, size_t stride, size_t n_items, const RsParams &rp, uint32_t cap, uint32_t m,
                    const float2 *shift) {
     return with_sf_osr(d->cfg.sf, d->k1_osr, unsupported_sf(d), [&](auto SF, auto D) {
@@ -1282,14 +1293,17 @@ static int rs_receive(lora_b200_decoder *d, const void *iq, size_t n_items, size
     CU(d->d_rs_nframes.reserve(1));
     CU(cudaMemsetAsync(d->d_rs_hold, 0xFF, sizeof(unsigned long long) * ns, st));
     CU(cudaMemsetAsync(d->d_rs_nframes, 0, sizeof(uint32_t), st));
-    if (rp.hyp == 0)
-        rs_detect_kernel<2><<<(ns + 127) / 128, 128, 0, st>>>(d->d_rs_bins[0], d->d_rs_mags[0], d->d_rs_bins[1], d->d_rs_mags[1], hs, stride,
-                                                              n_items, ns, rp, d->d_rs_cands, cap, d->d_rs_ncand, d->d_rs_dropped);
-    else
-        rs_detect_kernel<RS_MAX_SCREENS><<<(ns + 127) / 128, 128, 0, st>>>(d->d_rs_bins[0], d->d_rs_mags[0], d->d_rs_bins[1], d->d_rs_mags[1],
-                                                                           hs, stride, n_items, ns, rp, d->d_rs_cands, cap, d->d_rs_ncand,
-                                                                           d->d_rs_dropped);
-    if (int rc = launched(d)) return rc;
+    // the screens bound of the detector: 2 (the one hypothesis c = 0), else that of the decoder's rate (rs_max_screens)
+    auto detect = [&](auto S_MAX) {
+        rs_detect_kernel<S_MAX><<<(ns + 127) / 128, 128, 0, st>>>(d->d_rs_bins[0], d->d_rs_mags[0], d->d_rs_bins[1], d->d_rs_mags[1], hs,
+                                                                  stride, n_items, ns, rp, d->d_rs_cands, cap, d->d_rs_ncand, d->d_rs_dropped);
+        return launched(d);
+    };
+    const int rc_detect = rp.hyp == 0          ? detect(std::integral_constant<int, 2>{})
+                          : rp.hyp <= RS_MAX_HYP ? detect(std::integral_constant<int, RS_MAX_SCREENS>{})
+                          : rp.hyp <= rs_max_hyp(16) ? detect(std::integral_constant<int, rs_max_screens(16)>{})
+                                                     : detect(std::integral_constant<int, rs_max_screens(32)>{});
+    if (rc_detect) return rc_detect;
     if (int rc = rs_sync(d, x, stride, n_items, rp, cap, m, shift)) return rc;
     uint32_t n_sync = 0;
     std::vector<long long> dropped(ns);

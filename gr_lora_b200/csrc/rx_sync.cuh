@@ -43,16 +43,22 @@ struct RsParams {
     int32_t hyp;                       // C: coarse-offset hypotheses c = -C..C (rs_hypotheses; 0: the one screen of c = 0)
 };
 
-// coarse-offset hypotheses: the largest |c| the screen needs so that every |F| <= max_cfo_bins lies within N/4 of some c N/2
-constexpr int RS_MAX_HYP = 7;          // (fs - BW) / 2 at fs / bw = 8: 3.5 N bins
-constexpr int RS_MAX_SCREENS = 2 * (2 * RS_MAX_HYP + 1);
+// coarse-offset hypotheses: the largest |c| the screen needs so that every |F| <= max_cfo_bins lies within N/4 of some c N/2.
+// At fs / bw = D the sampled band, |F| <= (D - 1) N / 2, needs C <= D - 1 (7 at 8, 15 at 16, 31 at 32; 1 at 2), that is
+// 2 (2 C + 1) screens: 30, 62, 126.
+constexpr int rs_max_hyp(int D) { return D - 1; }
+constexpr int rs_max_screens(int D) { return 2 * (2 * rs_max_hyp(D) + 1); }
+constexpr int RS_MAX_HYP = rs_max_hyp(8);          // (fs - BW) / 2 at fs / bw = 8: 3.5 N bins
+constexpr int RS_MAX_SCREENS = rs_max_screens(8);
 inline int rs_hypotheses(float max_cfo_bins, uint32_t N) {
     const double c = std::ceil(((double)max_cfo_bins - 0.25 * N) / (0.5 * N));
     return c > 0.0 ? (int)c : 0;
 }
 
 // the shifted dechirp tables of hypotheses c = -C..C, out[((c + C) * 2 + up) * sps + n] = table[n] e^{-j pi c n / D}, table the
-// down- (up = 0) or up-chirp (up = 1); the phase is reduced exactly, (c n) mod 2D, and the product is formed in double
+// down- (up = 0) or up-chirp (up = 1); the phase is reduced exactly, (c n) mod 2D, and the product is formed in double.
+// (2 C + 1) 2 sps float2 in all, on the host and on the device: 7.9 MB at SF12, fs/bw = 8, C = 7, and 132 MB at SF12,
+// fs/bw = 32, C = 31 (the whole band of a 4 MS/s capture at 125 kHz)
 inline void rs_shift_tables(const float2 *down, const float2 *up, uint32_t sps, uint32_t D, int C, float2 *out) {
     for (int c = -C; c <= C; c++)
         for (int u = 0; u < 2; u++) {
@@ -708,7 +714,7 @@ LB_HD uint32_t rs_crc_block_bin(const RsCrcFrame &f, const uint8_t *nib, uint32_
 // ---- kernels ---------------------------------------------------------------------------------------------------------------
 // detect: one thread per stream.  The screen's windows of row s are the K1 results starting at s * stride / sps (stride a
 // multiple of sps) in each phase array, those of hypothesis c at (c + hyp) * hyp_stride further.  S_MAX bounds the screens
-// (2 without wide_cfo, RS_MAX_SCREENS with it).
+// (2 without wide_cfo, with it rs_max_screens(D) of the rate: RS_MAX_SCREENS up to fs/bw = 8, 62 at 16, 126 at 32).
 template <int S_MAX>
 __global__ void rs_detect_kernel(const uint32_t *__restrict__ bins0, const float *__restrict__ mags0, const uint32_t *__restrict__ bins1,
                                  const float *__restrict__ mags1, size_t hyp_stride, size_t stride, size_t n_items, uint32_t n_streams,

@@ -206,7 +206,8 @@ class decoder:
         runner-up nibbles, and the cheapest combination that satisfies the CRC is published (frames_crc_last() reports it
         RECOVERED).  A frame whose errors lie outside the list passes a wrong combination with probability about
         (2^K - 1) / 2^16; 0 (the default) is off.
-        wide_cfo: receive frames up to max_cfo_hz off carrier (finite, in (0, (fs - bw) / 2]: 3.5 bw at fs/bw = 8, bw / 2 at 2),
+        wide_cfo: receive frames up to max_cfo_hz off carrier (finite, in (0, (fs - bw) / 2]: 3.5 bw at fs/bw = 8, bw / 2 at 2,
+        7.5 bw at 16, 15.5 bw at 32),
         beyond the BW / 4 to which max_cfo_hz is clamped without it.  The screen then searches coarse offsets c * bw / 2,
         c = -C..C, C = ceil((max_cfo_hz - bw / 4) / (bw / 2)), each costing about one more screen.
         fine_toa: also time each published frame's arrival to a fraction of a sample from its dechirped preamble and SFD

@@ -131,7 +131,7 @@ int lora_b200_demod_fft_host(lora_b200_decoder *d, const void *iq, size_t n_symb
  * (> 0: bit 0), j < ppm.  The demodulated word of bin k is the receiver's: gray((k - 1) mod N), with (k - 1) mod N first
  * folded to N / 4 bins as reduced-rate symbols are (reduced = 1, ppm = SF - 2; reduced = 0: ppm = SF).  bins (may be NULL)
  * = lora_b200_demod_fft_dev's argmax of the same computation.  iq 16-byte aligned; device pointers, async on cuda_stream.
- * LORA_B200_EUNSUPPORTED unless samp_rate / bandwidth is 8 or 2 and SF7..SF12. */
+ * LORA_B200_EUNSUPPORTED unless samp_rate / bandwidth is 8, 2, 16 or 32 and SF7..SF12 (4 is refused). */
 int lora_b200_demod_llr_dev(lora_b200_decoder *d, const void *iq, size_t n_symbols, int reduced, float *llrs, uint32_t *bins,
                             void *cuda_stream);
 /* The window sums the dechirp receiver's synchroniser (lora_b200_receive, lora_b200_receive_antennas) measures, on their own,
@@ -314,7 +314,7 @@ size_t lora_b200_frames_crc_last(lora_b200_decoder *d, const uint8_t **status);
  * checked.  Data windows are de-rotated by the frame's CFO and demodulated by the K1 batch kernels; the FFT demodulator's
  * (bin - 1) mod N mapping and the stream path's integer chain follow.  Explicit headers whose 5-bit checksum fails are dropped
  * (and counted); frames whose payload CRC fails are published too (lora_b200_frames_crc_last reports it).  Implicit headers carry implicit_len payload bytes (0 with an implicit-header
- * decoder: LORA_B200_EINVAL).  Needs the FFT kernels (samp_rate / bandwidth == 8 or 2, SF7..SF12), else LORA_B200_EUNSUPPORTED;
+ * decoder: LORA_B200_EINVAL).  Needs the FFT kernels (samp_rate / bandwidth == 8, 2, 16 or 32, SF7..SF12), else LORA_B200_EUNSUPPORTED;
  * at 2 (e.g. 500 kHz channels at 1 MS/s, or a channelizer's output at 2 samples per chip) timing is refined to +-1 sample.
  * Clock offset: a transmitter whose clock is off by delta = ppm * 1e-6 (delta > 0: fast against the receiver) sends TX symbol
  * position j (0..7 preamble, 8, 9 sync word, 10..12.25 SFD, 12.25 + k data symbol k) at receiver sample

@@ -14,11 +14,13 @@ points gain two SNRs 1.5 and 3 dB below its lowest, and the stages gain the soft
 part of assemble + K1).
 With --osr 2 the sensitivity curve is measured at fs/bw = 2 (250 kS/s, the generic K1 and LLR kernels at D = 2), and the
 real-time shape is decoded at fs/bw = 8 and at fs/bw = 2 (the same payloads, CFOs and layout, synthesised at each rate),
-alternating call by call; its results carry the suffix _osr8 / _osr2.
+alternating call by call; its results carry the suffix _osr8 / _osr2.  --osr 16 and --osr 32 do the same at 2 MS/s and 4 MS/s
+(the real-time shape has 192 streams at fs/bw = 32: about 12 GB of cf32 either way), and --all-rates times the shape at
+fs/bw = 2, 8, 16 and 32 in one run.
 With --cfo-range LO HI every frame's CFO is uniform in +-[LO, HI] BW (a random sign), and every capture is decoded with the
 coarse-offset search (lora_b200_rx_params.wide_cfo, max_cfo_hz = --max-cfo, default HI, in BW) and without it, alternating;
 results carry the suffix _wide / _off.
-Usage: python tools/bench_rx_sync.py [--quick] [--ppm P | --soft | --cfo-range LO HI [--max-cfo M]] [--osr 2]"""
+Usage: python tools/bench_rx_sync.py [--quick] [--ppm P | --soft | --cfo-range LO HI [--max-cfo M]] [--osr 2|16|32] [--all-rates]"""
 from __future__ import annotations
 
 import argparse
@@ -144,8 +146,10 @@ def main():
     ap.add_argument("--ppm", type=float, default=0.0, help="per-frame crystal offset uniform in +-PPM at 868.1 MHz (0: none)")
     ap.add_argument("--soft", action="store_true", help="decode every capture with hard and with soft decisions, alternating, "
                     "at two more SNRs 1.5 and 3 dB below each SF's lowest point")
-    ap.add_argument("--osr", type=int, default=8, choices=(8, 2), help="fs/bw of the sensitivity curve; 2 also times the "
-                    "real-time shape at fs/bw = 8 against fs/bw = 2")
+    ap.add_argument("--osr", type=int, default=8, choices=(8, 2, 16, 32), help="fs/bw of the sensitivity curve; another "
+                    "than 8 also times the real-time shape at fs/bw = 8 against it")
+    ap.add_argument("--all-rates", action="store_true", help="time the real-time shape at fs/bw = 2, 8, 16 and 32, alternating "
+                    "(192 streams at 32, 384 below)")
     ap.add_argument("--cfo-range", type=float, nargs=2, metavar=("LO", "HI"), help="CFO uniform in +-[LO, HI] BW; decode with "
                     "and without wide_cfo, alternating")
     ap.add_argument("--max-cfo", type=float, default=None, help="max_cfo_hz of the wide_cfo decodes, in BW (default: HI)")
@@ -208,13 +212,14 @@ def main():
     res["sensitivity"] = curve
     # config-4 shape: 384 SF7 streams x 2 s, frames 3 dB above the sensitivity point; with --osr 2 the same frames at both
     # rates, the calls alternating between them
-    rates = [8, 2] if a.osr != 8 else [8]
-    sfx = (lambda d: f"_osr{d}") if a.osr != 8 else (lambda d: "")
+    rates = [2, 8, 16, 32] if a.all_rates else [8, a.osr] if a.osr != 8 else [8]
+    sfx = (lambda d: f"_osr{d}") if len(rates) > 1 else (lambda d: "")
+    n_str = {d: 192 if d == 32 else 384 for d in rates}       # about 12 GB of cf32 at fs/bw = 16 and 32
     shape = {}
     for d in rates:
         set_osr(d)
-        out, placed, n_items = capture(torch, 7, 384, 40, 1.0, seed=4, n_items=int(2 * FS), ppm=a.ppm)
-        rx = dec(7, False, n_streams=384, max_items_per_call=n_items, max_frames_per_call=64)
+        out, placed, n_items = capture(torch, 7, n_str[d], 40, 1.0, seed=4, n_items=int(2 * FS), ppm=a.ppm)
+        rx = dec(7, False, n_streams=n_str[d], max_items_per_call=n_items, max_frames_per_call=64)
         shape[d] = (out, placed, n_items, rx, FS)
         for m, kw in modes.items():
             runs = [stages(torch, rx, out, n_items, **kw) for _ in range(a.repeats)]
@@ -232,9 +237,9 @@ def main():
                 times[m, d].append(time.perf_counter() - t0)
                 med = float(np.median(times[m, d]))
                 res["realtime" + (m and "_" + m) + sfx(d)] = {
-                    "streams": 384, "seconds_per_stream": n_items / fs, "frames_placed": len(placed),
+                    "streams": n_str[d], "seconds_per_stream": n_items / fs, "frames_placed": len(placed),
                     "frames_decoded": decoded(frames, placed), "call_s_median": round(med, 4), "call_s_min": round(min(times[m, d]), 4),
-                    "call_s_max": round(max(times[m, d]), 4), "realtime_factor": round(384 * n_items / fs / med, 1)}
+                    "call_s_max": round(max(times[m, d]), 4), "realtime_factor": round(n_str[d] * n_items / fs / med, 1)}
     print(json.dumps(res))
 
 
